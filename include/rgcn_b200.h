@@ -345,6 +345,40 @@ int distmult_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel,
                   int64_t n, int side, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
                   int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * ComplEx triple scorer (decoders/complex.py).  Every row of width d is [real | imaginary] with h = d/2 columns
+ * each (extract_real_and_imaginary, :71-75); d % 4 == 0 is required (then h is even), other widths return
+ * RGCN_ERR_INVALID.  With a = codes[X[n,0]], b = rel[X[n,1]], c = codes[X[n,2]]:
+ *
+ *   energy[n] = sum_k ar*br*cr + ai*br*ci + ar*bi*ci - ai*bi*cr                 (:38-41)
+ *   loss_out[0] = mean_n( (1-y)x + log1p(exp(-|x|)) + max(-x,0) )               (:43-45, only if Y != NULL)
+ *   loss_out[1] = mean(a^2) + mean(b^2) + mean(c^2) over the gathered rows, all d columns  (:108-114, un-scaled;
+ *                 the caller multiplies by RegularizationParameter)
+ * Shapes, pointers and the backward's upstream gradients (g_loss, g_reg, g_scale_dev[2], g_energy[N]) are those of
+ * distmult_forward / distmult_backward.  The backward ACCUMULATES (+=) into dcodes [V,d] and drel [Vrel,d]
+ *   da = g [br cr + bi ci, br ci - bi cr],  db = g [ar cr + ai ci, ar ci - ai cr],  dc = g [ar br - ai bi, ai br + ar bi]
+ * plus 2*g_reg*x/(N*d) each, and, when rel_slice_sumsq != NULL, adds to that device float the sum over triples of
+ * |db|^2 (both halves): the relation table's IndexedSlices term of tf.clip_by_global_norm.
+ * ---------------------------------------------------------------------------------------------- */
+int rgcn_complex_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                         const int32_t* X, int64_t N, const float* Y, float* energies, float* loss_out,
+                         void* stream);
+int rgcn_complex_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                          const int32_t* X, int64_t N, const float* Y, const float* energies, float g_loss,
+                          float g_reg, const float* g_scale_dev, const float* g_energy, float* dcodes, float* drel,
+                          float* rel_slice_sumsq, void* stream);
+
+/* ComplEx all-entity scoring + ranking, fused: predict_all_subject_scores / predict_all_object_scores
+ * (complex.py:77-106) are one [n,d] x [d,V] product each, with the query rows
+ *   side 0 (subjects corrupted): q = [br cr + bi ci, br ci - bi cr]      (c = codes[o] kept, gold = s)
+ *   side 1 (objects corrupted):  q = [ar br - ai bi, ai br + ar bi]      (a = codes[s] kept, gold = o)
+ * and the same counting rules, known-mask format, split reuse and error codes as distmult_rank (workspace too
+ * small: RGCN_ERR_WORKSPACE). */
+int64_t rgcn_complex_rank_workspace_bytes(int32_t V, int32_t d, int64_t n);
+int rgcn_complex_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                      int64_t n, int side, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
+                      int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,6 +22,7 @@ EXPORTED_SYMBOLS = [
     "rgcn_basis_workspace_bytes", "rgcn_basis_forward", "rgcn_basis_backward",
     "distmult_forward", "distmult_backward", "distmult_rank_workspace_bytes", "distmult_rank",
     "distmult_backward_slices", "rgcn_block_slice_sumsq_workspace_bytes", "rgcn_block_slice_sumsq",
+    "rgcn_complex_forward", "rgcn_complex_backward", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_rank",
 ]
 
 RGCN_NORM_CANONICAL, RGCN_NORM_EXPLICIT, RGCN_NORM_NONE = 0, 1, 2
@@ -134,6 +135,16 @@ def _declare(lib):
     lib.distmult_backward.restype = c_int
     lib.distmult_backward.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, vp, vp,
                                       c_float, c_float, vp, vp, vp, vp, vp]
+    lib.rgcn_complex_forward.restype = c_int
+    lib.rgcn_complex_forward.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, vp, vp, vp, vp]
+    lib.rgcn_complex_backward.restype = c_int
+    lib.rgcn_complex_backward.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, vp, vp,
+                                          c_float, c_float, vp, vp, vp, vp, vp, vp]
+    lib.rgcn_complex_rank_workspace_bytes.restype = c_int64
+    lib.rgcn_complex_rank_workspace_bytes.argtypes = [c_int32, c_int32, c_int64]
+    lib.rgcn_complex_rank.restype = c_int
+    lib.rgcn_complex_rank.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, vp, c_int, vp, vp, vp,
+                                      c_int64, vp]
 
 
 def load():

@@ -1,9 +1,10 @@
 """Name= -> component chain factory (reference: common/model_builder.py:26-184, :273-319).
 
 Only the branches on the accelerated path are built: encoders `gcn_basis` (BasisGcn, or ConcatGcn
-when Concatenation=Yes) and `embedding`; decoder `bilinear-diag`.  Unknown names return None exactly
+when Concatenation=Yes) and `embedding`; decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag
+from ..decoders.complex import Complex
 from ..encoders.affine_transform import AffineTransform
 from ..encoders.message_gcns.gcn_basis import BasisGcn
 from ..encoders.message_gcns.gcn_basis_concat import ConcatGcn
@@ -63,4 +64,6 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
 def build_decoder(encoder, decoder_settings):
     if decoder_settings['Name'] == "bilinear-diag":
         return BilinearDiag(encoder, decoder_settings)
+    if decoder_settings['Name'] == "complex":
+        return Complex(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
     return None

@@ -853,6 +853,37 @@ extern "C" int rgcn_block_slice_sumsq(const rgcn_graph_t* g, int32_t d, int32_t 
 // ------------------------------------------------------------------------------------------------
 // DistMult all-entity scoring + ranking, fused (next row N3)
 // ------------------------------------------------------------------------------------------------
+// The decoder-independent body of distmult_rank / rgcn_complex_rank: hi/lo split of `codes` (unless reused), the
+// decoder's query rows + gold scores, the scoring GEMM with its rank-counting epilogue, raw/filtered ranks.
+// Workspace layout: [hi V*d | lo V*d | Q n*d | gold_sig n | gold_col n | raw_cnt n | known_cnt n].
+typedef int (*RankPrepareFn)(const float*, const float*, int, const int32_t*, int64_t, int, float*, float*, int32_t*,
+                             cudaStream_t);
+
+static int rank_with_queries(RankPrepareFn prepare, const float* codes, const float* rel, int32_t V, int32_t d,
+                             const int32_t* X, int64_t n, int side, const uint32_t* known_mask, int reuse_split,
+                             int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                             cudaStream_t st) {
+  Carver ws(workspace, workspace_bytes);
+  float* hi = ws.take<float>((int64_t)V * d);
+  float* lo = ws.take<float>((int64_t)V * d);
+  float* Q = ws.take<float>(n * d);
+  float* gold_sig = ws.take<float>(n);
+  int32_t* gold_col = ws.take<int32_t>(n);
+  int32_t* raw_cnt = ws.take<int32_t>(n);
+  int32_t* known_cnt = ws.take<int32_t>(n);
+  int rc = RGCN_OK;
+  if (!reuse_split) rc = launch_gemm_split_b(codes, d, V, d, /*transposed=*/0, hi, lo, st);
+  if (rc || n == 0) return rc;
+  rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
+  if (rc) return rc;
+  rc = prepare(codes, rel, d, X, n, side, Q, gold_sig, gold_col, st);
+  if (rc) return rc;
+  rc = launch_gemm_rank_tf32x3(Q, d, hi, lo, d, (int)n, V, d, gold_sig, gold_col, known_mask, (V + 31) / 32, raw_cnt,
+                               known_cnt, st);
+  if (rc) return rc;
+  return launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
+}
+
 extern "C" int64_t distmult_rank_workspace_bytes(int32_t V, int32_t d, int64_t n) {
   if (V <= 0 || d <= 0 || n < 0) {
     rgcn_set_error("distmult_rank_workspace_bytes: bad arguments");
@@ -874,24 +905,59 @@ extern "C" int distmult_rank(const float* codes, const float* rel, int32_t V, in
     rgcn_set_error("distmult_rank: workspace too small");
     return RGCN_ERR_WORKSPACE;
   }
-  cudaStream_t st = (cudaStream_t)stream;
-  Carver ws(workspace, workspace_bytes);
-  float* hi = ws.take<float>((int64_t)V * d);
-  float* lo = ws.take<float>((int64_t)V * d);
-  float* Q = ws.take<float>(n * d);
-  float* gold_sig = ws.take<float>(n);
-  int32_t* gold_col = ws.take<int32_t>(n);
-  int32_t* raw_cnt = ws.take<int32_t>(n);
-  int32_t* known_cnt = ws.take<int32_t>(n);
-  int rc = RGCN_OK;
-  if (!reuse_split) rc = launch_gemm_split_b(codes, d, V, d, /*transposed=*/0, hi, lo, st);
-  if (rc || n == 0) return rc;
-  rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
-  if (rc) return rc;
-  rc = launch_distmult_rank_prepare(codes, rel, d, X, n, side, Q, gold_sig, gold_col, st);
-  if (rc) return rc;
-  rc = launch_gemm_rank_tf32x3(Q, d, hi, lo, d, (int)n, V, d, gold_sig, gold_col, known_mask, (V + 31) / 32, raw_cnt,
-                               known_cnt, st);
-  if (rc) return rc;
-  return launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
+  return rank_with_queries(launch_distmult_rank_prepare, codes, rel, V, d, X, n, side, known_mask, reuse_split,
+                           raw_rank, filtered_rank, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------------
+// ComplEx (complex.cu): scorer, backward and fused all-entity ranking
+// ------------------------------------------------------------------------------------------------
+extern "C" int rgcn_complex_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                    const int32_t* X, int64_t N, const float* Y, float* energies, float* loss_out,
+                                    void* stream) {
+  if (!codes || !rel || (N > 0 && (!X || !energies)) || !loss_out || d <= 0 || d % 4 != 0 || V <= 0 ||
+      Vrel <= 0 || N < 0) {
+    rgcn_set_error("rgcn_complex_forward: bad arguments (need d % 4 == 0, non-null pointers)");
+    return RGCN_ERR_INVALID;
+  }
+  return launch_complex_forward(codes, rel, d, X, N, Y, energies, loss_out, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_complex_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                     const int32_t* X, int64_t N, const float* Y, const float* energies, float g_loss,
+                                     float g_reg, const float* g_scale_dev, const float* g_energy, float* dcodes,
+                                     float* drel, float* rel_slice_sumsq, void* stream) {
+  if (!codes || !rel || (N > 0 && !X) || !dcodes || !drel || d <= 0 || d % 4 != 0 || V <= 0 || Vrel <= 0 ||
+      N < 0 || (Y && !energies)) {
+    rgcn_set_error("rgcn_complex_backward: bad arguments (need d % 4 == 0, non-null pointers, energies with Y)");
+    return RGCN_ERR_INVALID;
+  }
+  return launch_complex_backward(codes, rel, d, X, N, Y, energies, g_loss, g_reg, g_scale_dev, g_energy, dcodes,
+                                 drel, rel_slice_sumsq, (cudaStream_t)stream);
+}
+
+extern "C" int64_t rgcn_complex_rank_workspace_bytes(int32_t V, int32_t d, int64_t n) {
+  if (V <= 0 || d <= 0 || d % 4 != 0 || n < 0) {
+    rgcn_set_error("rgcn_complex_rank_workspace_bytes: bad arguments (need d % 4 == 0)");
+    return RGCN_ERR_INVALID;
+  }
+  return distmult_rank_workspace_bytes(V, d, n);  // same layout (rank_with_queries)
+}
+
+extern "C" int rgcn_complex_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                 const int32_t* X, int64_t n, int side, const uint32_t* known_mask, int reuse_split,
+                                 int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                                 void* stream) {
+  if (!codes || !rel || (n > 0 && (!X || !raw_rank)) || !workspace || V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 ||
+      n < 0 || n > 0x7fffffffLL || (side != 0 && side != 1) || (filtered_rank && !known_mask)) {
+    rgcn_set_error("rgcn_complex_rank: bad arguments (need d % 4 == 0, side in {0,1}, a known mask when filtered "
+                   "ranks are requested)");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_complex_rank_workspace_bytes(V, d, n)) {
+    rgcn_set_error("rgcn_complex_rank: workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  return rank_with_queries(launch_complex_rank_prepare, codes, rel, V, d, X, n, side, known_mask, reuse_split,
+                           raw_rank, filtered_rank, workspace, workspace_bytes, (cudaStream_t)stream);
 }

@@ -121,3 +121,15 @@ int launch_distmult_backward(const float* codes, const float* rel, int d, const 
                              int64_t N, const float* Y, const float* energies, float g_loss,
                              float g_reg, const float* g_scale_dev, const float* g_energy,
                              float* dcodes, float* drel, float* rel_slice_sumsq, cudaStream_t st);
+
+// ComplEx (complex.cu): same contracts as the DistMult launchers above, rows split as [real | imaginary]
+int launch_complex_forward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                           float* energies, float* loss_out, cudaStream_t st);
+int launch_complex_backward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                            const float* energies, float g_loss, float g_reg, const float* g_scale_dev,
+                            const float* g_energy, float* dcodes, float* drel, float* rel_slice_sumsq,
+                            cudaStream_t st);
+// side 0: Q[t] = [rr e2r + ri e2i, rr e2i - ri e2r], gold = s;  side 1: Q[t] = [e1r rr - e1i ri, e1i rr + e1r ri],
+// gold = o.  gold_sig[t] = sigmoid(<Q[t], codes[gold]>)
+int launch_complex_rank_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
+                                float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);

@@ -43,9 +43,15 @@ class BilinearDiag(Model):
             Y = None
             if mode == 'train':
                 Y = torch.as_tensor(np.asarray(self.Y.value, dtype=np.float32), device=self.get_device())
-            self._scored[mode] = ops.distmult(subject_codes.contiguous(), relation_codes.contiguous(),
-                                              self._x_device(), Y)
+            self._scored[mode] = self._score_op()(subject_codes.contiguous(), relation_codes.contiguous(),
+                                                  self._x_device(), Y)
         return self._scored[mode]
+
+    def _score_op(self):
+        return ops.distmult
+
+    def _ranker(self, codes, rel):
+        return ops.DistMultRanker(codes, rel)
 
     def compute_codes(self, mode='train'):
         """(e1s, rs, e2s) row gathers (bilinear_diag.py:14-24) -- only the all-entity scoring GEMMs
@@ -97,7 +103,7 @@ class BilinearDiag(Model):
         subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='test')
         assert subject_codes is object_codes, "DistMult ranking expects one shared entity code matrix"
         codes, rel = subject_codes.contiguous(), relation_codes.contiguous()
-        ranker = ops.DistMultRanker(codes, rel)
+        ranker = self._ranker(codes, rel)
         V = codes.shape[0]
         tri = np.ascontiguousarray(np.asarray(triplets, dtype=np.int32).reshape(-1, 3))
         out = [[], [], [], []]

@@ -315,64 +315,91 @@ def basis_layer(H, W_forward, W_backward, C_forward, C_backward, W_self, graph, 
                                drop_mask, keep, relu)
 
 
+def _triple_forward(ctx, entry, codes, rel, X, Y):
+    """Forward of a triple scorer entry point with the distmult_forward argument list."""
+    lib = _lib.load()
+    _check_cuda_f32("codes", codes)
+    _check_cuda_f32("relation table", rel)
+    if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2
+            and X.shape[1] == 3):
+        raise _lib.RgcnError("X must be a contiguous CUDA int32 [N,3] tensor")
+    if Y is not None:
+        _check_cuda_f32("Y", Y, (X.shape[0],))
+    V, d = codes.shape
+    dev = codes.device
+    N = X.shape[0]
+    energies = torch.empty(N, dtype=torch.float32, device=dev)
+    loss2 = torch.empty(2, dtype=torch.float32, device=dev)
+    rc = getattr(lib, entry)(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, _ptr(Y),
+                             _ptr(energies), _ptr(loss2), _stream(dev))
+    _lib.check(rc, entry)
+    ctx.has_y = Y is not None
+    ctx.rel_param = rel
+    ctx.save_for_backward(codes, rel, X, Y if Y is not None else torch.empty(0, device=dev),
+                          energies)
+    return energies, loss2[0], loss2[1]
+
+
+def _triple_backward(ctx, entry, g_energy, g_loss, g_reg):
+    """Backward of a triple scorer entry point with the distmult_backward_slices argument list."""
+    lib = _lib.load()
+    codes, rel, X, Y, energies = ctx.saved_tensors
+    Y = Y if ctx.has_y else None
+    V, d = codes.shape
+    dev = codes.device
+    dcodes = torch.zeros_like(codes)
+    drel = torch.zeros_like(rel)
+    ge = None
+    if g_energy is not None:
+        ge = g_energy.contiguous()
+    # upstream scalar gradients stay on the device (no host sync): passed as g_scale_dev[2]
+    gs = torch.zeros(2, dtype=torch.float32, device=dev)
+    if g_loss is not None:
+        gs[0] = g_loss
+    if g_reg is not None:
+        gs[1] = g_reg
+    ss = torch.zeros(1, dtype=torch.float32, device=dev) if _SLICE_NORMS else None
+    rc = getattr(lib, entry)(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), X.shape[0],
+                             _ptr(Y), _ptr(energies), 1.0, 1.0, _ptr(gs), _ptr(ge),
+                             _ptr(dcodes), _ptr(drel), _ptr(ss), _stream(dev))
+    _lib.check(rc, entry)
+    if ss is not None:
+        _add_slice_sumsq(ctx.rel_param, ss[0])
+    return dcodes, drel, None, None
+
+
 class _DistMultFn(torch.autograd.Function):
     """Returns (energies[N], loss, reg): loss = mean sigmoid-CE (0 if Y is None), reg = un-scaled L2."""
 
     @staticmethod
     def forward(ctx, codes, rel, X, Y):
-        lib = _lib.load()
-        _check_cuda_f32("codes", codes)
-        _check_cuda_f32("relation table", rel)
-        if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2
-                and X.shape[1] == 3):
-            raise _lib.RgcnError("X must be a contiguous CUDA int32 [N,3] tensor")
-        if Y is not None:
-            _check_cuda_f32("Y", Y, (X.shape[0],))
-        V, d = codes.shape
-        dev = codes.device
-        N = X.shape[0]
-        energies = torch.empty(N, dtype=torch.float32, device=dev)
-        loss2 = torch.empty(2, dtype=torch.float32, device=dev)
-        rc = lib.distmult_forward(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, _ptr(Y),
-                                  _ptr(energies), _ptr(loss2), _stream(dev))
-        _lib.check(rc, "distmult_forward")
-        ctx.has_y = Y is not None
-        ctx.rel_param = rel
-        ctx.save_for_backward(codes, rel, X, Y if Y is not None else torch.empty(0, device=dev),
-                              energies)
-        return energies, loss2[0], loss2[1]
+        return _triple_forward(ctx, "distmult_forward", codes, rel, X, Y)
 
     @staticmethod
     def backward(ctx, g_energy, g_loss, g_reg):
-        lib = _lib.load()
-        codes, rel, X, Y, energies = ctx.saved_tensors
-        Y = Y if ctx.has_y else None
-        V, d = codes.shape
-        dev = codes.device
-        dcodes = torch.zeros_like(codes)
-        drel = torch.zeros_like(rel)
-        ge = None
-        if g_energy is not None:
-            ge = g_energy.contiguous()
-        # upstream scalar gradients stay on the device (no host sync): passed as g_scale_dev[2]
-        gs = torch.zeros(2, dtype=torch.float32, device=dev)
-        if g_loss is not None:
-            gs[0] = g_loss
-        if g_reg is not None:
-            gs[1] = g_reg
-        ss = torch.zeros(1, dtype=torch.float32, device=dev) if _SLICE_NORMS else None
-        rc = lib.distmult_backward_slices(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), X.shape[0],
-                                          _ptr(Y), _ptr(energies), 1.0, 1.0, _ptr(gs), _ptr(ge),
-                                          _ptr(dcodes), _ptr(drel), _ptr(ss), _stream(dev))
-        _lib.check(rc, "distmult_backward_slices")
-        if ss is not None:
-            _add_slice_sumsq(ctx.rel_param, ss[0])
-        return dcodes, drel, None, None
+        return _triple_backward(ctx, "distmult_backward_slices", g_energy, g_loss, g_reg)
 
 
 def distmult(codes, rel, X, Y=None):
     """DistMult energies + sigmoid cross-entropy + L2 term (bilinear_diag.py:14-34,63-69)."""
     return _DistMultFn.apply(codes, rel, X, Y)
+
+
+class _ComplexFn(torch.autograd.Function):
+    """Returns (energies[N], loss, reg) of the ComplEx scorer, same conventions as _DistMultFn."""
+
+    @staticmethod
+    def forward(ctx, codes, rel, X, Y):
+        return _triple_forward(ctx, "rgcn_complex_forward", codes, rel, X, Y)
+
+    @staticmethod
+    def backward(ctx, g_energy, g_loss, g_reg):
+        return _triple_backward(ctx, "rgcn_complex_backward", g_energy, g_loss, g_reg)
+
+
+def complex_score(codes, rel, X, Y=None):
+    """ComplEx energies + sigmoid cross-entropy + L2 term (complex.py:31-45,108-114); rows are [real | imaginary]."""
+    return _ComplexFn.apply(codes, rel, X, Y)
 
 
 def gemm_tf32x3(A, B, b_is_nk=False, out=None, accumulate=False):
@@ -479,6 +506,7 @@ def block_aggregate_backward(X, W_forward, W_backward, G, graph, n_blocks, dWf=N
 class DistMultRanker(object):
     """Fused all-entity scoring + ranking over one entity code matrix (distmult_rank, include/rgcn_b200.h): the
     hi/lo split of `codes` is made once and reused by every chunk / corruption side."""
+    _RANK, _WORKSPACE = "distmult_rank", "distmult_rank_workspace_bytes"
 
     def __init__(self, codes, rel):
         _check_cuda_f32("codes", codes)
@@ -500,15 +528,21 @@ class DistMultRanker(object):
             raise _lib.RgcnError("known_mask must be a contiguous CUDA int32 [n, ceil(V/32)] tensor (bit masks)")
         dev = self.codes.device
         if self._ws is None or n > self._ws_n:
-            nb = lib.distmult_rank_workspace_bytes(V, d, n)
+            nb = getattr(lib, self._WORKSPACE)(V, d, n)
             if nb < 0:
-                _lib.check(int(nb), "distmult_rank_workspace_bytes")
+                _lib.check(int(nb), self._WORKSPACE)
             self._ws, self._ws_n, self._split_ready = _workspace(nb, dev), n, False
         raw = torch.empty(n, dtype=torch.int32, device=dev)
         filt = torch.empty(n, dtype=torch.int32, device=dev) if known_mask is not None else None
-        rc = lib.distmult_rank(_ptr(self.codes), _ptr(self.rel), V, self.rel.shape[0], d, _ptr(X), n, int(side),
-                               _ptr(known_mask), int(self._split_ready), _ptr(raw), _ptr(filt), _ptr(self._ws),
-                               self._ws.numel(), _stream(dev))
-        _lib.check(rc, "distmult_rank")
+        rc = getattr(lib, self._RANK)(_ptr(self.codes), _ptr(self.rel), V, self.rel.shape[0], d, _ptr(X), n,
+                                      int(side), _ptr(known_mask), int(self._split_ready), _ptr(raw), _ptr(filt),
+                                      _ptr(self._ws), self._ws.numel(), _stream(dev))
+        _lib.check(rc, self._RANK)
         self._split_ready = True
         return raw, filt
+
+
+class ComplexRanker(DistMultRanker):
+    """Fused all-entity scoring + ranking of the ComplEx decoder (rgcn_complex_rank): same interface and split reuse
+    as DistMultRanker, the query rows are the complex products of complex.py:77-106."""
+    _RANK, _WORKSPACE = "rgcn_complex_rank", "rgcn_complex_rank_workspace_bytes"

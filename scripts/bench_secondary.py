@@ -1,6 +1,8 @@
-"""Secondary measurements (not the headline bench): DistMult scorer fwd/bwd bandwidth, basis layer
+"""Secondary measurements (not the headline bench): DistMult and ComplEx scorer fwd/bwd bandwidth and fused
+ranking, basis layer
 (WN18 shape, BASELINE configs[2]; shipped gcn_basis.exp shape), block layer train-step graph."""
 import json
+import subprocess
 import sys
 import time
 
@@ -73,6 +75,47 @@ out["distmult_hbm"] = {"V": V2, "N": N2, "d": 512, "fwd_ms": t2, "fwd_GBps_algor
                        "frac_of_measured_hbm_6569.6": N2 * (8 * 512 + 16) / t2 / 1e6 / 6569.6,
                        "note": "2 of the 3 rows per triple come from HBM (entity table 2 GB), the relation row from L2"}
 del codes2, rel2, X2, Y2
+
+
+# ---- ComplEx at the same shape (complex.exp: d = 500, so the imaginary half is 8-byte aligned: float2 path) ----
+def cx_fwd():
+    with torch.no_grad():
+        ops.complex_score(codes, rel, X, Y)
+
+
+def cx_fwd_bwd():
+    codes.grad = None
+    rel.grad = None
+    e, l, r = ops.complex_score(codes, rel, X, Y)
+    (l + 0.01 * r).backward()
+
+
+# fused ranking of the FB15k-237 test set (20466 triples) under both corruptions, one split for all chunks
+n_rank = 20466
+X_rank = torch.stack([torch.randint(0, V, (n_rank,), device=dev, generator=g),
+                      torch.randint(0, 237, (n_rank,), device=dev, generator=g),
+                      torch.randint(0, V, (n_rank,), device=dev, generator=g)], 1).int().contiguous()
+codes_d, rel_d = codes.detach(), rel.detach()
+
+
+def rank_all(ranker_cls, chunk=4096):
+    ranker = ranker_cls(codes_d, rel_d)
+    for c0 in range(0, n_rank, chunk):
+        for side in (0, 1):
+            ranker.rank(X_rank[c0:c0 + chunk], side, None)
+
+
+# the two decoders alternate in one run so that both see the same card state
+t_dm_f, t_dm_fb, t_cx_f, t_cx_fb = timeit(dm_fwd), timeit(dm_fwd_bwd), timeit(cx_fwd), timeit(cx_fwd_bwd)
+t_dm_r, t_cx_r = timeit(lambda: rank_all(ops.DistMultRanker), n=5), timeit(lambda: rank_all(ops.ComplexRanker), n=5)
+gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                     capture_output=True, text=True).stdout.strip()
+out["complex"] = {"N": N, "d": d, "V": V, "gpu": gpu, "fwd_ms": t_cx_f, "fwd_bwd_ms": t_cx_fb,
+                  "fwd_GBps_algorithmic": alg_f / t_cx_f / 1e6,
+                  "bwd_GBps_algorithmic": alg_b / max(t_cx_fb - t_cx_f, 1e-6) / 1e6,
+                  "rank_triples": n_rank, "rank_both_sides_ms": t_cx_r,
+                  "distmult_same_run": {"fwd_ms": t_dm_f, "fwd_bwd_ms": t_dm_fb, "rank_both_sides_ms": t_dm_r},
+                  "ratio_to_distmult": {"fwd": t_cx_f / t_dm_f, "fwd_bwd": t_cx_fb / t_dm_fb, "rank": t_cx_r / t_dm_r}}
 
 
 # ---- layers ----
