@@ -284,6 +284,32 @@ int rgcn_basis_backward(const rgcn_graph_t* g, int32_t d, int32_t B, const float
                         void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * One-hot (featureless) basis layer: layer 0 of the gcn_basis encoder with UseInputTransform=No
+ * (model_builder.py:140-168, :277-283: Representation -> BasisGcn(onehot_input=True)).  With one-hot input
+ * dot_or_lookup is an embedding lookup (shared_functions.py:5-9, gcn_basis.py:15-71, message_gcn.py:28-79):
+ *
+ *   out[v] = act( sum_dir sum_{m -> v} norm_m sum_b C_dir[r_m,b] W_dir[u_m,b,:]  +  dropout(W_self[v]) )
+ *
+ * Wf, Wb : [V_src, B, d] (vertex_feature_dimension = EntityCount);  Cf, Cb : [R, B];  Wself : [V_dst, d].
+ * Backward:  G = dOut * relu'(out),  dW_dir[u,b,:] = sum_{m from u} norm_m C_dir[r_m,b] G[v_m,:],
+ *            dC_dir[r,b] = sum_{m: r_m = r} norm_m < W_dir[u_m,b,:], G[v_m,:] >,  dWself = G * mask / keep.
+ * The layer has no input, hence no input gradient.  Every dW row is written (rows without messages are zero).
+ * Both calls walk the source-major CSR view: a graph prepared with graph_views = 2 is rejected (RGCN_ERR_INVALID).
+ * Argument rules as rgcn_basis_*: d % 4 == 0, B >= 1, keep > 0, drop_mask uint8 [V_dst, d] or NULL.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_basis_onehot_workspace_bytes(const rgcn_graph_t* g, int32_t d, int32_t B, int backward);
+
+int rgcn_basis_onehot_forward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* Wf, const float* Wb,
+                              const float* Cf, const float* Cb, const float* Wself, const uint8_t* drop_mask,
+                              float keep, int relu, float* out, void* workspace, int64_t workspace_bytes,
+                              void* stream);
+
+int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* Wf, const float* Wb,
+                               const float* Cf, const float* Cb, const uint8_t* drop_mask, float keep, int relu,
+                               const float* out, const float* dOut, float* dWf, float* dWb, float* dCf,
+                               float* dCb, float* dWself, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * DistMult triple scorer ("BilinearDiag", decoders/bilinear_diag.py:14-34, :63-69).
  *
  *   energy[n] = sum_k codes[X[n,0],k] * rel[X[n,1],k] * codes[X[n,2],k]

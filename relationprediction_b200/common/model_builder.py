@@ -1,7 +1,7 @@
 """Name= -> component chain factory (reference: common/model_builder.py:26-184, :273-319).
 
 Only the branches on the accelerated path are built: encoders `gcn_basis` (BasisGcn, or ConcatGcn
-when Concatenation=Yes) and `embedding`; decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
+when Concatenation=Yes; with UseInputTransform=No layer 0 is a one-hot BasisGcn) and `embedding`; decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag
 from ..decoders.complex import Complex
@@ -33,11 +33,14 @@ def build_encoder(encoder_settings, triples):
         relation_shape = [int(encoder_settings['EntityCount']), int(encoder_settings['CodeDimension'])]
         layers = int(encoder_settings['NumberOfLayers'])
 
-        if _flag(encoder_settings, 'UseInputTransform') != "Yes":
-            raise NotImplementedError("UseInputTransform=No / RandomInput / PartiallyRandomInput variants are "
-                                      "outside the accelerated path (SURVEY.md 2.1 #6)")
-        encoding = AffineTransform(input_shape, encoder_settings, next_component=graph, onehot_input=True,
-                                   use_bias=True, use_nonlinearity=True)
+        if _flag(encoder_settings, 'UseInputTransform') == "Yes":
+            encoding = AffineTransform(input_shape, encoder_settings, next_component=graph, onehot_input=True,
+                                       use_bias=True, use_nonlinearity=True)
+        elif _flag(encoder_settings, 'RandomInput') == "Yes" or _flag(encoder_settings, 'PartiallyRandomInput') == "Yes":
+            raise NotImplementedError("RandomInput / PartiallyRandomInput variants are outside the accelerated path "
+                                      "(SURVEY.md 2.1 #6)")
+        else:
+            encoding = graph   # featureless: layer 0 reads one-hot entity input (model_builder.py:166-167)
         encoding = apply_basis_gcn(encoder_settings, encoding, internal_shape, layers)
         if _flag(encoder_settings, 'UseOutputTransform') == "Yes":
             encoding = AffineTransform(projection_shape, encoder_settings, next_component=encoding,
@@ -56,7 +59,11 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
     model = ConcatGcn if _flag(encoder_settings, 'Concatenation') == "Yes" else BasisGcn
     for layer in range(layers):
         use_nonlinearity = layer < layers - 1  # the last layer is linear (model_builder.py:275)
-        encoding = model(internal_shape, encoder_settings, next_component=encoding, onehot_input=False,
+        # only layer 0 of a featureless encoder reads one-hot input (model_builder.py:277-283)
+        onehot_input = (layer == 0 and _flag(encoder_settings, 'UseInputTransform') == "No"
+                        and _flag(encoder_settings, 'RandomInput') == "No"
+                        and _flag(encoder_settings, 'PartiallyRandomInput') == "No")
+        encoding = model(internal_shape, encoder_settings, next_component=encoding, onehot_input=onehot_input,
                          use_nonlinearity=use_nonlinearity)
     return encoding
 

@@ -769,6 +769,134 @@ extern "C" int rgcn_basis_backward(const rgcn_graph_t* g, int32_t d, int32_t B, 
 }
 
 // ------------------------------------------------------------------------------------------------
+// One-hot (featureless) basis layer: layer 0 of gcn_basis with UseInputTransform=No
+// ------------------------------------------------------------------------------------------------
+extern "C" int64_t rgcn_basis_onehot_workspace_bytes(const rgcn_graph_t* g, int32_t d, int32_t B, int backward) {
+  if (!g || d <= 0 || B <= 0) {
+    rgcn_set_error("rgcn_basis_onehot_workspace_bytes: bad arguments");
+    return RGCN_ERR_INVALID;
+  }
+  int64_t bytes = align_up((int64_t)g->n_relw * B * 4);  // concatenated coefficient table
+  if (backward) {
+    bytes += align_up((int64_t)g->n_relw * B * 4);       // dC (concatenated)
+    bytes += align_up((int64_t)g->V_dst * d * 4);        // G (used when a dropout mask is given)
+  }
+  return bytes + 256;
+}
+
+// argument validation runs before anything touches the device: bad shapes, null pointers and short workspaces are
+// RGCN_ERR_INVALID / RGCN_ERR_WORKSPACE even for a host-only graph
+static int onehot_shape_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
+  if (!g || d <= 0 || d % 4 != 0 || B <= 0) {
+    rgcn_set_error(std::string(who) + ": need a graph, d > 0, d % 4 == 0, B > 0");
+    return RGCN_ERR_INVALID;
+  }
+  return RGCN_OK;
+}
+
+static int onehot_graph_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
+  int rc = layer_checks(g, d, B, who);
+  if (rc) return rc;
+  return need_views(g, true, false, who);
+}
+
+static int concat_coefficients(const float* Cf, const float* Cb, int R, int B, float* Ccat, cudaStream_t st) {
+  int rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat, Cf, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy Cf");
+  if (!rc) rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat + (size_t)R * B, Cb, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy Cb");
+  return rc;
+}
+
+extern "C" int rgcn_basis_onehot_forward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* Wf,
+                                         const float* Wb, const float* Cf, const float* Cb, const float* Wself,
+                                         const uint8_t* drop_mask, float keep, int relu, float* out, void* workspace,
+                                         int64_t workspace_bytes, void* stream) {
+  int rc = onehot_shape_checks(g, d, B, "rgcn_basis_onehot_forward");
+  if (rc) return rc;
+  if (!Wf || !Wb || !Cf || !Cb || !Wself || !out || !workspace || keep <= 0.f) {
+    rgcn_set_error("rgcn_basis_onehot_forward: null pointer or keep <= 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_basis_onehot_workspace_bytes(g, d, B, 0)) {
+    rgcn_set_error("rgcn_basis_onehot_forward: workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onehot_graph_checks(g, d, B, "rgcn_basis_onehot_forward");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
+  if (rc) return rc;
+  const int R = g->n_relw / 2;
+  const int64_t n = (int64_t)g->V_dst * d;
+  Carver ws(workspace, workspace_bytes);
+  float* Ccat = ws.take<float>((int64_t)g->n_relw * B);
+  rc = concat_coefficients(Cf, Cb, R, B, Ccat, st);
+  if (rc) return rc;
+  MARK("start");
+  // out = dropout(W_self)  (the self loop looks up W_self with tf.range(V): message_gcn.py:56, gcn_basis.py:70-71)
+  rc = rgcn_check_cuda(cudaMemcpyAsync(out, Wself, (size_t)n * 4, cudaMemcpyDeviceToDevice, st), "copy W_self");
+  if (!rc) rc = launch_mask_relu(out, drop_mask, 1.0f / keep, 0, n, st);
+  if (rc) return rc;
+  MARK("onehot_self_loop");
+  // out[dst] += norm * sum_b C[relw,b] W_dir[src,b,:]
+  rc = launch_basis_onehot_push(g->by_src.d_items, (int)g->by_src.n_items, g->by_src.d_nbr, g->by_src.d_relw,
+                                g->by_src.d_norm, Wf, Wb, Ccat, B, d, g->n_relw, out, st);
+  if (rc) return rc;
+  MARK("onehot_push_fwd");
+  rc = launch_mask_relu(out, nullptr, 1.f, relu, n, st);
+  MARK("relu_epilogue");
+  return rc;
+}
+
+extern "C" int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* Wf,
+                                          const float* Wb, const float* Cf, const float* Cb,
+                                          const uint8_t* drop_mask, float keep, int relu, const float* out,
+                                          const float* dOut, float* dWf, float* dWb, float* dCf, float* dCb,
+                                          float* dWself, void* workspace, int64_t workspace_bytes, void* stream) {
+  int rc = onehot_shape_checks(g, d, B, "rgcn_basis_onehot_backward");
+  if (rc) return rc;
+  if (!Wf || !Wb || !Cf || !Cb || !dOut || !dWf || !dWb || !dCf || !dCb || !dWself || !workspace ||
+      (relu && !out) || keep <= 0.f) {
+    rgcn_set_error("rgcn_basis_onehot_backward: null pointer or keep <= 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_basis_onehot_workspace_bytes(g, d, B, 1)) {
+    rgcn_set_error("rgcn_basis_onehot_backward: workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onehot_graph_checks(g, d, B, "rgcn_basis_onehot_backward");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
+  if (rc) return rc;
+  const int R = g->n_relw / 2;
+  const int64_t dB = (int64_t)d * B;
+  Carver ws(workspace, workspace_bytes);
+  float* Ccat = ws.take<float>((int64_t)g->n_relw * B);
+  float* dCcat = ws.take<float>((int64_t)g->n_relw * B);
+  float* G = ws.take<float>((int64_t)g->V_dst * d);
+  rc = concat_coefficients(Cf, Cb, R, B, Ccat, st);
+  if (rc) return rc;
+  MARK("start");
+  // G = dOut * relu'(out);  dW_self = G * mask / keep (without a mask dW_self IS G: written once, read in place)
+  if (!drop_mask) G = dWself;
+  rc = launch_grad_prologue(dOut, out, drop_mask, 1.0f / keep, relu, (int64_t)g->V_dst * d, G, dWself, st);
+  if (rc) return rc;
+  MARK("grad_prologue");
+  // dW_dir[u] = sum_{m from u} norm C[relw] (x) G[dst];  dC[relw] += < W_dir[u], sum_run norm G[dst] >
+  rc = rgcn_check_cuda(cudaMemsetAsync(dCcat, 0, (size_t)g->n_relw * B * 4, st), "memset(dC)");
+  if (!rc) rc = launch_zero_rows(dWf, dB, g->by_src.d_split_rows, (int)g->by_src.n_split, st);
+  if (!rc) rc = launch_zero_rows(dWb, dB, g->by_src.d_split_rows, (int)g->by_src.n_split, st);
+  if (rc) return rc;
+  AggLaunch a = make_agg(g->by_src, G, d, d, nullptr, nullptr);
+  rc = launch_basis_agg_dc(a, Ccat, B, g->n_relw, Wf, Wb, dWf, dWb, dCcat, st);
+  if (rc) return rc;
+  MARK("onehot_agg_dW_dC");
+  rc = rgcn_check_cuda(cudaMemcpyAsync(dCf, dCcat, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy dCf");
+  if (!rc) rc = rgcn_check_cuda(cudaMemcpyAsync(dCb, dCcat + (size_t)R * B, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy dCb");
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------
 // DistMult
 // ------------------------------------------------------------------------------------------------
 extern "C" int distmult_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel,

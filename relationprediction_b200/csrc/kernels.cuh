@@ -69,6 +69,19 @@ int launch_block_unlayout(const float* dWt, int R, int B, int s, float* dWf, flo
 int launch_basis_agg(const AggLaunch& a, const float* C, int B, int n_relw, int layout, float* Agg,
                      cudaStream_t st);
 
+// One-hot basis layer backward (source major, X = G): the planar basis aggregation written straight into the two
+// [V_src][B][d] weight-gradient tables, dW_dir[u][b][:] = sum_{m: src_m = u, dir} norm_m C[relw_m,b] G[dst_m,:],
+// fused with dC[w][b] += sum_{m: relw_m = w} norm_m < W_dir[src_m][b][:], G[dst_m,:] > (dC zeroed by the caller).
+// Rows without messages in a direction are written as zeros; split rows must be zeroed first.
+int launch_basis_agg_dc(const AggLaunch& a, const float* C, int B, int n_relw, const float* W0, const float* W1,
+                        float* dW0, float* dW1, float* dC, cudaStream_t st);
+
+// basis_onehot.cu -- one-hot basis layer forward (push over the source-major view; `out` holds the self-loop term):
+//   out[dst_m,:] += norm_m * sum_b C[relw_m,b] W_dir[src_m][b][:]     (W_dir = Wf for relw < n_relw/2, else Wb)
+int launch_basis_onehot_push(const WorkItem* items, int n_items, const int32_t* nbr, const int32_t* relw,
+                             const float* norm, const float* Wf, const float* Wb, const float* C, int B, int d,
+                             int n_relw, float* out, cudaStream_t st);
+
 // Basis coefficient gradient (destination major):
 //   dC[w][b] += sum_{m into row, relw_m = w} norm_m * < H[src_m,:], dAgg[row][dir][:, b] >
 int launch_basis_dc(const AggLaunch& a, const float* dAgg, int B, int n_relw, float* dC,

@@ -722,11 +722,17 @@ __global__ void k_block_unlayout(const float* __restrict__ dWt, int R, int B, in
 }
 
 // ------------------------------------------------------------------------------------------------
-// Basis aggregation:  Agg[row][dir][k,b] = sum_m norm_m * C[relw_m, b] * X[nbr_m, k]
+// Basis aggregation:  Agg_dir[row][k,b] = sum_m norm_m * C[relw_m, b] * X[nbr_m, k]
+// The two directions' rows live at Agg0 / Agg1 + row * row_stride (one interleaved [V][2][d*B] array, or two
+// separate [V][B][d] weight-gradient tables of the one-hot layer).
+// DC (one-hot layer backward, LAYOUT 1, rows = sources, X = G): each run's pre-sum S = sum norm_m X[nbr_m] also
+// yields the coefficient gradient dC[relw][b] += < W_dir[row][b][:], S > (W0 / W1 = the [V][B][d] tables).
 // ------------------------------------------------------------------------------------------------
-template <int BC, int NV, int LAYOUT>
+template <int BC, int NV, int LAYOUT, bool DC>
 __global__ void __launch_bounds__(RGCN_THREADS, 1)
-    k_basis_agg(AggLaunch a, const float* __restrict__ C, int B, int half, float* __restrict__ Agg) {
+    k_basis_agg(AggLaunch a, const float* __restrict__ C, int B, int half, float* __restrict__ Agg0,
+                float* __restrict__ Agg1, int64_t row_stride, const float* __restrict__ W0,
+                const float* __restrict__ W1, float* __restrict__ dC) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int item = blockIdx.x * RGCN_WARPS_PER_BLOCK + warp;
   if (item >= a.n_items) return;
@@ -735,7 +741,6 @@ __global__ void __launch_bounds__(RGCN_THREADS, 1)
   const int4 itv = __ldg(reinterpret_cast<const int4*>(a.items) + item);
   const int beg = itv.x, end = itv.y, row = itv.z, split = itv.w;
   const size_t dB = (size_t)d * B;
-  float* arow = Agg + (size_t)row * 2 * dB;
 
   for (int b0 = 0; b0 < B; b0 += BC) {
     float4 acc[BC][NV], xs[NV];
@@ -748,7 +753,7 @@ __global__ void __launch_bounds__(RGCN_THREADS, 1)
     int cur = -1, curdir = -1, written = 0;
 
     auto write_out = [&](int dir) {
-      float* ad = arow + (size_t)dir * dB;
+      float* ad = DC ? (dir ? Agg1 : Agg0) + (size_t)row * row_stride : Agg0 + (size_t)row * 2 * dB + (size_t)dir * dB;
 #pragma unroll
       for (int b = 0; b < BC; ++b) {
         if (b0 + b < B) {
@@ -797,6 +802,28 @@ __global__ void __launch_bounds__(RGCN_THREADS, 1)
         const float cb = (b0 + b < B) ? __ldg(C + (size_t)w * B + b0 + b) : 0.f;
 #pragma unroll
         for (int k = 0; k < NV; ++k) fma4(acc[b][k], cb, xs[k]);
+      }
+      if (DC) {
+        const float* wr = (dir ? W1 : W0) + (size_t)row * dB;
+#pragma unroll 1
+        for (int b = 0; b < BC; ++b) {  // not unrolled: one basis' table quads live at a time
+          if (b0 + b < B) {
+            float p = 0.f;
+#pragma unroll
+            for (int k = 0; k < NV; ++k) {
+              const int col = c0 + 4 * (lane + 32 * k);
+              if (col < d) {
+                const float4 wv = ldg4(wr + (size_t)(b0 + b) * d + col);
+                p = fmaf(xs[k].x, wv.x, p);
+                p = fmaf(xs[k].y, wv.y, p);
+                p = fmaf(xs[k].z, wv.z, p);
+                p = fmaf(xs[k].w, wv.w, p);
+              }
+            }
+            p = warp_sum(p);
+            if (lane == 0) atomicAdd(dC + (size_t)w * B + b0 + b, p);
+          }
+        }
       }
     };
 
@@ -1258,39 +1285,53 @@ int launch_block_unlayout(const float* dWt, int R, int B, int s, float* dWf, flo
   return check_launch("k_block_unlayout");
 }
 
-template <int BC, int LAYOUT>
-static int launch_basis_agg_t(const AggLaunch& a, const float* C, int B, int n_relw, float* Agg,
-                              cudaStream_t st) {
-  const int nv = pick_nv(a.d);
+template <int BC, int LAYOUT, bool DC>
+static int launch_basis_agg_t(const AggLaunch& a, const float* C, int B, int n_relw, float* Agg0, float* Agg1,
+                              int64_t row_stride, const float* W0, const float* W1, float* dC, cudaStream_t st) {
+  // the fused dC variant works on column slabs of at most 256 (the coefficient accumulators of up to 5 bases and
+  // the rows in flight then fit the register file); slabs split the columns, not the gathered bytes
+  const int nv = DC ? std::min(pick_nv(a.d), 2) : pick_nv(a.d);
   const int slabs = (a.d + nv * 128 - 1) / (nv * 128);
   dim3 grid((a.n_items + RGCN_WARPS_PER_BLOCK - 1) / RGCN_WARPS_PER_BLOCK, slabs);
   const int half = n_relw / 2;
-  switch (nv) {
-    case 1: k_basis_agg<BC, 1, LAYOUT><<<grid, RGCN_THREADS, 0, st>>>(a, C, B, half, Agg); break;
-    case 2: k_basis_agg<BC, 2, LAYOUT><<<grid, RGCN_THREADS, 0, st>>>(a, C, B, half, Agg); break;
-    case 3: k_basis_agg<BC, 3, LAYOUT><<<grid, RGCN_THREADS, 0, st>>>(a, C, B, half, Agg); break;
-    default: k_basis_agg<BC, 4, LAYOUT><<<grid, RGCN_THREADS, 0, st>>>(a, C, B, half, Agg); break;
+#define BA(NV_) \
+  k_basis_agg<BC, NV_, LAYOUT, DC><<<grid, RGCN_THREADS, 0, st>>>(a, C, B, half, Agg0, Agg1, row_stride, W0, W1, dC)
+  if constexpr (DC) {
+    if (nv == 1) BA(1); else BA(2);
+  } else {
+    switch (nv) {
+      case 1: BA(1); break;
+      case 2: BA(2); break;
+      case 3: BA(3); break;
+      default: BA(4); break;
+    }
   }
+#undef BA
   return check_launch("k_basis_agg");
+}
+
+// bases per pass: all of them when they fit the register budget, else passes of 4
+template <int LAYOUT, bool DC>
+static int launch_basis_agg_b(const AggLaunch& a, const float* C, int B, int n_relw, float* Agg0, float* Agg1,
+                              int64_t row_stride, const float* W0, const float* W1, float* dC, cudaStream_t st) {
+  if (a.n_items == 0) return RGCN_OK;
+  if (B == 1) return launch_basis_agg_t<1, LAYOUT, DC>(a, C, B, n_relw, Agg0, Agg1, row_stride, W0, W1, dC, st);
+  if (B == 2) return launch_basis_agg_t<2, LAYOUT, DC>(a, C, B, n_relw, Agg0, Agg1, row_stride, W0, W1, dC, st);
+  if (B == 5) return launch_basis_agg_t<5, LAYOUT, DC>(a, C, B, n_relw, Agg0, Agg1, row_stride, W0, W1, dC, st);
+  return launch_basis_agg_t<4, LAYOUT, DC>(a, C, B, n_relw, Agg0, Agg1, row_stride, W0, W1, dC, st);
 }
 
 int launch_basis_agg(const AggLaunch& a, const float* C, int B, int n_relw, int layout, float* Agg,
                      cudaStream_t st) {
-  if (a.n_items == 0) return RGCN_OK;
-  // bases per pass: all of them when they fit the register budget, else passes of 4
-  if (layout == 0) {
-    if (B == 1) return launch_basis_agg_t<1, 0>(a, C, B, n_relw, Agg, st);
-    if (B == 2) return launch_basis_agg_t<2, 0>(a, C, B, n_relw, Agg, st);
-    if (B <= 4) return launch_basis_agg_t<4, 0>(a, C, B, n_relw, Agg, st);
-    if (B == 5) return launch_basis_agg_t<5, 0>(a, C, B, n_relw, Agg, st);
-    return launch_basis_agg_t<4, 0>(a, C, B, n_relw, Agg, st);
-  } else {
-    if (B == 1) return launch_basis_agg_t<1, 1>(a, C, B, n_relw, Agg, st);
-    if (B == 2) return launch_basis_agg_t<2, 1>(a, C, B, n_relw, Agg, st);
-    if (B <= 4) return launch_basis_agg_t<4, 1>(a, C, B, n_relw, Agg, st);
-    if (B == 5) return launch_basis_agg_t<5, 1>(a, C, B, n_relw, Agg, st);
-    return launch_basis_agg_t<4, 1>(a, C, B, n_relw, Agg, st);
-  }
+  const int64_t dB = (int64_t)a.d * B;
+  if (layout == 0)
+    return launch_basis_agg_b<0, false>(a, C, B, n_relw, Agg, Agg + dB, 2 * dB, nullptr, nullptr, nullptr, st);
+  return launch_basis_agg_b<1, false>(a, C, B, n_relw, Agg, Agg + dB, 2 * dB, nullptr, nullptr, nullptr, st);
+}
+
+int launch_basis_agg_dc(const AggLaunch& a, const float* C, int B, int n_relw, const float* W0, const float* W1,
+                        float* dW0, float* dW1, float* dC, cudaStream_t st) {
+  return launch_basis_agg_b<1, true>(a, C, B, n_relw, dW0, dW1, (int64_t)a.d * B, W0, W1, dC, st);
 }
 
 template <int BC>

@@ -11,7 +11,7 @@ class BasisGcn(MessageGcn):
 
     def local_initialize_train(self):
         dev = self.get_device()
-        d_in = self.shape[0]
+        d_in = self.entity_count if self.onehot_input else self.shape[0]   # gcn_basis.py:16
         type_matrix_shape = (self.relation_count, self.n_coefficients)
         vertex_matrix_shape = (d_in, self.n_coefficients, self.shape[1])
         std = glorot_variance([vertex_matrix_shape[0], vertex_matrix_shape[2]])  # gcn_basis.py:21
@@ -27,6 +27,9 @@ class BasisGcn(MessageGcn):
 
     def fused_layer(self, H, graph, mode):
         mask, keep = self.make_drop_mask(graph.handle.V_dst, mode)
+        if self.onehot_input:
+            return ops.basis_onehot_layer(self.W_forward, self.W_backward, self.C_forward, self.C_backward,
+                                          self.W_self, graph.handle, mask, keep, self.use_nonlinearity)
         return ops.basis_layer(H, self.W_forward, self.W_backward, self.C_forward, self.C_backward,
                                self.W_self, graph.handle, mask, keep, self.use_nonlinearity)
 

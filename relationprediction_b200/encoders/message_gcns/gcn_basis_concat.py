@@ -5,6 +5,13 @@ from .message_gcn import MessageGcn
 
 
 class ConcatGcn(MessageGcn):
+    def __init__(self, shape, settings, next_component=None, onehot_input=False, use_nonlinearity=True):
+        if onehot_input:
+            raise NotImplementedError(
+                "ConcatGcn has no one-hot input layer: the reference reshapes the integer index vector as "
+                "[-1, B, s] features (gcn_basis_concat.py:42-43) and cannot run with UseInputTransform=No")
+        MessageGcn.__init__(self, shape, settings, next_component, onehot_input, use_nonlinearity)
+
     def parse_settings(self):
         self.dropout_keep_probability = float(self.settings['DropoutKeepProbability'])
         self.n_coefficients = int(self.settings['NumberOfBasisFunctions'])

@@ -21,10 +21,6 @@ class MessageGcn(Model):
         self.shape = shape
         self.vertex_embedding_function = {'train': None, 'test': None}
         Model.__init__(self, next_component, settings)
-        if onehot_input:
-            raise NotImplementedError(
-                "one-hot input layers (UseInputTransform=No) are outside the accelerated path; "
-                "both shipped R-GCN configs use UseInputTransform=Yes")
 
     def needs_graph(self):
         return True
@@ -34,9 +30,11 @@ class MessageGcn(Model):
 
     def get_vertex_features(self, senders=True, mode='train'):
         """H[sender] / H[receiver] row gathers (message_gcn.py:28-42) -- kept for API completeness;
-        the fused layer gathers rows inside the kernel instead."""
+        the fused layer gathers rows inside the kernel instead.  One-hot input: the index vector itself."""
         g = self.get_graph()
         idx = g.get_sender_indices() if senders else g.get_receiver_indices()
+        if self.onehot_input:
+            return idx
         code = self.next_component.get_all_codes(mode=mode)[0]
         return code[torch.as_tensor(idx, device=code.device).long()]
 
@@ -63,9 +61,10 @@ class MessageGcn(Model):
 
     def compute_vertex_embeddings(self, mode='train'):
         if self.vertex_embedding_function[mode] is None:
-            H = self.next_component.get_all_codes(mode=mode)[0]
             graph = self.get_graph()
-            self.vertex_embedding_function[mode] = self.fused_layer(H.contiguous(), graph, mode)
+            # one-hot input (message_gcn.py:33-34, :55-56): the input is the identity, nothing below is asked for codes
+            H = None if self.onehot_input else self.next_component.get_all_codes(mode=mode)[0].contiguous()
+            self.vertex_embedding_function[mode] = self.fused_layer(H, graph, mode)
         return self.vertex_embedding_function[mode]
 
     def get_all_codes(self, mode='train'):

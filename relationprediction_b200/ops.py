@@ -315,6 +315,64 @@ def basis_layer(H, W_forward, W_backward, C_forward, C_backward, W_self, graph, 
                                drop_mask, keep, relu)
 
 
+class _BasisOnehotLayerFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, Wf, Wb, Cf, Cb, Wself, graph, drop_mask, keep, relu):
+        lib = _lib.load()
+        if not (isinstance(Wf, torch.Tensor) and Wf.dim() == 3):
+            raise _lib.RgcnError("W_forward must be a [V, B, d] tensor")
+        _, B, d = Wf.shape
+        R = graph.n_relw // 2
+        _check_cuda_f32("W_forward", Wf, (graph.V_src, B, d))
+        _check_cuda_f32("W_backward", Wb, (graph.V_src, B, d))
+        _check_cuda_f32("C_forward", Cf, (R, B))
+        _check_cuda_f32("C_backward", Cb, (R, B))
+        _check_cuda_f32("W_self", Wself, (graph.V_dst, d))
+        mask = _mask_arg(drop_mask, graph.V_dst, d)
+        dev = Wf.device
+        out = torch.empty(graph.V_dst, d, dtype=torch.float32, device=dev)
+        nb = lib.rgcn_basis_onehot_workspace_bytes(graph.handle, d, B, 0)
+        if nb < 0:
+            _lib.check(int(nb), "rgcn_basis_onehot_workspace_bytes")
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_basis_onehot_forward(graph.handle, d, B, _ptr(Wf), _ptr(Wb), _ptr(Cf), _ptr(Cb), _ptr(Wself),
+                                           _ptr(mask), float(keep), int(bool(relu)), _ptr(out), _ptr(ws),
+                                           ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_basis_onehot_forward")
+        ctx.graph, ctx.keep, ctx.relu, ctx.mask = graph, float(keep), bool(relu), mask
+        ctx.save_for_backward(Wf, Wb, Cf, Cb, Wself, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, dOut):
+        lib = _lib.load()
+        Wf, Wb, Cf, Cb, Wself, out = ctx.saved_tensors
+        graph = ctx.graph
+        B, d = Wf.shape[1], Wf.shape[2]
+        dOut = dOut.contiguous()
+        _check_cuda_f32("dOut", dOut, (graph.V_dst, d))
+        dev = Wf.device
+        dWf, dWb = torch.empty_like(Wf), torch.empty_like(Wb)
+        dCf, dCb, dWself = torch.empty_like(Cf), torch.empty_like(Cb), torch.empty_like(Wself)
+        nb = lib.rgcn_basis_onehot_workspace_bytes(graph.handle, d, B, 1)
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_basis_onehot_backward(graph.handle, d, B, _ptr(Wf), _ptr(Wb), _ptr(Cf), _ptr(Cb),
+                                            _ptr(ctx.mask), ctx.keep, int(ctx.relu), _ptr(out), _ptr(dOut),
+                                            _ptr(dWf), _ptr(dWb), _ptr(dCf), _ptr(dCb), _ptr(dWself), _ptr(ws),
+                                            ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_basis_onehot_backward")
+        return dWf, dWb, dCf, dCb, dWself, None, None, None, None
+
+
+def basis_onehot_layer(W_forward, W_backward, C_forward, C_backward, W_self, graph, drop_mask=None, keep=1.0,
+                       relu=True):
+    """Featureless first basis layer (BasisGcn with onehot_input=True, gcn_basis.py:15-71): the input is the
+    identity, so the basis terms of a message are rows W_dir[source] of the [V, B, d] tables.  Differentiable in
+    every weight; there is no input gradient."""
+    return _BasisOnehotLayerFn.apply(W_forward, W_backward, C_forward, C_backward, W_self, graph, drop_mask, keep,
+                                     relu)
+
+
 def _triple_forward(ctx, entry, codes, rel, X, Y):
     """Forward of a triple scorer entry point with the distmult_forward argument list."""
     lib = _lib.load()

@@ -1,6 +1,7 @@
 """Secondary measurements (not the headline bench): DistMult and ComplEx scorer fwd/bwd bandwidth and fused
 ranking, basis layer
-(WN18 shape, BASELINE configs[2]; shipped gcn_basis.exp shape), block layer train-step graph."""
+(WN18 shape, BASELINE configs[2]; shipped gcn_basis.exp shape), block layer train-step graph, and the one-hot
+(UseInputTransform=No) first basis layer at the same shapes next to the feature-input basis layer."""
 import json
 import subprocess
 import sys
@@ -158,8 +159,56 @@ def layer_case(name, V, R, E, d, B, variant, skewed):
                  "M_edges_per_s": E / ms / 1e3, "stages_ms": {k: round(v, 4) for k, v in acc.items()}}
 
 
+def onehot_case(name, V, R, E, d, B):
+    """The featureless first basis layer (ops.basis_onehot_layer), no dropout mask, ReLU on.  Algorithmic bytes:
+    forward = distinct (source, direction) table rows * B*d*4 + M*(4d + 12) (one 4d-byte reduction and the index,
+    weight id and norm per message) + 4 [V, d] passes (W_self copy, ReLU); backward = the same table rows (dC) and
+    M*(4d + 12) (G gathers) + both dW tables written in full + 3 [V, d] passes (dOut and out read, G = dW_self
+    written)."""
+    tr = synthetic_kg(V, R, E, seed=1234, skewed=True)
+    gr = ops.Graph(tr, V, R, device=0)
+    std = 3.0 / np.sqrt(V + d)
+    ws = [(torch.randn(V, B, d, device=dev, generator=g) * std).requires_grad_(True) for _ in range(2)]
+    ws += [torch.randn(R, B, device=dev, generator=g).requires_grad_(True) for _ in range(2)]
+    ws.append((torch.randn(V, d, device=dev, generator=g) * std).requires_grad_(True))
+    dOut = torch.randn(V, d, device=dev, generator=g)
+    f = lambda: ops.basis_onehot_layer(ws[0], ws[1], ws[2], ws[3], ws[4], gr, None, 1.0, True)
+
+    def step():
+        for w in ws:
+            w.grad = None
+        f().backward(dOut)
+    ms = timeit(step, n=10)
+    with torch.no_grad():
+        ms_f = timeit(lambda: f(), n=10)
+    _lib.profile_enable(True)
+    acc = {}
+    for _ in range(5):
+        flush.zero_()
+        step()
+        torch.cuda.synchronize()
+        for nm, v in _lib.profile_read():
+            acc[nm] = acc.get(nm, 0.0) + v / 5
+    _lib.profile_enable(False)
+    M = 2 * E
+    rows = len(np.unique(tr[:, 0])) + len(np.unique(tr[:, 2]))     # (source, direction) pairs with messages
+    table = rows * B * d * 4
+    msgs = M * (4 * d + 12)
+    alg_f = table + msgs + 4 * V * d * 4
+    alg_b = table + msgs + 2 * V * B * d * 4 + 3 * V * d * 4
+    out[name] = {"V": V, "R": R, "E": E, "M": M, "d": d, "B": B, "gpu": gpu, "fwd_ms": ms_f, "fwd_bwd_ms": ms,
+                 "source_dir_rows": rows, "fwd_bytes_algorithmic": alg_f, "bwd_bytes_algorithmic": alg_b,
+                 "fwd_GBps_algorithmic": alg_f / ms_f / 1e6, "bwd_GBps_algorithmic": alg_b / max(ms - ms_f, 1e-6) / 1e6,
+                 "frac_of_3350_GBps": {"fwd": alg_f / ms_f / 1e6 / 3350, "bwd": alg_b / max(ms - ms_f, 1e-6) / 1e6 / 3350},
+                 "stages_ms": {k: round(v, 4) for k, v in acc.items()}}
+
+
 layer_case("wn18_basis_B2_d200 (BASELINE configs[2])", 40943, 18, 141442, 200, 2, "basis", True)
 layer_case("fb15k237_basis_B5_d500 (shipped gcn_basis.exp)", 14541, 237, 272115, 500, 5, "basis", True)
+layer_case("fb15k237_basis_B5_d500_trainstep_E15000", 14541, 237, 15000, 500, 5, "basis", True)
+onehot_case("wn18_onehot_B2_d200 (UseInputTransform=No)", 40943, 18, 141442, 200, 2)
+onehot_case("fb15k237_onehot_B5_d500 (gcn_basis.exp, UseInputTransform=No)", 14541, 237, 272115, 500, 5)
+onehot_case("fb15k237_onehot_B5_d500_trainstep_E15000", 14541, 237, 15000, 500, 5)
 layer_case("fb15k237_block_trainstep_E15000", 14541, 237, 15000, 500, 100, "block", True)
 layer_case("fb15k_block_B100_d500 (BASELINE configs[3] shape, 1 GPU)", 14951, 1345, 483142, 500, 100, "block", True)
 print(json.dumps(out, indent=1))
