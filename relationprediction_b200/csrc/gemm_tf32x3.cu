@@ -16,7 +16,8 @@
 //   warpgroups 1-2  consumers: rows 0-63 / 64-127 of the tile.  Per K block 4 K-steps x 3 wgmma.m64n128k8.tf32
 //                   into two register accumulators (hi*hi; the two cross terms), then the stage is released.  The
 //                   epilogue works straight from the accumulator registers.
-//   3-stage smem ring (64 KB per stage: A_hi, A_lo, B_hi, B_lo).
+//   3-stage smem ring (64 KB per stage: A_hi, A_lo, B_hi, B_lo); the TN kernel has 2 stages plus a ring of raw fp32
+//   blocks that its producer fills with cp.async and transposes from (see k_gemm_tn_tf32x3).
 // The NT kernel is persistent (min(tiles, SMs) CTAs walk the tiles; the producer runs on into the next tile while
 // the consumers finish the last one); the TN kernel keeps one tile (x split-K) per CTA.
 #include <cuda_runtime.h>
@@ -125,8 +126,9 @@ __device__ __forceinline__ uint32_t swz(int r, int c) {  // byte offset of 16 B 
   return (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4));
 }
 
+template <int NST = STAGES>
 __device__ __forceinline__ void init_barriers(uint64_t* full_bar, uint64_t* empty_bar) {
-  for (int s = 0; s < STAGES; ++s) {
+  for (int s = 0; s < NST; ++s) {
     mbar_init(&full_bar[s], N_PRODUCERS);
     mbar_init(&empty_bar[s], N_CONSUMERS);
   }
@@ -136,14 +138,15 @@ __device__ __forceinline__ void init_barriers(uint64_t* full_bar, uint64_t* empt
 // The K loop of one tile for one consumer warpgroup: k-blocks g0 .. g0 + num_kb - 1 of the CTA's stage sequence.
 // The hi*hi products and the cross terms go to separate accumulators (the tensor core adds into its accumulator
 // with truncation; same-magnitude additions per accumulator keep the result at SGEMM-level accuracy) and are summed
-// in fp32 in the epilogue.
+// in fp32 in the epilogue.  NST: stages in the ring.
+template <int NST = STAGES>
 __device__ __forceinline__ void consume_tile(uint32_t smem_base, uint64_t* full_bar, uint64_t* empty_bar, int g0,
                                              int num_kb, uint32_t a_rows, float (&big)[N_FRAG],
                                              float (&small)[N_FRAG]) {
   for (int kb = 0; kb < num_kb; ++kb) {
     const int g = g0 + kb;
-    const int s = g % STAGES;
-    mbar_wait(&full_bar[s], (uint32_t)(g / STAGES) & 1u);
+    const int s = g % NST;
+    mbar_wait(&full_bar[s], (uint32_t)(g / NST) & 1u);
     const uint32_t a_hi = smem_base + s * STAGE_BYTES + a_rows, a_lo = a_hi + TILE_BYTES;
     const uint32_t b_hi = smem_base + s * STAGE_BYTES + 2 * TILE_BYTES, b_lo = b_hi + TILE_BYTES;
     asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
@@ -395,101 +398,152 @@ __global__ void __launch_bounds__(N_THREADS, 1)
 // ------------------------------------------------------------------------------------------------
 // C[M,N] += A^T B with A [K,M] and B [K,N] row-major: the V-long reductions of the backward pass
 // (dW_self = H^T dS, basis dV = Agg^T G).  Both operands are MN-major in memory (the contraction index is the
-// slow one); TF32 wgmma reads K-major shared memory only, so the producer transposes while it splits: it loads
-// 16 B (4 consecutive M or N values of one k) and stores the 4 values as 4-byte elements of 4 K-major rows.
-// Lane mapping: 16 k-rows x 2 adjacent 16 B chunks per warp instruction (32 B sectors fully used in global
-// memory); the stores of a warp then hit 32 different banks.  Split-K over gridDim.z; partial tiles are added
-// with red.global.add.v2.
+// slow one); TF32 wgmma reads K-major shared memory only, so the producer transposes while it splits.
+//
+// Producer, two passes per k-block:
+//   copy       cp.async.cg of the raw fp32 [32 k x 128] slabs of A and B into a ring of TN_RAW staging blocks,
+//              TN_RAW - 1 k-blocks ahead of the conversion.  The loads in flight live in shared memory, not in
+//              registers.  A warp fetches one 512 B k-row per instruction.  Chunk q (16 B) of k-row k is stored at
+//              chunk q ^ ((k / 4) % 8) of its row, so that the conversion reads without bank conflicts.
+//   transpose  a thread reads 4 k-rows x 4 consecutive M (N) values (4 ld.shared.v4), transposes the 4 x 4 in
+//              registers, splits, and writes 4 + 4 st.shared.v4: the (hi, lo) chunks of 4 K-major rows in the
+//              SWIZZLE_128B layout.  The 8 lanes of a quarter-warp take the 8 k-groups of one 4-row group, so both
+//              their reads (staging chunks h ^ g) and their writes (swizzled chunks g ^ (r % 8)) cover all 32 banks.
+// Two MMA stages (128 KB) and three staging blocks (96 KB) fill the 227 KB of shared memory of a block.
+//
+// Split-K: CTA b computes tile b % tiles over k-block range b / tiles (see launch_gemm_tn_tf32x3 for the split
+// count); partial tiles are added into C with red.global.add.v2.  The CTAs of one k range are consecutive in the
+// grid and run at the same time, so each row of A and B comes from HBM once and is re-read from L2.
+//
+// Accuracy: the tensor core adds into its accumulator with truncation, so the error of one accumulation chain grows
+// with its length (K = 50 000, M = N = 512, normal inputs: 7e-6 relative for 92 k-blocks per chain, 1.6e-5 for
+// 196; K = 5 M with 17 splits: 5.8e-4).  A CTA therefore adds its partial tile into C (round-to-nearest) every
+// TN_FLUSH_KB k-blocks and restarts the accumulators, which bounds the chain whatever the split length: 3e-6 at
+// K = 50 000 and at K = 5 M.  On an H100 SXM the flushes cost about 1 ms of 29 at K = 5 M, M = N = 512.
 // ------------------------------------------------------------------------------------------------
+constexpr int TN_FLUSH_KB = 32;                         // k-blocks per accumulation chain
+constexpr int TN_STAGES = 2;                            // MMA stages (A_hi, A_lo, B_hi, B_lo)
+constexpr int TN_RAW = 3;                               // fp32 staging blocks
+constexpr int RAW_TILE_BYTES = BK * BM * 4;             // 16 KB: 32 k-rows x 128 values of one operand
+constexpr int RAW_BYTES = 2 * RAW_TILE_BYTES;           // A and B
+constexpr int TN_SMEM_BYTES = TN_STAGES * STAGE_BYTES + TN_RAW * RAW_BYTES + 1024;
+static_assert(TN_SMEM_BYTES <= 227 * 1024, "TN kernel exceeds the shared memory of a block");
+static_assert(N_PRODUCERS == 128 && BK == 32 && BM == 128, "the TN producer's lane mapping assumes these");
+
+__device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, float x, float y, float z, float w) {
+  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(x), "f"(y), "f"(z), "f"(w) : "memory");
+}
+
 __global__ void __launch_bounds__(N_THREADS, 1)
     k_gemm_tn_tf32x3(const float* __restrict__ A, int64_t lda, const float* __restrict__ B, int64_t ldb,
                      float* __restrict__ C, int64_t ldc, int M, int N, int K, int kb_per_split) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
+  __shared__ __align__(8) uint64_t full_bar[TN_STAGES], empty_bar[TN_STAGES];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
-  const int kb_total = (K + BK - 1) / BK;
-  const int kb_begin = blockIdx.z * kb_per_split;
-  const int num_kb = min(kb_per_split, kb_total - kb_begin);
-  if (num_kb <= 0) return;
+  const int tm = (M + BM - 1) / BM, tiles = tm * ((N + BN - 1) / BN);
+  const int tile = (int)blockIdx.x % tiles, split = (int)blockIdx.x / tiles;
+  const int m0 = (tile % tm) * BM, n0 = (tile / tm) * BN;
+  const int kb_begin = split * kb_per_split;
+  const int num_kb = min(kb_per_split, (K + BK - 1) / BK - kb_begin);   // >= 1: the launch makes no empty split
 
-  if (tid == 0) init_barriers(full_bar, empty_bar);
+  if (tid == 0) init_barriers<TN_STAGES>(full_bar, empty_bar);
   __syncthreads();
 
   if (tid < N_PRODUCERS) {
-    constexpr int NC = 8;                                  // 16 B chunks of each operand per thread and k-block
-    const int kr = (lane & 15) + 16 * (warp & 1);          // k-row of the block
-    const int cm0 = (lane >> 4) + 16 * (warp >> 1);        // chunk i covers M (N) values 4 (cm0 + 2 i) .. +3
-    auto load_ab = [&](int kbi, float4 (&va)[NC], float4 (&vb)[NC]) {
-      const int krow = (kb_begin + kbi) * BK + kr;
-      const bool kok = krow < K;
-      const float* pa = A + (size_t)(kok ? krow : 0) * lda + m0;
-      const float* pb = B + (size_t)(kok ? krow : 0) * ldb + n0;
+    const uint32_t raw_base = smem_base + TN_STAGES * STAGE_BYTES;
+    // copy pass: this thread fetches chunk `lane` of k-rows warp + 4 i (i < 8) of both operands
+    const bool a_ok = m0 + 4 * lane < M, b_ok = n0 + 4 * lane < N;   // M, N % 4 == 0: a chunk is all in or all out
+    const float* pa = A + (a_ok ? m0 + 4 * lane : 0);
+    const float* pb = B + (b_ok ? n0 + 4 * lane : 0);
+    auto issue = [&](int kbi) {
+      const uint32_t dst = raw_base + (kbi % TN_RAW) * RAW_BYTES;
+      const int k0 = (kb_begin + kbi) * BK + warp;
 #pragma unroll
-      for (int i = 0; i < NC; ++i) {
-        const int cm = cm0 + 2 * i;
-        va[i] = (kok && m0 + 4 * cm < M) ? __ldg(reinterpret_cast<const float4*>(pa + 4 * cm))
-                                         : make_float4(0.f, 0.f, 0.f, 0.f);
-        vb[i] = (kok && n0 + 4 * cm < N) ? __ldg(reinterpret_cast<const float4*>(pb + 4 * cm))
-                                         : make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int i = 0; i < 8; ++i) {
+        const bool kok = k0 + 4 * i < K;
+        const size_t row = kok ? (size_t)(k0 + 4 * i) : 0;
+        const uint32_t off = (uint32_t)((warp + 4 * i) * 512 + ((lane ^ i) << 4));   // (k / 4) % 8 == i
+        cp_async16(dst + off, pa + row * lda, kok && a_ok ? 16u : 0u);
+        cp_async16(dst + RAW_TILE_BYTES + off, pb + row * ldb, kok && b_ok ? 16u : 0u);
       }
+      asm volatile("cp.async.commit_group;" ::: "memory");
     };
-    auto store4 = [&](uint32_t hi_base, const float4& v, int cm) {
-      const float x[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const int r = 4 * cm + j;   // K-major tile row (M or N index); kr is the column
-        const uint32_t off =
-            (uint32_t)((r >> 3) * 1024 + (r & 7) * 128 + ((((kr >> 2) ^ (r & 7)) << 4) | ((kr & 3) << 2)));
-        float hi, lo;
-        split_tf32_trunc(x[j], hi, lo);
-        asm volatile("st.shared.f32 [%0], %1;" ::"r"(hi_base + off), "f"(hi) : "memory");
-        asm volatile("st.shared.f32 [%0], %1;" ::"r"(hi_base + TILE_BYTES + off), "f"(lo) : "memory");
-      }
-    };
-    // the loads of block kb+1 are in flight while block kb is split and stored
-    float4 va[2][NC], vb[2][NC];
-    load_ab(0, va[0], vb[0]);
-    for (int kb0 = 0; kb0 < num_kb; kb0 += 2) {
+    // transpose pass: this thread converts k-group g (k-rows 4g .. 4g+3) of the 4-row groups h and h + 16
+    const int g = lane & 7;
+    auto convert = [&](uint32_t raw, uint32_t hi_plane) {
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
-        const int kbi = kb0 + u;
-        if (kbi >= num_kb) break;
-        if (kbi + 1 < num_kb) load_ab(kbi + 1, va[u ^ 1], vb[u ^ 1]);
-        const int s = kbi % STAGES;
-        mbar_wait(&empty_bar[s], ((uint32_t)(kbi / STAGES) & 1u) ^ 1u);
-        const uint32_t a_hi = smem_base + s * STAGE_BYTES, b_hi = a_hi + 2 * TILE_BYTES;
+        const int h = (lane >> 3) + 4 * warp + 16 * u;
+        float4 v[4];
 #pragma unroll
-        for (int i = 0; i < NC; ++i) {
-          store4(a_hi, va[u][i], cm0 + 2 * i);
-          store4(b_hi, vb[u][i], cm0 + 2 * i);
+        for (int j = 0; j < 4; ++j) v[j] = ld_shared_v4(raw + (4 * g + j) * 512 + ((h ^ g) << 4));
+        const float x[4][4] = {{v[0].x, v[1].x, v[2].x, v[3].x}, {v[0].y, v[1].y, v[2].y, v[3].y},
+                               {v[0].z, v[1].z, v[2].z, v[3].z}, {v[0].w, v[1].w, v[2].w, v[3].w}};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {   // K-major tile row 4 h + i, chunk g: k = 4g .. 4g+3
+          float hi[4], lo[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) split_tf32_trunc(x[i][j], hi[j], lo[j]);
+          const uint32_t a = hi_plane + swz(4 * h + i, g);
+          st_shared_v4(a, hi[0], hi[1], hi[2], hi[3]);
+          st_shared_v4(a + TILE_BYTES, lo[0], lo[1], lo[2], lo[3]);
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbar_arrive(&full_bar[s]);
       }
+    };
+    issue(0);
+    if (num_kb > 1)
+      issue(1);
+    else
+      asm volatile("cp.async.commit_group;" ::: "memory");   // one group per k-block, empty ones included
+    for (int kb = 0; kb < num_kb; ++kb) {
+      asm volatile("cp.async.wait_group 1;" ::: "memory");     // this thread's copies of block kb have landed
+      // everyone's copies of block kb are visible, and nobody reads block kb - 1's staging block any more
+      asm volatile("bar.sync 1, %0;" ::"n"(N_PRODUCERS) : "memory");
+      if (kb + 2 < num_kb)
+        issue(kb + 2);
+      else
+        asm volatile("cp.async.commit_group;" ::: "memory");
+      const int s = kb % TN_STAGES;
+      mbar_wait(&empty_bar[s], ((uint32_t)(kb / TN_STAGES) & 1u) ^ 1u);
+      const uint32_t raw = raw_base + (kb % TN_RAW) * RAW_BYTES, stage = smem_base + s * STAGE_BYTES;
+      convert(raw, stage);                                          // A -> A_hi, A_lo
+      convert(raw + RAW_TILE_BYTES, stage + 2 * TILE_BYTES);        // B -> B_hi, B_lo
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> tensor core
+      mbar_arrive(&full_bar[s]);
     }
   } else {
-    // consumers: the same K loop as the NT kernel, then this split's tile is added into C
+    // consumers: the same K loop as the NT kernel, in chunks of at most TN_FLUSH_KB k-blocks; after each chunk the
+    // partial tile is added into C and the accumulators start again from zero
     const int ctid = tid - N_PRODUCERS;
     const int wg = ctid >> 7;
-    float big[N_FRAG], small[N_FRAG];
-    consume_tile(smem_base, full_bar, empty_bar, 0, num_kb, (uint32_t)(wg * 64 * 128), big, small);
     const int r0 = m0 + wg * 64 + ((ctid >> 5) & 3) * 16 + (lane >> 2);
     const int c0 = n0 + 2 * (lane & 3);
+    float* const cbase = C + (size_t)r0 * ldc + c0;
+    float big[N_FRAG], small[N_FRAG];
+    for (int kc = 0; kc < num_kb; kc += TN_FLUSH_KB) {
+      consume_tile<TN_STAGES>(smem_base, full_bar, empty_bar, kc, min(TN_FLUSH_KB, num_kb - kc),
+                              (uint32_t)(wg * 64 * 128), big, small);
+      float* cp = cbase;
+      asm volatile("" : "+l"(cp));   // keeps the 32 addresses below from being hoisted out of the loop (spills)
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r0 + 8 * h;
-      if (row >= M) continue;
-      float* crow = C + (size_t)row * ldc;
+      for (int h = 0; h < 2; ++h) {
+        if (r0 + 8 * h >= M) continue;
+        float* crow = cp + (size_t)(8 * h) * ldc;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = c0 + 8 * j;
-        if (col < N)
-          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(crow + col),
-                       "f"(big[4 * j + 2 * h] + small[4 * j + 2 * h]),
-                       "f"(big[4 * j + 2 * h + 1] + small[4 * j + 2 * h + 1])
-                       : "memory");
+        for (int j = 0; j < BN / 8; ++j) {
+          if (c0 + 8 * j < N)
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(crow + 8 * j),
+                         "f"(big[4 * j + 2 * h] + small[4 * j + 2 * h]),
+                         "f"(big[4 * j + 2 * h + 1] + small[4 * j + 2 * h + 1])
+                         : "memory");
+        }
       }
     }
   }
@@ -618,20 +672,35 @@ int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t l
   static bool attr_set = false;
   if (!attr_set) {
     int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tn_tf32x3, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  SMEM_BYTES),
+                                                  TN_SMEM_BYTES),
                              "cudaFuncSetAttribute(gemm tn smem)");
     if (rc) return rc;
     attr_set = true;
   }
-  const int tm = (M + BM - 1) / BM, tn = (N + BN - 1) / BN;
-  const int kb_total = (K + BK - 1) / BK;
-  int splits = (2 * sm_count() + tm * tn - 1) / (tm * tn);  // about two waves of CTAs
-  if (splits > kb_total / 4) splits = kb_total / 4;  // at least 4 K blocks per split
-  if (splits < 1) splits = 1;
-  const int kb_per_split = (kb_total + splits - 1) / splits;
-  splits = (kb_total + kb_per_split - 1) / kb_per_split;
-  dim3 grid(tm, tn, splits);
-  k_gemm_tn_tf32x3<<<grid, N_THREADS, SMEM_BYTES, st>>>(A, lda, B, ldb, C, ldc, M, N, K, kb_per_split);
+  // Split count: one CTA per SM, so the CTAs run in waves of `sms`; a split of kb_per_split k-blocks costs its
+  // k-blocks plus about TN_KB_FIXED k-blocks of pipeline fill and epilogue.  Take the split count with the least
+  // waves x (kb_per_split + TN_KB_FIXED), the smallest one on ties.  When the tiles fit the SMs this is one wave of
+  // floor(sms / tiles) splits for long K (M = N = 512, K = 5 M on 132 SMs: 8 splits, 128 CTAs); with more tiles
+  // than one wave holds, more (shorter) splits fill the last wave.
+  constexpr int64_t TN_KB_FIXED = 4;
+  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+  const int64_t kb_total = (K + BK - 1) / BK, sms = sm_count();
+  int64_t splits = 1, kb_per_split = kb_total, best = -1;
+  for (int64_t s = 1; s <= kb_total && (s == 1 || s * tiles <= 8 * sms); ++s) {
+    const int64_t kps = (kb_total + s - 1) / s, s_eff = (kb_total + kps - 1) / kps;   // no empty split
+    const int64_t cost = (s_eff * tiles + sms - 1) / sms * (kps + TN_KB_FIXED);
+    if (best < 0 || cost < best) {
+      best = cost;
+      splits = s_eff;
+      kb_per_split = kps;
+    }
+  }
+  if (tiles * splits > 0x7fffffffLL) {
+    rgcn_set_error("gemm_tn_tf32x3: too many tiles");
+    return RGCN_ERR_INVALID;
+  }
+  k_gemm_tn_tf32x3<<<(unsigned)(tiles * splits), N_THREADS, TN_SMEM_BYTES, st>>>(A, lda, B, ldb, C, ldc, M, N, K,
+                                                                                 (int)kb_per_split);
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tn_tf32x3");
 }
