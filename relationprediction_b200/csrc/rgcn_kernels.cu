@@ -1204,11 +1204,19 @@ bool block_rel_supported(int d, int s) {
   return false;
 }
 
+// warps per item of the s = 5 group kernel (k_block_relg): 4 or 2; any other RGCN_REL_GROUP value selects the
+// one-warp-per-slab k_block_rel<5, NV, false>, which has no dW-fused form
+static int rel_group_s5() {
+  int G = 4;
+  if (const char* e = std::getenv("RGCN_REL_GROUP")) G = std::atoi(e);
+  return (G == 4 || G == 2) ? G : 0;
+}
+
 // the dW-fused variant keeps 2*s*NV float4 of weights + gradient accumulators in registers
 bool block_rel_fuse_dw_supported(int d, int s) {
   if (s == 5) {  // group-kernel variant: dH+dW in one walk (RGCN_FUSE_DW_S5=0: two separate walks)
     const char* e = std::getenv("RGCN_FUSE_DW_S5");
-    return d <= 512 && !(e && std::atoi(e) == 0);
+    return d <= 512 && rel_group_s5() != 0 && !(e && std::atoi(e) == 0);
   }
   return s == 4 || s == 8 || s == 16;
 }
@@ -1218,7 +1226,7 @@ int launch_block_rel(const WorkItem* items, int n_items, const int32_t* r_row, c
                      float* out, const float* Hrow, int ldh, float* dWt, cudaStream_t st) {
   if (n_items == 0) return RGCN_OK;
   const bool fuse = dWt != nullptr;
-  if (fuse && !block_rel_fuse_dw_supported(d, s) && s != 5) {
+  if (fuse && !block_rel_fuse_dw_supported(d, s)) {  // a caller that asks for dW must get it, or an error
     rgcn_set_error("rel-major block kernel: dW fusion unsupported for this block size");
     return RGCN_ERR_INVALID;
   }
@@ -1238,9 +1246,8 @@ int launch_block_rel(const WorkItem* items, int n_items, const int32_t* r_row, c
     if (v >= 1 && v <= 4 && s != 5 && (v * 128) % s == 0) nv = std::min(nv, v);
   }
   if (s == 5) {
-    int G = 4;
-    if (const char* e = std::getenv("RGCN_REL_GROUP")) G = std::atoi(e);
-    if (G == 4 || G == 2) {
+    const int G = rel_group_s5();
+    if (G != 0) {
       const int groups = RGCN_WARPS_PER_BLOCK / G;
       dim3 grid((n_items + groups - 1) / groups);
       if (G == 4) {
