@@ -310,6 +310,29 @@ int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int32_t B, cons
                                float* dCb, float* dWself, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Highway skip connection between R-GCN layers (SkipConnections=Highway, model_builder.py:304-305;
+ * extras/highway_layer.py:14-38).  c1 = the wrapped layer's output, c2 = the layer's input:
+ *
+ *   g = sigmoid(c2 W + b),   out = g * c1 + (1 - g) * c2          (highway_layer.py:21, :34-38)
+ *
+ * c1, c2, out, gate, dOut, dc1, dc2 : [V, d];  W, dW : [d, d] (z = c2 W, W indexed [in, out]);  b, db : [d].
+ * The forward is one gate GEMM with the blend in its epilogue; `gate` (g) is written for the backward pass.
+ * Backward:  dc1 = g dOut,  dz = dOut (c1 - c2) g (1 - g),  dc2 = (1 - g) dOut + dz W^T,  dW = c2^T dz,
+ *            db = column sums of dz.  Every output is overwritten (dc2 does not include the gradient c2 receives
+ *            through the wrapped layer).
+ * Arguments are checked before any device work: null pointers, V < 0 or d <= 0 or d % 4 != 0 are RGCN_ERR_INVALID,
+ * a short workspace RGCN_ERR_WORKSPACE.  V = 0 does nothing.  No device: RGCN_ERR_NODEVICE.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_highway_workspace_bytes(int64_t V, int32_t d, int backward);
+
+int rgcn_highway_forward(const float* c1, const float* c2, const float* W, const float* b, int64_t V, int32_t d,
+                         float* out, float* gate, void* workspace, int64_t workspace_bytes, void* stream);
+
+int rgcn_highway_backward(const float* c1, const float* c2, const float* W, const float* gate, const float* dOut,
+                          int64_t V, int32_t d, float* dc1, float* dc2, float* dW, float* db, void* workspace,
+                          int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * DistMult triple scorer ("BilinearDiag", decoders/bilinear_diag.py:14-34, :63-69).
  *
  *   energy[n] = sum_k codes[X[n,0],k] * rel[X[n,1],k] * codes[X[n,2],k]

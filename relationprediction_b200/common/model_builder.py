@@ -1,7 +1,8 @@
 """Name= -> component chain factory (reference: common/model_builder.py:26-184, :273-319).
 
 Only the branches on the accelerated path are built: encoders `gcn_basis` (BasisGcn, or ConcatGcn
-when Concatenation=Yes; with UseInputTransform=No layer 0 is a one-hot BasisGcn) and `embedding`; decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
+when Concatenation=Yes; with UseInputTransform=No layer 0 is a one-hot BasisGcn; SkipConnections=Highway wraps every
+feature-input layer in a HighwayLayer) and `embedding`; decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag
 from ..decoders.complex import Complex
@@ -10,6 +11,7 @@ from ..encoders.message_gcns.gcn_basis import BasisGcn
 from ..encoders.message_gcns.gcn_basis_concat import ConcatGcn
 from ..encoders.relation_embedding import RelationEmbedding
 from ..extras.graph_representations import Representation
+from ..extras.highway_layer import HighwayLayer
 
 
 def _flag(settings, key, default="No"):
@@ -53,9 +55,16 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
     for flag in ('AddDiagonal', 'DiagonalCoefficients', 'StoreEdgeData'):
         if _flag(encoder_settings, flag) == "Yes":
             raise NotImplementedError("%s=Yes selects an ablation variant outside the accelerated path" % flag)
-    if _flag(encoder_settings, 'SkipConnections', 'None') not in ('None', 'Residual'):
-        # 'Residual' is a no-op in the reference (model_builder.py:302-307 overwrites it); 'Highway' is not
-        raise NotImplementedError("SkipConnections=Highway is outside the accelerated path")
+    skip = _flag(encoder_settings, 'SkipConnections', 'None')
+    if skip not in ('None', 'Residual', 'Highway'):
+        raise NotImplementedError("SkipConnections=%s is not a reference option" % skip)
+    if skip == 'Highway' and _flag(encoder_settings, 'UseInputTransform') == "No":
+        # In the reference, layer 1's highway reads its carry input from MessageGcn's class-level cache, which by
+        # then holds layer 1's own output: out = g L1 + (1 - g) L1 = L1 and the gate gets zero gradient.  Neither
+        # that dead gate nor a working one (which would silently differ from the reference) is built.
+        raise NotImplementedError("SkipConnections=Highway with UseInputTransform=No: the reference's highway gate "
+                                  "is dead there (its carry input is the layer's own output through the shared "
+                                  "MessageGcn cache), so this combination is not built")
     model = ConcatGcn if _flag(encoder_settings, 'Concatenation') == "Yes" else BasisGcn
     for layer in range(layers):
         use_nonlinearity = layer < layers - 1  # the last layer is linear (model_builder.py:275)
@@ -63,8 +72,13 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
         onehot_input = (layer == 0 and _flag(encoder_settings, 'UseInputTransform') == "No"
                         and _flag(encoder_settings, 'RandomInput') == "No"
                         and _flag(encoder_settings, 'PartiallyRandomInput') == "No")
-        encoding = model(internal_shape, encoder_settings, next_component=encoding, onehot_input=onehot_input,
-                         use_nonlinearity=use_nonlinearity)
+        new_encoding = model(internal_shape, encoder_settings, next_component=encoding, onehot_input=onehot_input,
+                             use_nonlinearity=use_nonlinearity)
+        # 'Residual' is a no-op in the reference (model_builder.py:302-307: the else branch overwrites it)
+        if skip == 'Highway' and not onehot_input:
+            encoding = HighwayLayer(internal_shape, next_component=new_encoding, next_component_2=encoding)
+        else:
+            encoding = new_encoding
     return encoding
 
 

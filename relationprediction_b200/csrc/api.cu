@@ -897,6 +897,84 @@ extern "C" int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int3
 }
 
 // ------------------------------------------------------------------------------------------------
+// Highway skip connection (extras/highway_layer.py): one gate GEMM with the blend epilogue forward; an elementwise
+// prologue and two GEMMs backward
+// ------------------------------------------------------------------------------------------------
+extern "C" int64_t rgcn_highway_workspace_bytes(int64_t V, int32_t d, int backward) {
+  if (V < 0 || d <= 0) {
+    rgcn_set_error("rgcn_highway_workspace_bytes: bad arguments");
+    return RGCN_ERR_INVALID;
+  }
+  int64_t bytes = align_up((int64_t)2 * d * d * 4);     // hi / lo planes of the pre-split W (or W^T)
+  if (backward) bytes += align_up(V * d * 4);           // dz
+  return bytes + 256;
+}
+
+static int highway_checks(bool ok, int64_t V, int32_t d, int64_t workspace_bytes, int backward, const char* who) {
+  if (!ok || V < 0 || V > 0x7fffffffLL || d <= 0 || d % 4 != 0) {
+    rgcn_set_error(std::string(who) + ": need non-null pointers, 0 <= V < 2^31, d > 0, d % 4 == 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_highway_workspace_bytes(V, d, backward)) {
+    rgcn_set_error(std::string(who) + ": workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  if (V == 0) return RGCN_OK;
+  int n_dev = 0;
+  if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
+    cudaGetLastError();
+    rgcn_set_error(std::string(who) + ": no CUDA device");
+    return RGCN_ERR_NODEVICE;
+  }
+  return RGCN_OK;
+}
+
+extern "C" int rgcn_highway_forward(const float* c1, const float* c2, const float* W, const float* b, int64_t V,
+                                    int32_t d, float* out, float* gate, void* workspace, int64_t workspace_bytes,
+                                    void* stream) {
+  int rc = highway_checks(c1 && c2 && W && b && out && gate && workspace, V, d, workspace_bytes, 0,
+                          "rgcn_highway_forward");
+  if (rc || V == 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver ws(workspace, workspace_bytes);
+  float* hi = ws.take<float>((int64_t)2 * d * d);
+  float* lo = hi + (size_t)d * d;
+  MARK("start");
+  // Bt = W^T (B = W is [K = in, N = out]); the split is d^2 elements, the GEMM V d^2
+  rc = launch_gemm_split_b(W, d, d, d, /*transposed=*/1, hi, lo, st);
+  if (rc) return rc;
+  rc = launch_gemm_highway_tf32x3(c2, hi, lo, b, c1, out, gate, (int)V, d, st);
+  MARK("highway_gate_gemm");
+  return rc;
+}
+
+extern "C" int rgcn_highway_backward(const float* c1, const float* c2, const float* W, const float* gate,
+                                     const float* dOut, int64_t V, int32_t d, float* dc1, float* dc2, float* dW,
+                                     float* db, void* workspace, int64_t workspace_bytes, void* stream) {
+  int rc = highway_checks(c1 && c2 && W && gate && dOut && dc1 && dc2 && dW && db && workspace, V, d,
+                          workspace_bytes, 1, "rgcn_highway_backward");
+  if (rc || V == 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver ws(workspace, workspace_bytes);
+  float* hi = ws.take<float>((int64_t)2 * d * d);
+  float* lo = hi + (size_t)d * d;
+  float* dz = ws.take<float>(V * d);
+  MARK("start");
+  rc = launch_highway_prologue(c1, c2, gate, dOut, V, d, dc1, dz, dc2, db, st);
+  if (rc) return rc;
+  MARK("highway_prologue");
+  // dc2 += dz W^T: Bt = W itself ([N = in, K = out], already K-major)
+  rc = launch_gemm_split_b(W, d, d, d, /*transposed=*/0, hi, lo, st);
+  if (!rc) rc = launch_gemm_tf32x3(dz, d, hi, lo, d, dc2, d, (int)V, d, d, /*accumulate=*/1, st);
+  if (rc) return rc;
+  MARK("highway_dc2_gemm");
+  // dW = c2^T dz (contraction over V)
+  rc = launch_gemm_tn_tf32x3(c2, d, dz, d, dW, d, d, d, (int)V, /*accumulate=*/0, st);
+  MARK("highway_dW_gemm");
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------
 // DistMult
 // ------------------------------------------------------------------------------------------------
 extern "C" int distmult_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel,

@@ -182,6 +182,24 @@ struct RankEpi {
 };
 __device__ __forceinline__ float sigmoid_ref(float x) { return 1.0f / (1.0f + expf(-x)); }
 
+// EPI = 2: HIGHWAY epilogue (the gate of extras/highway_layer.py:19-38): A = c2 [M, K = N] is the layer input, Bt the
+// gate weight W^T, and each accumulator pair becomes  z = acc + bias[col],  g = sigmoid(z),
+// out = c2 + g (c1 - c2)  (= g c1 + (1 - g) c2), written to C together with g (kept for the backward pass).  z itself
+// is never stored.  c1, C and gate share the leading dimension ldc; c2 is read through A with lda.
+struct HighwayEpi {
+  const float* bias;           // [N]
+  const float* c1;             // [M, ldc] the wrapped layer's output
+  float* gate;                 // [M, ldc] g
+};
+template <int EPI>
+struct EpiArgs {
+  using type = RankEpi;
+};
+template <>
+struct EpiArgs<2> {
+  using type = HighwayEpi;
+};
+
 // PERSISTENT: a CTA walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... (N tiles fastest, see below); the
 // shared-memory stages and their barrier phases run on across tile boundaries, so the producer fills the pipeline of
 // tile t+1 (global-load latency included) while the consumers run the epilogue of tile t.
@@ -189,7 +207,7 @@ template <int EPI>
 __global__ void __launch_bounds__(N_THREADS, 1)
     k_gemm_tf32x3(const float* __restrict__ A, int64_t lda, const float* __restrict__ Bhi,
                   const float* __restrict__ Blo, int64_t ldb, float* __restrict__ C, int64_t ldc,
-                  int M, int N, int K, int accumulate, int n_tiles, RankEpi re) {
+                  int M, int N, int K, int accumulate, int n_tiles, typename EpiArgs<EPI>::type re) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
@@ -338,7 +356,29 @@ __global__ void __launch_bounds__(N_THREADS, 1)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = r0 + 8 * h;
-        if (EPI == 1) {
+        if constexpr (EPI == 2) {
+          if (row >= M) continue;
+          const float* c2row = A + (size_t)row * lda;
+          const float* c1row = re.c1 + (size_t)row * ldc;
+          float* orow = C + (size_t)row * ldc;
+          float* grow = re.gate + (size_t)row * ldc;
+          asm volatile("" : "+l"(c2row), "+l"(c1row));   // no hoisting of the 16 pairs' loads ahead of use (spills)
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = c0 + 8 * j;
+            if (col < N) {  // N % 4 == 0: both columns of the pair exist
+              const float2 bb = __ldg(reinterpret_cast<const float2*>(re.bias + col));
+              const float2 x1 = __ldg(reinterpret_cast<const float2*>(c1row + col));
+              const float2 x2 = __ldg(reinterpret_cast<const float2*>(c2row + col));
+              const float g0 = sigmoid_ref(big[4 * j + 2 * h] + small[4 * j + 2 * h] + bb.x);
+              const float g1 = sigmoid_ref(big[4 * j + 2 * h + 1] + small[4 * j + 2 * h + 1] + bb.y);
+              *reinterpret_cast<float2*>(orow + col) = make_float2(x2.x + g0 * (x1.x - x2.x), x2.y + g1 * (x1.y - x2.y));
+              *reinterpret_cast<float2*>(grow + col) = make_float2(g0, g1);
+            }
+          }
+          continue;
+        }
+        if constexpr (EPI == 1) {
           int raw = 0, kn = 0;
           if (row < M) {
             const float gold_s = __ldg(re.gold_sig + row);
@@ -653,6 +693,35 @@ int launch_gemm_rank_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
                                                          (int)tiles, re);
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<rank>");
+}
+
+// Highway gate GEMM with the blend epilogue (EPI = 2): z = c2 @ W + bias with W pre-split as Bt = W^T [d, d];
+// out = c2 + sigmoid(z) (c1 - c2), gate = sigmoid(z).  All matrices [M, d] row-major, contiguous.
+int launch_gemm_highway_tf32x3(const float* c2, const float* Bt_hi, const float* Bt_lo, const float* bias,
+                               const float* c1, float* out, float* gate, int M, int d, cudaStream_t st) {
+  if (M == 0) return RGCN_OK;
+  if (d <= 0 || d % 4 != 0) {
+    rgcn_set_error("gemm_highway_tf32x3: d > 0, d % 4 == 0");
+    return RGCN_ERR_INVALID;
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  SMEM_BYTES),
+                             "cudaFuncSetAttribute(gemm highway smem)");
+    if (rc) return rc;
+    attr_set = true;
+  }
+  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((d + BN - 1) / BN);
+  if (tiles > 0x7fffffffLL) {
+    rgcn_set_error("gemm_highway_tf32x3: too many tiles");
+    return RGCN_ERR_INVALID;
+  }
+  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
+  k_gemm_tf32x3<2><<<grid, N_THREADS, SMEM_BYTES, st>>>(c2, d, Bt_hi, Bt_lo, d, out, d, M, d, d, 0, (int)tiles,
+                                                         HighwayEpi{bias, c1, gate});
+  ++g_rgcn_launches;
+  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<highway>");
 }
 
 // C[M,N] (+)= A^T B, A [K,M] row-major, B [K,N] row-major (see k_gemm_tn_tf32x3)

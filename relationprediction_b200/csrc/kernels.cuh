@@ -121,6 +121,15 @@ int launch_gemm_rank_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
 int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
                           int M, int N, int K, int accumulate, cudaStream_t st);
 
+// Highway gate GEMM with the blend epilogue: gate = sigmoid(c2 W + bias), out = c2 + gate (c1 - c2); W given
+// pre-split as Bt = W^T [d, d]; all [M, d] matrices contiguous
+int launch_gemm_highway_tf32x3(const float* c2, const float* Bt_hi, const float* Bt_lo, const float* bias,
+                               const float* c1, float* out, float* gate, int M, int d, cudaStream_t st);
+// highway.cu -- highway backward prologue: dc1 = g dY, dc2 = (1 - g) dY, dz = dY (c1 - c2) g (1 - g),
+// db = column sums of dz (db is overwritten)
+int launch_highway_prologue(const float* c1, const float* c2, const float* g, const float* dY, int64_t V, int d,
+                            float* dc1, float* dz, float* dc2, float* db, cudaStream_t st);
+
 // DistMult
 // queries + gold scores of the fused scorer/ranker: side 0 (subjects corrupted): Q[t] = rel[r] * codes[o], gold = s;
 // side 1 (objects corrupted): Q[t] = codes[s] * rel[r], gold = o.  gold_sig[t] = sigmoid(<Q[t], codes[gold]>)

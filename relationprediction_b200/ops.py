@@ -373,6 +373,54 @@ def basis_onehot_layer(W_forward, W_backward, C_forward, C_backward, W_self, gra
                                      relu)
 
 
+class _HighwayFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, c1, c2, W, b):
+        lib = _lib.load()
+        if not (isinstance(c1, torch.Tensor) and c1.dim() == 2):
+            raise _lib.RgcnError("c1 must be a [V, d] tensor")
+        V, d = c1.shape
+        _check_cuda_f32("c1", c1)
+        _check_cuda_f32("c2", c2, (V, d))
+        _check_cuda_f32("W", W, (d, d))
+        _check_cuda_f32("b", b, (d,))
+        dev = c1.device
+        out = torch.empty(V, d, dtype=torch.float32, device=dev)
+        gate = torch.empty(V, d, dtype=torch.float32, device=dev)
+        nb = lib.rgcn_highway_workspace_bytes(V, d, 0)
+        if nb < 0:
+            _lib.check(int(nb), "rgcn_highway_workspace_bytes")
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_highway_forward(_ptr(c1), _ptr(c2), _ptr(W), _ptr(b), V, d, _ptr(out), _ptr(gate), _ptr(ws),
+                                      ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_highway_forward")
+        ctx.save_for_backward(c1, c2, W, gate)
+        return out
+
+    @staticmethod
+    def backward(ctx, dOut):
+        lib = _lib.load()
+        c1, c2, W, gate = ctx.saved_tensors
+        V, d = c1.shape
+        dOut = dOut.contiguous()
+        _check_cuda_f32("dOut", dOut, (V, d))
+        dev = c1.device
+        dc1, dc2, dW = torch.empty_like(c1), torch.empty_like(c2), torch.empty_like(W)
+        db = torch.empty(d, dtype=torch.float32, device=dev)
+        nb = lib.rgcn_highway_workspace_bytes(V, d, 1)
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_highway_backward(_ptr(c1), _ptr(c2), _ptr(W), _ptr(gate), _ptr(dOut), V, d, _ptr(dc1),
+                                       _ptr(dc2), _ptr(dW), _ptr(db), _ptr(ws), ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_highway_backward")
+        return dc1, dc2, dW, db
+
+
+def highway(c1, c2, W, b):
+    """Highway skip connection (extras/highway_layer.py:14-38): g = sigmoid(c2 @ W + b), out = g * c1 + (1 - g) * c2,
+    with c1 the wrapped layer's output and c2 its input.  One library call each way; differentiable in all four."""
+    return _HighwayFn.apply(c1, c2, W, b)
+
+
 def _triple_forward(ctx, entry, codes, rel, X, Y):
     """Forward of a triple scorer entry point with the distmult_forward argument list."""
     lib = _lib.load()

@@ -1,7 +1,8 @@
 """Secondary measurements (not the headline bench): DistMult and ComplEx scorer fwd/bwd bandwidth and fused
 ranking, basis layer
 (WN18 shape, BASELINE configs[2]; shipped gcn_basis.exp shape), block layer train-step graph, and the one-hot
-(UseInputTransform=No) first basis layer at the same shapes next to the feature-input basis layer."""
+(UseInputTransform=No) first basis layer at the same shapes next to the feature-input basis layer, and the highway
+skip connection next to the plain GEMM of its shape."""
 import json
 import subprocess
 import sys
@@ -211,4 +212,61 @@ onehot_case("fb15k237_onehot_B5_d500 (gcn_basis.exp, UseInputTransform=No)", 145
 onehot_case("fb15k237_onehot_B5_d500_trainstep_E15000", 14541, 237, 15000, 500, 5)
 layer_case("fb15k237_block_trainstep_E15000", 14541, 237, 15000, 500, 100, "block", True)
 layer_case("fb15k_block_B100_d500 (BASELINE configs[3] shape, 1 GPU)", 14951, 1345, 483142, 500, 100, "block", True)
+
+
+# ---- highway skip connection (SkipConnections=Highway) next to the plain 3xTF32 GEMM of the same [V,d]x[d,d] shape ----
+def highway_case(name, V, d):
+    """ops.highway forward (gate GEMM + blend epilogue) and forward+backward (prologue, dc2 += dz W^T, dW = c2^T dz),
+    alternating with rgcn_gemm_tf32x3 (C = A W) in the same run.  Algorithmic bytes: forward reads c1, c2 and writes
+    out, g (4 [V, d] streams); backward reads c1, c2, g, dOut and writes dc1, dc2 (6 streams).  Flops: 2 V d^2 forward,
+    4 V d^2 backward.  Share of peak: the larger of bytes / 3.35 TB/s and flops / (495 / 3) TFLOP/s (three TF32 MMAs
+    per product) over the measured time."""
+    c1 = torch.randn(V, d, device=dev, generator=g).requires_grad_(True)
+    c2 = torch.randn(V, d, device=dev, generator=g).requires_grad_(True)
+    W = (torch.randn(d, d, device=dev, generator=g) / np.sqrt(d)).requires_grad_(True)
+    b = torch.ones(d, device=dev).requires_grad_(True)
+    dOut = torch.randn(V, d, device=dev, generator=g)
+    C = torch.empty(V, d, device=dev)
+    A, Wd = c2.detach(), W.detach()
+
+    def step():
+        for t in (c1, c2, W, b):
+            t.grad = None
+        ops.highway(c1, c2, W, b).backward(dOut)
+
+    def fwd():
+        with torch.no_grad():
+            ops.highway(c1, c2, W, b)
+    gemm = lambda: ops.gemm_tf32x3(A, Wd, out=C)
+    ms = {"gemm": [], "fwd": [], "fwd_bwd": []}
+    for _ in range(3):                      # alternate, so that all three see the same card state
+        ms["gemm"].append(timeit(gemm, n=10))
+        ms["fwd"].append(timeit(fwd, n=10))
+        ms["fwd_bwd"].append(timeit(step, n=5))
+    t_g, t_f, t_fb = (float(np.median(ms[k])) for k in ("gemm", "fwd", "fwd_bwd"))
+    _lib.profile_enable(True)
+    acc = {}
+    for _ in range(3):
+        flush.zero_()
+        step()
+        torch.cuda.synchronize()
+        for nm, v in _lib.profile_read():
+            acc[nm] = acc.get(nm, 0.0) + v / 3
+    _lib.profile_enable(False)
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                          capture_output=True, text=True).stdout.strip()
+    by_f, by_b = 4 * V * d * 4, 6 * V * d * 4
+    fl_f, fl_b = 2 * V * d * d, 4 * V * d * d
+    bound = lambda by, fl: max(by / 3.35e12, fl / 165e12) * 1e3       # ms
+    out[name] = {"V": V, "d": d, "gpu": card, "gemm_ms": t_g, "fwd_ms": t_f, "fwd_bwd_ms": t_fb,
+                 "runs_ms": ms, "fwd_over_gemm": t_f / t_g, "fwd_bwd_over_gemm": t_fb / t_g,
+                 "fwd_bytes_algorithmic": by_f, "bwd_bytes_algorithmic": by_b, "fwd_flops": fl_f, "bwd_flops": fl_b,
+                 "fwd_GBps_algorithmic": by_f / t_f / 1e6, "fwd_TFLOPs": fl_f / t_f / 1e9,
+                 "share_of_peak": {"fwd": bound(by_f, fl_f) / t_f, "bwd": bound(by_b, fl_b) / max(t_fb - t_f, 1e-6)},
+                 "stages_ms": {k: round(v, 4) for k, v in acc.items()}}
+    del c1, c2, W, b, dOut, C, A, Wd
+
+
+highway_case("highway_fb15k237_V14541_d500", 14541, 500)
+highway_case("highway_V2M_d512", 2_000_000, 512)
 print(json.dumps(out, indent=1))
