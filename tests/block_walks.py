@@ -168,10 +168,11 @@ def table_kernels():
     return frozenset().union(*(r.kernels for r in ROWS))
 
 
-def canonical(name):
-    """`k_block_*<...>` of a demangled kernel name, in the table's spelling: cu++filt writes `<(int)8, (bool)0>`,
-    the CUDA profiler `<8, false>`.  None when the name is not a block-layer kernel."""
-    m = re.search(r"\b(k_block_\w+)(<[^<>]*>)?", name)
+def canonical(name, prefix="k_block_"):
+    """`<prefix>*<...>` of a demangled kernel name, in the table's spelling: cu++filt writes `<(int)8, (bool)0>`,
+    the CUDA profiler `<8, false>`.  None when the name is not a kernel of that family (default: the block
+    layer's)."""
+    m = re.search(r"\b(%s\w+)(<[^<>]*>)?" % re.escape(prefix), name)
     if not m:
         return None
     if not m.group(2):

@@ -12,12 +12,15 @@ import block_walks as bw
 from relationprediction_b200 import _lib
 
 
-def _library_kernels():
+def _library_kernels(raw=False):
+    """canonical `k_block_*` names of the kernels in the library's SASS (raw=True: every demangled kernel name)"""
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, check=True).stdout
     mangled = [f.split("\n", 1)[0].strip() for f in sass.split("Function : ")[1:]]
     names = subprocess.run(["cu++filt"], input="\n".join(mangled) + "\n", capture_output=True, text=True,
                            check=True).stdout.splitlines()
     assert len(names) == len(mangled)
+    if raw:
+        return names
     return {c for c in map(bw.canonical, names) if c is not None}
 
 
