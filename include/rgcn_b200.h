@@ -310,6 +310,38 @@ int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int32_t B, cons
                                float* dCb, float* dWself, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Basis layer with per-channel sigmoid coefficients (DiagonalCoefficients=Yes, "BasisGcnTimesDiag",
+ * encoders/message_gcns/gcn_basis_times_diag.py with message_gcn.py:49-79), feature input:
+ *
+ *   P_dir  = H @ V_dir.reshape(d, B*d)                                   ([V_src, B, d] per direction)
+ *   m      = sum_b sigmoid(C_dir[r_m,b,:]) * P_dir[u_m,b,:]              (per output channel)
+ *   out    = act( A_f m_f + A_b m_b + dropout(H @ W_self) + b )
+ *
+ * Vf, Vb : [d, B, d];  Cf, Cb : [R, B, d];  Wself : [d, d];  b, db : [d].  `saved` (float [V_src, 2*B*d]) receives
+ * P_f | P_b per row and must be handed unchanged to backward.
+ * Backward:  G = dOut * relu'(out),  dS = G * mask / keep,  dWself = H^T dS,  db = column sums of G,
+ *            dP_dir[u,b,:] = sum_{m from u} norm_m sigmoid(C[r_m,b,:]) * G[v_m,:],  dV_dir = H^T dP_dir,
+ *            dH = dS W_self^T + sum_dir dP_dir V_dir^T,
+ *            dC_dir[r,b,:] = s (1 - s) * sum_{m: r_m = r} norm_m P_dir[u_m,b,:] * G[v_m,:]   (s = sigmoid(C)).
+ * Every output is overwritten.  The forward walks the destination-major CSR view, the backward both CSR and the
+ * weight-id-major views: a graph prepared without all of them (graph_views != 3) is RGCN_ERR_INVALID.
+ * Arguments are checked before any device work: null pointers, d % 4 != 0, B < 1 or keep <= 0 are RGCN_ERR_INVALID,
+ * a short workspace RGCN_ERR_WORKSPACE; a host-only graph is RGCN_ERR_NODEVICE.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_basis_diagcoef_workspace_bytes(const rgcn_graph_t* g, int32_t d, int32_t B, int backward);
+
+int rgcn_basis_diagcoef_forward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* H, const float* Vf,
+                                const float* Vb, const float* Cf, const float* Cb, const float* Wself, const float* b,
+                                const uint8_t* drop_mask, float keep, int relu, float* out, float* saved,
+                                void* workspace, int64_t workspace_bytes, void* stream);
+
+int rgcn_basis_diagcoef_backward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* H, const float* Vf,
+                                 const float* Vb, const float* Cf, const float* Cb, const float* Wself,
+                                 const uint8_t* drop_mask, float keep, int relu, const float* out, const float* saved,
+                                 const float* dOut, float* dH, float* dVf, float* dVb, float* dCf, float* dCb,
+                                 float* dWself, float* db, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Highway skip connection between R-GCN layers (SkipConnections=Highway, model_builder.py:304-305;
  * extras/highway_layer.py:14-38).  c1 = the wrapped layer's output, c2 = the layer's input:
  *

@@ -21,6 +21,7 @@ EXPORTED_SYMBOLS = [
     "rgcn_block_aggregate_workspace_bytes", "rgcn_block_aggregate", "rgcn_block_aggregate_backward", "rgcn_rows_add", "rgcn_rows_gather", "rgcn_relu_backward",
     "rgcn_basis_workspace_bytes", "rgcn_basis_forward", "rgcn_basis_backward",
     "rgcn_basis_onehot_workspace_bytes", "rgcn_basis_onehot_forward", "rgcn_basis_onehot_backward",
+    "rgcn_basis_diagcoef_workspace_bytes", "rgcn_basis_diagcoef_forward", "rgcn_basis_diagcoef_backward",
     "rgcn_highway_workspace_bytes", "rgcn_highway_forward", "rgcn_highway_backward",
     "distmult_forward", "distmult_backward", "distmult_rank_workspace_bytes", "distmult_rank",
     "distmult_backward_slices", "rgcn_block_slice_sumsq_workspace_bytes", "rgcn_block_slice_sumsq",
@@ -129,6 +130,14 @@ def _declare(lib):
     lib.rgcn_basis_onehot_backward.restype = c_int
     lib.rgcn_basis_onehot_backward.argtypes = [vp, c_int32, c_int32, vp, vp, vp, vp, vp, c_float, c_int, vp, vp, vp,
                                                vp, vp, vp, vp, vp, c_int64, vp]
+    lib.rgcn_basis_diagcoef_workspace_bytes.restype = c_int64
+    lib.rgcn_basis_diagcoef_workspace_bytes.argtypes = [vp, c_int32, c_int32, c_int]
+    lib.rgcn_basis_diagcoef_forward.restype = c_int
+    lib.rgcn_basis_diagcoef_forward.argtypes = [vp, c_int32, c_int32, vp, vp, vp, vp, vp, vp, vp, vp, c_float, c_int,
+                                                vp, vp, vp, c_int64, vp]
+    lib.rgcn_basis_diagcoef_backward.restype = c_int
+    lib.rgcn_basis_diagcoef_backward.argtypes = [vp, c_int32, c_int32, vp, vp, vp, vp, vp, vp, vp, c_float, c_int,
+                                                 vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, c_int64, vp]
     lib.rgcn_highway_workspace_bytes.restype = c_int64
     lib.rgcn_highway_workspace_bytes.argtypes = [c_int64, c_int32, c_int]
     lib.rgcn_highway_forward.restype = c_int

@@ -1,7 +1,8 @@
 """Name= -> component chain factory (reference: common/model_builder.py:26-184, :273-319).
 
 Only the branches on the accelerated path are built: encoders `gcn_basis` (BasisGcn, or ConcatGcn
-when Concatenation=Yes; with UseInputTransform=No layer 0 is a one-hot BasisGcn; SkipConnections=Highway wraps every
+when Concatenation=Yes, BasisGcnTimesDiag when DiagonalCoefficients=Yes; with UseInputTransform=No layer 0 is a one-hot
+BasisGcn; SkipConnections=Highway wraps every
 feature-input layer in a HighwayLayer) and `embedding`; decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag
@@ -9,6 +10,7 @@ from ..decoders.complex import Complex
 from ..encoders.affine_transform import AffineTransform
 from ..encoders.message_gcns.gcn_basis import BasisGcn
 from ..encoders.message_gcns.gcn_basis_concat import ConcatGcn
+from ..encoders.message_gcns.gcn_basis_times_diag import BasisGcnTimesDiag
 from ..encoders.relation_embedding import RelationEmbedding
 from ..extras.graph_representations import Representation
 from ..extras.highway_layer import HighwayLayer
@@ -52,9 +54,19 @@ def build_encoder(encoder_settings, triples):
 
 
 def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
+    # the reference's layer precedence (model_builder.py:285-294): AddDiagonal > DiagonalCoefficients > StoreEdgeData
+    # > Concatenation
+    diagonal_coefficients = False
     for flag in ('AddDiagonal', 'DiagonalCoefficients', 'StoreEdgeData'):
-        if _flag(encoder_settings, flag) == "Yes":
-            raise NotImplementedError("%s=Yes selects an ablation variant outside the accelerated path" % flag)
+        if _flag(encoder_settings, flag) != "Yes":
+            continue
+        if flag == 'DiagonalCoefficients' and _flag(encoder_settings, 'UseInputTransform') != "No":
+            diagonal_coefficients = True
+            break
+        if flag == 'DiagonalCoefficients':
+            raise NotImplementedError("DiagonalCoefficients=Yes with UseInputTransform=No: the featureless first "
+                                      "layer would need its own per-channel push kernel, which is not built")
+        raise NotImplementedError("%s=Yes selects an ablation variant outside the accelerated path" % flag)
     skip = _flag(encoder_settings, 'SkipConnections', 'None')
     if skip not in ('None', 'Residual', 'Highway'):
         raise NotImplementedError("SkipConnections=%s is not a reference option" % skip)
@@ -65,7 +77,10 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
         raise NotImplementedError("SkipConnections=Highway with UseInputTransform=No: the reference's highway gate "
                                   "is dead there (its carry input is the layer's own output through the shared "
                                   "MessageGcn cache), so this combination is not built")
-    model = ConcatGcn if _flag(encoder_settings, 'Concatenation') == "Yes" else BasisGcn
+    if diagonal_coefficients:
+        model = BasisGcnTimesDiag
+    else:
+        model = ConcatGcn if _flag(encoder_settings, 'Concatenation') == "Yes" else BasisGcn
     for layer in range(layers):
         use_nonlinearity = layer < layers - 1  # the last layer is linear (model_builder.py:275)
         # only layer 0 of a featureless encoder reads one-hot input (model_builder.py:277-283)

@@ -897,6 +897,157 @@ extern "C" int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int3
 }
 
 // ------------------------------------------------------------------------------------------------
+// Basis layer with per-channel sigmoid coefficients (DiagonalCoefficients=Yes, basis_diagcoef.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int64_t rgcn_basis_diagcoef_workspace_bytes(const rgcn_graph_t* g, int32_t d, int32_t B, int backward) {
+  if (!g || d <= 0 || B <= 0) {
+    rgcn_set_error("rgcn_basis_diagcoef_workspace_bytes: bad arguments");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t dB = (int64_t)d * B;
+  int64_t bytes = align_up((int64_t)g->n_relw * dB * 4);  // sigmoid(C) table
+  bytes += align_up((int64_t)2 * d * dB * 4);              // hi/lo split of the GEMM B operands
+  if (backward) {
+    bytes += 2 * align_up((int64_t)g->V_dst * d * 4);      // G, dS
+    bytes += align_up((int64_t)g->V_src * 2 * dB * 4);     // dP (planar, both directions)
+  }
+  return bytes + 256;
+}
+
+// shape, pointer and workspace checks first, then the graph (device, views) -- nothing touches the device before
+static int diagcoef_graph_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
+  int rc = layer_checks(g, d, B, who);
+  if (rc) return rc;
+  return need_views(g, true, true, who);
+}
+
+extern "C" int rgcn_basis_diagcoef_forward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* H,
+                                           const float* Vf, const float* Vb, const float* Cf, const float* Cb,
+                                           const float* Wself, const float* b, const uint8_t* drop_mask, float keep,
+                                           int relu, float* out, float* saved, void* workspace,
+                                           int64_t workspace_bytes, void* stream) {
+  int rc = onehot_shape_checks(g, d, B, "rgcn_basis_diagcoef_forward");
+  if (rc) return rc;
+  if (!H || !Vf || !Vb || !Cf || !Cb || !Wself || !b || !out || !saved || !workspace || keep <= 0.f) {
+    rgcn_set_error("rgcn_basis_diagcoef_forward: null pointer or keep <= 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_basis_diagcoef_workspace_bytes(g, d, B, 0)) {
+    rgcn_set_error("rgcn_basis_diagcoef_forward: workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = diagcoef_graph_checks(g, d, B, "rgcn_basis_diagcoef_forward");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
+  if (rc) return rc;
+  const int R = g->n_relw / 2;
+  const int64_t dB = (int64_t)d * B;
+  Carver ws(workspace, workspace_bytes);
+  float* sig = ws.take<float>((int64_t)g->n_relw * dB);
+  float* split_ws = ws.take<float>((int64_t)2 * d * dB);
+  MARK("start");
+  rc = launch_diagcoef_sigmoid(Cf, Cb, (int64_t)R * dB, sig, st);
+  if (rc) return rc;
+  // saved = P: row u holds P_f[u] | P_b[u]  (P_dir = H V_dir.reshape(d, B*d), gcn_basis_times_diag.py:61-72)
+  rc = gemm_any(st, split_ws, false, false, g->V_src, dB, d, H, d, Vf, dB, 0.f, saved, 2 * dB);
+  if (!rc) rc = gemm_any(st, split_ws, false, false, g->V_src, dB, d, H, d, Vb, dB, 0.f, saved + dB, 2 * dB);
+  if (rc) return rc;
+  MARK("diagcoef_gemms_P");
+  rc = gemm_any(st, split_ws, false, false, g->V_dst, d, d, H, d, Wself, d, 0.f, out, d);
+  if (!rc) rc = launch_mask_relu(out, drop_mask, 1.0f / keep, 0, (int64_t)g->V_dst * d, st);
+  if (rc) return rc;
+  MARK("gemm_self_loop");
+  rc = launch_diagcoef_fwd(g->by_dst.d_items, (int)g->by_dst.n_items, g->by_dst.d_nbr, g->by_dst.d_relw,
+                           g->by_dst.d_norm, saved, sig, B, d, g->n_relw, out, st);
+  if (rc) return rc;
+  MARK("diagcoef_walk_fwd");
+  rc = launch_diagcoef_bias_act(out, b, g->V_dst, d, relu, st);
+  MARK("bias_act_epilogue");
+  return rc;
+}
+
+extern "C" int rgcn_basis_diagcoef_backward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* H,
+                                            const float* Vf, const float* Vb, const float* Cf, const float* Cb,
+                                            const float* Wself, const uint8_t* drop_mask, float keep, int relu,
+                                            const float* out, const float* saved, const float* dOut, float* dH,
+                                            float* dVf, float* dVb, float* dCf, float* dCb, float* dWself, float* db,
+                                            void* workspace, int64_t workspace_bytes, void* stream) {
+  int rc = onehot_shape_checks(g, d, B, "rgcn_basis_diagcoef_backward");
+  if (rc) return rc;
+  if (!H || !Vf || !Vb || !Cf || !Cb || !Wself || !saved || !dOut || !dH || !dVf || !dVb || !dCf || !dCb ||
+      !dWself || !db || !workspace || (relu && !out) || keep <= 0.f) {
+    rgcn_set_error("rgcn_basis_diagcoef_backward: null pointer or keep <= 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_basis_diagcoef_workspace_bytes(g, d, B, 1)) {
+    rgcn_set_error("rgcn_basis_diagcoef_backward: workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = diagcoef_graph_checks(g, d, B, "rgcn_basis_diagcoef_backward");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
+  if (rc) return rc;
+  const int R = g->n_relw / 2;
+  const int64_t dB = (int64_t)d * B;
+  Carver ws(workspace, workspace_bytes);
+  float* sig = ws.take<float>((int64_t)g->n_relw * dB);
+  float* split_ws = ws.take<float>((int64_t)2 * d * dB);
+  float* G = ws.take<float>((int64_t)g->V_dst * d);
+  float* dS = ws.take<float>((int64_t)g->V_dst * d);
+  float* dP = ws.take<float>((int64_t)g->V_src * 2 * dB);
+  if (!drop_mask) dS = G;
+
+  MARK("start");
+  rc = launch_diagcoef_sigmoid(Cf, Cb, (int64_t)R * dB, sig, st);
+  if (rc) return rc;
+  // G = dOut * relu'(out);  dS = G * mask / keep   (dropout is on the self loop only)
+  if (!relu && !drop_mask) {
+    G = dS = const_cast<float*>(dOut);
+  } else {
+    rc = launch_grad_prologue(dOut, out, drop_mask, 1.0f / keep, relu, (int64_t)g->V_dst * d, G, dS, st);
+    if (rc) return rc;
+  }
+  rc = launch_diagcoef_colsum(G, g->V_dst, d, db, st);
+  if (rc) return rc;
+  MARK("grad_prologue_db");
+  rc = gemm_any(st, split_ws, true, false, d, d, g->V_dst, H, d, dS, d, 0.f, dWself, d);
+  if (rc) return rc;
+  rc = gemm_any(st, split_ws, false, true, g->V_dst, d, d, dS, d, Wself, d, 0.f, dH, d);
+  if (rc) return rc;
+  if (g->V_src > g->V_dst) {
+    rc = rgcn_check_cuda(cudaMemsetAsync(dH + (size_t)g->V_dst * d, 0,
+                                         (size_t)(g->V_src - g->V_dst) * d * sizeof(float), st),
+                         "memset(dH halo)");
+    if (rc) return rc;
+  }
+  MARK("diagcoef_self_loop_bwd");
+  // dP[u][dir][b][:] = sum_{m from u} norm_m sig[relw_m,b,:] G[dst_m,:]
+  rc = launch_zero_rows(dP, 2 * dB, g->by_src.d_split_rows, (int)g->by_src.n_split, st);
+  if (!rc)
+    rc = launch_diagcoef_dp(g->by_src.d_items, (int)g->by_src.n_items, g->by_src.d_nbr, g->by_src.d_relw,
+                            g->by_src.d_norm, G, sig, B, d, g->n_relw, dP, st);
+  if (rc) return rc;
+  MARK("diagcoef_walk_dP");
+  // dV_dir.reshape(d, B*d) = H^T dP_dir;  dH += dP_dir V_dir.reshape(d, B*d)^T
+  rc = gemm_any(st, split_ws, true, false, d, dB, g->V_src, H, d, dP, 2 * dB, 0.f, dVf, dB);
+  if (!rc) rc = gemm_any(st, split_ws, true, false, d, dB, g->V_src, H, d, dP + dB, 2 * dB, 0.f, dVb, dB);
+  if (!rc) rc = gemm_any(st, split_ws, false, true, g->V_src, d, dB, dP, 2 * dB, Vf, dB, 1.f, dH, d);
+  if (!rc) rc = gemm_any(st, split_ws, false, true, g->V_src, d, dB, dP + dB, 2 * dB, Vb, dB, 1.f, dH, d);
+  if (rc) return rc;
+  MARK("diagcoef_gemms_dV_dH");
+  // dC_dir[w][b][:] = sig' * sum_{m: relw_m = w} norm_m P[src_m][dir][b][:] G[dst_m,:]
+  rc = rgcn_check_cuda(cudaMemsetAsync(dCf, 0, (size_t)R * dB * 4, st), "memset(dCf)");
+  if (!rc) rc = rgcn_check_cuda(cudaMemsetAsync(dCb, 0, (size_t)R * dB * 4, st), "memset(dCb)");
+  if (!rc)
+    rc = launch_diagcoef_dc(g->by_rel_src.d_items, (int)g->by_rel_src.n_items, g->by_rel_src.d_row,
+                            g->by_rel_src.d_nbr, g->by_rel_src.d_norm, saved, G, sig, B, d, g->n_relw, dCf, dCb, st);
+  MARK("diagcoef_walk_dC");
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Highway skip connection (extras/highway_layer.py): one gate GEMM with the blend epilogue forward; an elementwise
 // prologue and two GEMMs backward
 // ------------------------------------------------------------------------------------------------

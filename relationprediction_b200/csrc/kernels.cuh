@@ -82,6 +82,26 @@ int launch_basis_onehot_push(const WorkItem* items, int n_items, const int32_t* 
                              const float* norm, const float* Wf, const float* Wb, const float* C, int B, int d,
                              int n_relw, float* out, cudaStream_t st);
 
+// basis_diagcoef.cu -- basis layer with per-channel sigmoid coefficients (gcn_basis_times_diag.py).  sig is the
+// [n_relw][B][d] table sigmoid([Cf; Cb]); P the [V_src][2][B][d] transformed rows H [V_f | V_b].
+int launch_diagcoef_sigmoid(const float* Cf, const float* Cb, int64_t n_half, float* sig, cudaStream_t st);
+//   out[dst_m,:] += norm_m * sum_b sig[relw_m,b,:] (.) P[src_m][dir][b][:]      (destination-major view)
+int launch_diagcoef_fwd(const WorkItem* items, int n_items, const int32_t* nbr, const int32_t* relw, const float* norm,
+                        const float* P, const float* sig, int B, int d, int n_relw, float* out, cudaStream_t st);
+// out = act(out + bias), bias [d]
+int launch_diagcoef_bias_act(float* out, const float* bias, int64_t rows, int d, int relu, cudaStream_t st);
+// db = column sums of G [rows, d] (db is overwritten)
+int launch_diagcoef_colsum(const float* G, int64_t rows, int d, float* db, cudaStream_t st);
+//   dP[u][dir][b][:] = sum_{m: src_m = u, dir} norm_m sig[relw_m,b,:] (.) G[dst_m,:]   (source-major view; rows
+//   without messages in a direction are written as zeros, split rows must be zeroed first)
+int launch_diagcoef_dp(const WorkItem* items, int n_items, const int32_t* nbr, const int32_t* relw, const float* norm,
+                       const float* G, const float* sig, int B, int d, int n_relw, float* dP, cudaStream_t st);
+//   dC_dir[w][b][:] += sig (1 - sig) (.) sum_{m: relw_m = w} norm_m P[src_m][dir][b][:] (.) G[dst_m,:]
+//   (weight-id-major view with rows = sources; dCf / dCb zeroed by the caller)
+int launch_diagcoef_dc(const WorkItem* items, int n_items, const int32_t* r_row, const int32_t* r_nbr,
+                       const float* r_norm, const float* P, const float* G, const float* sig, int B, int d, int n_relw,
+                       float* dCf, float* dCb, cudaStream_t st);
+
 // Basis coefficient gradient (destination major):
 //   dC[w][b] += sum_{m into row, relw_m = w} norm_m * < H[src_m,:], dAgg[row][dir][:, b] >
 int launch_basis_dc(const AggLaunch& a, const float* dAgg, int B, int n_relw, float* dC,

@@ -373,6 +373,70 @@ def basis_onehot_layer(W_forward, W_backward, C_forward, C_backward, W_self, gra
                                      relu)
 
 
+class _BasisDiagcoefLayerFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, H, Vf, Vb, Cf, Cb, Wself, b, graph, drop_mask, keep, relu):
+        lib = _lib.load()
+        if not (isinstance(Cf, torch.Tensor) and Cf.dim() == 3):
+            raise _lib.RgcnError("C_forward must be a [R, B, d] tensor")
+        d = H.shape[1]
+        R = graph.n_relw // 2
+        B = Cf.shape[1]
+        _check_cuda_f32("H", H, (graph.V_src, d))
+        _check_cuda_f32("W_forward", Vf, (d, B, d))
+        _check_cuda_f32("W_backward", Vb, (d, B, d))
+        _check_cuda_f32("C_forward", Cf, (R, B, d))
+        _check_cuda_f32("C_backward", Cb, (R, B, d))
+        _check_cuda_f32("W_self", Wself, (d, d))
+        _check_cuda_f32("b", b, (d,))
+        mask = _mask_arg(drop_mask, graph.V_dst, d)
+        dev = H.device
+        out = torch.empty(graph.V_dst, d, dtype=torch.float32, device=dev)
+        saved = torch.empty(graph.V_src, 2 * B * d, dtype=torch.float32, device=dev)
+        nb = lib.rgcn_basis_diagcoef_workspace_bytes(graph.handle, d, B, 0)
+        if nb < 0:
+            _lib.check(int(nb), "rgcn_basis_diagcoef_workspace_bytes")
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_basis_diagcoef_forward(graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf), _ptr(Cb),
+                                             _ptr(Wself), _ptr(b), _ptr(mask), float(keep), int(bool(relu)), _ptr(out),
+                                             _ptr(saved), _ptr(ws), ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_basis_diagcoef_forward")
+        ctx.graph, ctx.keep, ctx.relu, ctx.mask = graph, float(keep), bool(relu), mask
+        ctx.save_for_backward(H, Vf, Vb, Cf, Cb, Wself, out, saved)
+        return out
+
+    @staticmethod
+    def backward(ctx, dOut):
+        lib = _lib.load()
+        H, Vf, Vb, Cf, Cb, Wself, out, saved = ctx.saved_tensors
+        graph = ctx.graph
+        d, B = H.shape[1], Cf.shape[1]
+        dOut = dOut.contiguous()
+        _check_cuda_f32("dOut", dOut, (graph.V_dst, d))
+        dev = H.device
+        dH = torch.empty_like(H)
+        dVf, dVb = torch.empty_like(Vf), torch.empty_like(Vb)
+        dCf, dCb, dWself = torch.empty_like(Cf), torch.empty_like(Cb), torch.empty_like(Wself)
+        db = torch.empty(d, dtype=torch.float32, device=dev)
+        nb = lib.rgcn_basis_diagcoef_workspace_bytes(graph.handle, d, B, 1)
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_basis_diagcoef_backward(graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf), _ptr(Cb),
+                                              _ptr(Wself), _ptr(ctx.mask), ctx.keep, int(ctx.relu), _ptr(out),
+                                              _ptr(saved), _ptr(dOut), _ptr(dH), _ptr(dVf), _ptr(dVb), _ptr(dCf),
+                                              _ptr(dCb), _ptr(dWself), _ptr(db), _ptr(ws), ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_basis_diagcoef_backward")
+        return dH, dVf, dVb, dCf, dCb, dWself, db, None, None, None, None
+
+
+def basis_diagcoef_layer(H, W_forward, W_backward, C_forward, C_backward, W_self, b, graph, drop_mask=None, keep=1.0,
+                         relu=True):
+    """Basis R-GCN layer with per-channel sigmoid coefficients (BasisGcnTimesDiag, gcn_basis_times_diag.py, feature
+    input): m = sum_b sigmoid(C_dir[r, b, :]) * (H[s] @ V_dir[:, b, :]), out = act(A_f m_f + A_b m_b +
+    dropout(H @ W_self) + b).  C tables are [R, B, d]; differentiable in H and every weight, b included."""
+    return _BasisDiagcoefLayerFn.apply(H, W_forward, W_backward, C_forward, C_backward, W_self, b, graph, drop_mask,
+                                       keep, relu)
+
+
 class _HighwayFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, c1, c2, W, b):

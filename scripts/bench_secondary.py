@@ -1,7 +1,8 @@
 """Secondary measurements (not the headline bench): DistMult and ComplEx scorer fwd/bwd bandwidth and fused
 ranking, basis layer
 (WN18 shape, BASELINE configs[2]; shipped gcn_basis.exp shape), block layer train-step graph, and the one-hot
-(UseInputTransform=No) first basis layer at the same shapes next to the feature-input basis layer, and the highway
+(UseInputTransform=No) first basis layer and the per-channel-coefficient basis layer (DiagonalCoefficients=Yes) at
+the same shapes next to the feature-input basis layer, and the highway
 skip connection next to the plain GEMM of its shape."""
 import json
 import subprocess
@@ -132,6 +133,13 @@ def layer_case(name, V, R, E, d, B, variant, skewed):
         ws = [(torch.randn(R, B, s, s, device=dev, generator=g) * std).requires_grad_(True) for _ in range(2)]
         ws.append((torch.randn(d, d, device=dev, generator=g) * std).requires_grad_(True))
         f = lambda: ops.block_layer(H, ws[0], ws[1], ws[2], gr, B, None, 1.0, True)
+    elif variant == "times_diag":     # DiagonalCoefficients=Yes: [R, B, d] coefficient tables and a bias
+        std = 3.0 / np.sqrt(2 * d)
+        ws = [(torch.randn(d, B, d, device=dev, generator=g) * std).requires_grad_(True) for _ in range(2)]
+        ws += [torch.randn(R, B, d, device=dev, generator=g).requires_grad_(True) for _ in range(2)]
+        ws.append((torch.randn(d, d, device=dev, generator=g) * std).requires_grad_(True))
+        ws.append(torch.zeros(d, device=dev).requires_grad_(True))
+        f = lambda: ops.basis_diagcoef_layer(H, ws[0], ws[1], ws[2], ws[3], ws[4], ws[5], gr, None, 1.0, True)
     else:
         std = 3.0 / np.sqrt(2 * d)
         ws = [(torch.randn(d, B, d, device=dev, generator=g) * std).requires_grad_(True) for _ in range(2)]
@@ -158,6 +166,13 @@ def layer_case(name, V, R, E, d, B, variant, skewed):
     _lib.profile_enable(False)
     out[name] = {"V": V, "R": R, "E": E, "d": d, "B": B, "variant": variant, "fwd_ms": ms_f, "fwd_bwd_ms": ms,
                  "M_edges_per_s": E / ms / 1e3, "stages_ms": {k: round(v, 4) for k, v in acc.items()}}
+    if variant == "times_diag":
+        # the forward walk gathers one P_dir row (B*d floats) plus its sigmoid row (L2-resident) per message and
+        # reads the index, weight id and norm: M * (4 B d + 12) bytes from memory
+        walk = 2 * E * (4 * B * d + 12)
+        t_walk = acc.get("diagcoef_walk_fwd", 0.0)
+        out[name].update({"gpu": gpu, "fwd_walk_bytes_algorithmic": walk,
+                          "fwd_walk_GBps_algorithmic": walk / t_walk / 1e6 if t_walk > 0 else None})
 
 
 def onehot_case(name, V, R, E, d, B):
@@ -207,6 +222,10 @@ def onehot_case(name, V, R, E, d, B):
 layer_case("wn18_basis_B2_d200 (BASELINE configs[2])", 40943, 18, 141442, 200, 2, "basis", True)
 layer_case("fb15k237_basis_B5_d500 (shipped gcn_basis.exp)", 14541, 237, 272115, 500, 5, "basis", True)
 layer_case("fb15k237_basis_B5_d500_trainstep_E15000", 14541, 237, 15000, 500, 5, "basis", True)
+layer_case("wn18_times_diag_B2_d200 (DiagonalCoefficients=Yes)", 40943, 18, 141442, 200, 2, "times_diag", True)
+layer_case("fb15k237_times_diag_B5_d500 (gcn_basis.exp, DiagonalCoefficients=Yes)", 14541, 237, 272115, 500, 5,
+           "times_diag", True)
+layer_case("fb15k237_times_diag_B5_d500_trainstep_E15000", 14541, 237, 15000, 500, 5, "times_diag", True)
 onehot_case("wn18_onehot_B2_d200 (UseInputTransform=No)", 40943, 18, 141442, 200, 2)
 onehot_case("fb15k237_onehot_B5_d500 (gcn_basis.exp, UseInputTransform=No)", 14541, 237, 272115, 500, 5)
 onehot_case("fb15k237_onehot_B5_d500_trainstep_E15000", 14541, 237, 15000, 500, 5)
