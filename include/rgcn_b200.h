@@ -342,6 +342,36 @@ int rgcn_basis_diagcoef_backward(const rgcn_graph_t* g, int32_t d, int32_t B, co
                                  float* dWself, float* db, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Diagonal R-GCN layer (Name=gcn_diag, "DiagGcn", encoders/message_gcns/gcn_diag.py with message_gcn.py:49-79).
+ * Messages as above (forward s->o with weight id r, backward o->s with weight id r+R), D = [Df; Db]:
+ *
+ *   out[v] = act( sum_{m -> v} norm_m * D[w_m] (.) H[src_m]  +  dropout(H[v] @ W_self)  +  b )
+ *
+ * H : [V_src, d] (V_src >= V_dst: rows [V_dst, V_src) are halo rows that only send);  Df, Db : [R, d] with
+ * n_relw == 2R;  Wself : [d, d];  b, db : [d];  out, dOut : [V_dst, d].  d % 4 == 0.
+ * Backward:  G = dOut * relu'(out),  dS = G * mask / keep,  db = column sums of G,  dWself = H^T dS,
+ *            dH[u] = (dS W_self^T)[u] + sum_{m from u} norm_m D[w_m] (.) G[dst_m],
+ *            dD[w] = sum_{m: w_m = w} norm_m G[dst_m] (.) H[src_m].
+ * slice_sumsq2 (optional, float[2]; NULL skips it) receives, per direction, the sum of squares of the un-aggregated
+ * per-message gradient slices of Df / Db (what tf.clip_by_global_norm sees through tf.nn.embedding_lookup):
+ *            sum_m norm_m^2 sum_k G[dst_m,k]^2 H[src_m,k]^2.
+ * Every output is overwritten.  The forward walks the destination-major CSR view, the backward the source-major one:
+ * a graph prepared without the CSR views (graph_views == 2) is RGCN_ERR_INVALID.
+ * Arguments are checked before any device work: null pointers, d % 4 != 0 or keep <= 0 are RGCN_ERR_INVALID, a short
+ * workspace RGCN_ERR_WORKSPACE; a host-only graph is RGCN_ERR_NODEVICE.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_diag_workspace_bytes(const rgcn_graph_t* g, int32_t d, int backward);
+
+int rgcn_diag_forward(const rgcn_graph_t* g, int32_t d, const float* H, const float* Df, const float* Db,
+                      const float* Wself, const float* b, const uint8_t* drop_mask, float keep, int relu, float* out,
+                      void* workspace, int64_t workspace_bytes, void* stream);
+
+int rgcn_diag_backward(const rgcn_graph_t* g, int32_t d, const float* H, const float* Df, const float* Db,
+                       const float* Wself, const uint8_t* drop_mask, float keep, int relu, const float* out,
+                       const float* dOut, float* dH, float* dDf, float* dDb, float* dWself, float* db,
+                       float* slice_sumsq2, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Highway skip connection between R-GCN layers (SkipConnections=Highway, model_builder.py:304-305;
  * extras/highway_layer.py:14-38).  c1 = the wrapped layer's output, c2 = the layer's input:
  *

@@ -22,6 +22,7 @@ EXPORTED_SYMBOLS = [
     "rgcn_basis_workspace_bytes", "rgcn_basis_forward", "rgcn_basis_backward",
     "rgcn_basis_onehot_workspace_bytes", "rgcn_basis_onehot_forward", "rgcn_basis_onehot_backward",
     "rgcn_basis_diagcoef_workspace_bytes", "rgcn_basis_diagcoef_forward", "rgcn_basis_diagcoef_backward",
+    "rgcn_diag_workspace_bytes", "rgcn_diag_forward", "rgcn_diag_backward",
     "rgcn_highway_workspace_bytes", "rgcn_highway_forward", "rgcn_highway_backward",
     "distmult_forward", "distmult_backward", "distmult_rank_workspace_bytes", "distmult_rank",
     "distmult_backward_slices", "rgcn_block_slice_sumsq_workspace_bytes", "rgcn_block_slice_sumsq",
@@ -138,6 +139,13 @@ def _declare(lib):
     lib.rgcn_basis_diagcoef_backward.restype = c_int
     lib.rgcn_basis_diagcoef_backward.argtypes = [vp, c_int32, c_int32, vp, vp, vp, vp, vp, vp, vp, c_float, c_int,
                                                  vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, c_int64, vp]
+    lib.rgcn_diag_workspace_bytes.restype = c_int64
+    lib.rgcn_diag_workspace_bytes.argtypes = [vp, c_int32, c_int]
+    lib.rgcn_diag_forward.restype = c_int
+    lib.rgcn_diag_forward.argtypes = [vp, c_int32, vp, vp, vp, vp, vp, vp, c_float, c_int, vp, vp, c_int64, vp]
+    lib.rgcn_diag_backward.restype = c_int
+    lib.rgcn_diag_backward.argtypes = [vp, c_int32, vp, vp, vp, vp, vp, c_float, c_int, vp, vp, vp, vp, vp, vp, vp,
+                                       vp, vp, c_int64, vp]
     lib.rgcn_highway_workspace_bytes.restype = c_int64
     lib.rgcn_highway_workspace_bytes.argtypes = [c_int64, c_int32, c_int]
     lib.rgcn_highway_forward.restype = c_int

@@ -1,6 +1,6 @@
 """Name= -> component chain factory (reference: common/model_builder.py:26-184, :273-319).
 
-Only the branches on the accelerated path are built: encoders `gcn_basis` (BasisGcn, or ConcatGcn
+Only the branches on the accelerated path are built: encoders `gcn_diag` (DiagGcn layers), `gcn_basis` (BasisGcn, or ConcatGcn
 when Concatenation=Yes, BasisGcnTimesDiag when DiagonalCoefficients=Yes; with UseInputTransform=No layer 0 is a one-hot
 BasisGcn; SkipConnections=Highway wraps every
 feature-input layer in a HighwayLayer) and `embedding`; decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
@@ -11,6 +11,7 @@ from ..encoders.affine_transform import AffineTransform
 from ..encoders.message_gcns.gcn_basis import BasisGcn
 from ..encoders.message_gcns.gcn_basis_concat import ConcatGcn
 from ..encoders.message_gcns.gcn_basis_times_diag import BasisGcnTimesDiag
+from ..encoders.message_gcns.gcn_diag import DiagGcn
 from ..encoders.relation_embedding import RelationEmbedding
 from ..extras.graph_representations import Representation
 from ..extras.highway_layer import HighwayLayer
@@ -27,6 +28,28 @@ def build_encoder(encoder_settings, triples):
         embedding = AffineTransform(input_shape, encoder_settings, onehot_input=True, use_bias=False,
                                     use_nonlinearity=False)
         return RelationEmbedding(input_shape, encoder_settings, next_component=embedding)
+
+    if name == "gcn_diag":
+        # model_builder.py:71-119: always an input AffineTransform, then NumberOfLayers DiagGcn layers (the last one
+        # linear), the optional output projection and RelationEmbedding.  The branch reads none of
+        # UseInputTransform, SkipConnections, Concatenation, DiagonalCoefficients, AddDiagonal, StoreEdgeData or
+        # RandomInput, so neither does this one.
+        graph = Representation(triples, encoder_settings)
+        d_int = int(encoder_settings['InternalEncoderDimension'])
+        input_shape = [int(encoder_settings['EntityCount']), d_int]
+        internal_shape = [d_int, d_int]
+        projection_shape = [d_int, int(encoder_settings['CodeDimension'])]
+        relation_shape = [int(encoder_settings['EntityCount']), int(encoder_settings['CodeDimension'])]
+        layers = int(encoder_settings['NumberOfLayers'])
+        encoding = AffineTransform(input_shape, encoder_settings, next_component=graph, onehot_input=True,
+                                   use_bias=True, use_nonlinearity=True)
+        for layer in range(layers):
+            encoding = DiagGcn(internal_shape, encoder_settings, next_component=encoding, onehot_input=False,
+                               use_nonlinearity=layer < layers - 1)
+        if _flag(encoder_settings, 'UseOutputTransform') == "Yes":
+            encoding = AffineTransform(projection_shape, encoder_settings, next_component=encoding,
+                                       onehot_input=False, use_nonlinearity=False, use_bias=True)
+        return RelationEmbedding(relation_shape, encoder_settings, next_component=encoding)
 
     if name == "gcn_basis":
         graph = Representation(triples, encoder_settings)

@@ -1048,6 +1048,133 @@ extern "C" int rgcn_basis_diagcoef_backward(const rgcn_graph_t* g, int32_t d, in
 }
 
 // ------------------------------------------------------------------------------------------------
+// Diagonal R-GCN layer (Name=gcn_diag, gcn_diag.cu)
+// ------------------------------------------------------------------------------------------------
+extern "C" int64_t rgcn_diag_workspace_bytes(const rgcn_graph_t* g, int32_t d, int backward) {
+  if (!g || d <= 0) {
+    rgcn_set_error("rgcn_diag_workspace_bytes: bad arguments");
+    return RGCN_ERR_INVALID;
+  }
+  int64_t bytes = align_up((int64_t)2 * d * d * 4);  // hi/lo split of W_self for the tensor-core GEMM
+  if (!backward) {
+    bytes += align_up(g->by_dst.n_split * d * 4);                    // split-row scratch
+    bytes += align_up(g->by_dst.n_split * slabs_for(d) * 4);         // split-row arrival counters
+  } else {
+    bytes += 2 * align_up((int64_t)g->V_dst * d * 4);                // G, dS
+  }
+  return bytes + 256;
+}
+
+// shape, pointer and workspace checks come first (they need no device), then the graph: device, V_src >= V_dst, CSR
+static int diag_graph_checks(const rgcn_graph_t* g, int32_t d, const char* who) {
+  int rc = layer_checks(g, d, 1, who);
+  if (rc) return rc;
+  return need_views(g, true, false, who);
+}
+
+extern "C" int rgcn_diag_forward(const rgcn_graph_t* g, int32_t d, const float* H, const float* Df, const float* Db,
+                                 const float* Wself, const float* b, const uint8_t* drop_mask, float keep, int relu,
+                                 float* out, void* workspace, int64_t workspace_bytes, void* stream) {
+  int rc = onehot_shape_checks(g, d, 1, "rgcn_diag_forward");
+  if (rc) return rc;
+  if (!H || !Df || !Db || !Wself || !b || !out || !workspace || keep <= 0.f) {
+    rgcn_set_error("rgcn_diag_forward: null pointer or keep <= 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_diag_workspace_bytes(g, d, 0)) {
+    rgcn_set_error("rgcn_diag_forward: workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = diag_graph_checks(g, d, "rgcn_diag_forward");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
+  if (rc) return rc;
+  const int64_t n_split = g->by_dst.n_split;
+  const int slabs = slabs_for(d);
+  Carver ws(workspace, workspace_bytes);
+  float* split_ws = ws.take<float>((int64_t)2 * d * d);
+  float* scratch = ws.take<float>(n_split * d);
+  int* counters = ws.take<int>(n_split * slabs);
+  MARK("start");
+  if (n_split > 0) {
+    rc = rgcn_check_cuda(cudaMemsetAsync(scratch, 0, (char*)(counters + n_split * slabs) - (char*)scratch, st),
+                         "memset(scratch)");
+    if (rc) return rc;
+  }
+  // self-loop term H[0:V_dst] W_self written straight into `out`; the walk applies the dropout mask (gcn_diag.py:39-40)
+  rc = gemm_any(st, split_ws, false, false, g->V_dst, d, d, H, d, Wself, d, 0.f, out, d);
+  if (rc) return rc;
+  MARK("gemm_self_loop");
+  // out[v] = act(dropout(out[v]) + sum_{m into v} norm_m D[relw_m] (.) H[src_m] + b)   (gcn_diag.py:29-58)
+  rc = launch_diaggcn_fwd(g->by_dst.d_items, (int)g->by_dst.n_items, g->by_dst.d_nbr, g->by_dst.d_relw,
+                          g->by_dst.d_norm, H, Df, Db, d, g->n_relw, b, drop_mask, 1.0f / keep, relu,
+                          g->by_dst.d_split_nitems, scratch, counters, out, st);
+  MARK("diag_walk_fwd");
+  return rc;
+}
+
+extern "C" int rgcn_diag_backward(const rgcn_graph_t* g, int32_t d, const float* H, const float* Df, const float* Db,
+                                  const float* Wself, const uint8_t* drop_mask, float keep, int relu, const float* out,
+                                  const float* dOut, float* dH, float* dDf, float* dDb, float* dWself, float* db,
+                                  float* slice_sumsq2, void* workspace, int64_t workspace_bytes, void* stream) {
+  int rc = onehot_shape_checks(g, d, 1, "rgcn_diag_backward");
+  if (rc) return rc;
+  if (!H || !Df || !Db || !Wself || !dOut || !dH || !dDf || !dDb || !dWself || !db || !workspace ||
+      (relu && !out) || keep <= 0.f) {
+    rgcn_set_error("rgcn_diag_backward: null pointer or keep <= 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_diag_workspace_bytes(g, d, 1)) {
+    rgcn_set_error("rgcn_diag_backward: workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = diag_graph_checks(g, d, "rgcn_diag_backward");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
+  if (rc) return rc;
+  const int R = g->n_relw / 2;
+  Carver ws(workspace, workspace_bytes);
+  float* split_ws = ws.take<float>((int64_t)2 * d * d);
+  float* G = ws.take<float>((int64_t)g->V_dst * d);
+  float* dS = ws.take<float>((int64_t)g->V_dst * d);
+  if (!drop_mask) dS = G;
+
+  MARK("start");
+  // G = dOut * relu'(out);  dS = G * mask / keep   (dropout is on the self loop only)
+  if (!relu && !drop_mask) {
+    G = dS = const_cast<float*>(dOut);
+  } else {
+    rc = launch_grad_prologue(dOut, out, drop_mask, 1.0f / keep, relu, (int64_t)g->V_dst * d, G, dS, st);
+    if (rc) return rc;
+  }
+  rc = launch_diagcoef_colsum(G, g->V_dst, d, db, st);
+  if (rc) return rc;
+  MARK("grad_prologue_db");
+  rc = gemm_any(st, split_ws, true, false, d, d, g->V_dst, H, d, dS, d, 0.f, dWself, d);
+  if (rc) return rc;
+  rc = gemm_any(st, split_ws, false, true, g->V_dst, d, d, dS, d, Wself, d, 0.f, dH, d);
+  if (rc) return rc;
+  if (g->V_src > g->V_dst) {
+    rc = rgcn_check_cuda(cudaMemsetAsync(dH + (size_t)g->V_dst * d, 0,
+                                         (size_t)(g->V_src - g->V_dst) * d * sizeof(float), st),
+                         "memset(dH halo)");
+    if (rc) return rc;
+  }
+  MARK("diag_self_loop_bwd");
+  // dH[u] += sum_{m from u} norm_m D[relw_m] (.) G[dst_m];  dD[w] = sum_{m: relw_m = w} norm_m H[src_m] (.) G[dst_m]
+  rc = rgcn_check_cuda(cudaMemsetAsync(dDf, 0, (size_t)R * d * 4, st), "memset(dDf)");
+  if (!rc) rc = rgcn_check_cuda(cudaMemsetAsync(dDb, 0, (size_t)R * d * 4, st), "memset(dDb)");
+  if (!rc && slice_sumsq2) rc = rgcn_check_cuda(cudaMemsetAsync(slice_sumsq2, 0, 2 * 4, st), "memset(sumsq2)");
+  if (!rc)
+    rc = launch_diaggcn_bwd(g->by_src.d_items, (int)g->by_src.n_items, g->by_src.d_nbr, g->by_src.d_relw,
+                            g->by_src.d_norm, G, H, Df, Db, d, g->n_relw, dH, dDf, dDb, slice_sumsq2, st);
+  MARK("diag_walk_bwd");
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Highway skip connection (extras/highway_layer.py): one gate GEMM with the blend epilogue forward; an elementwise
 // prologue and two GEMMs backward
 // ------------------------------------------------------------------------------------------------

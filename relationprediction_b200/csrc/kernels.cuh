@@ -102,6 +102,21 @@ int launch_diagcoef_dc(const WorkItem* items, int n_items, const int32_t* r_row,
                        const float* r_norm, const float* P, const float* G, const float* sig, int B, int d, int n_relw,
                        float* dCf, float* dCb, cudaStream_t st);
 
+// gcn_diag.cu -- diagonal R-GCN layer (gcn_diag.py); D_dir tables [R][d], weight id w reads Df[w] (w < n_relw/2)
+// or Db[w - n_relw/2].  Forward, destination-major view, `out` holding H W_self (unmasked):
+//   out[row] = act( dropout(out[row]) + sum_{m into row} norm_m D[relw_m] (.) H[src_m] + bias )
+// (split rows: scratch [n_split, d] and counters [n_split * slabs] zeroed by the caller)
+int launch_diaggcn_fwd(const WorkItem* items, int n_items, const int32_t* nbr, const int32_t* relw, const float* norm,
+                       const float* H, const float* Df, const float* Db, int d, int n_relw, const float* bias,
+                       const uint8_t* mask, float inv_keep, int relu, const int32_t* split_nitems, float* scratch,
+                       int* counters, float* out, cudaStream_t st);
+// Backward, source-major view (rows = sources u):  dH[u] += sum_{m from u} norm_m D[relw_m] (.) G[dst_m];
+// dD[w] += sum_{m: relw_m = w} norm_m H[src_m] (.) G[dst_m] (dDf / dDb zeroed by the caller); if sumsq2 != null,
+// sumsq2[dir] += sum_m norm_m^2 |H[src_m] (.) G[dst_m]|^2 over the messages of each direction.
+int launch_diaggcn_bwd(const WorkItem* items, int n_items, const int32_t* nbr, const int32_t* relw, const float* norm,
+                       const float* G, const float* H, const float* Df, const float* Db, int d, int n_relw, float* dH,
+                       float* dDf, float* dDb, float* sumsq2, cudaStream_t st);
+
 // Basis coefficient gradient (destination major):
 //   dC[w][b] += sum_{m into row, relw_m = w} norm_m * < H[src_m,:], dAgg[row][dir][:, b] >
 int launch_basis_dc(const AggLaunch& a, const float* dAgg, int B, int n_relw, float* dC,

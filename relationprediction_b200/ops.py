@@ -437,6 +437,67 @@ def basis_diagcoef_layer(H, W_forward, W_backward, C_forward, C_backward, W_self
                                        keep, relu)
 
 
+class _DiagLayerFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, H, Df, Db, Wself, b, graph, drop_mask, keep, relu):
+        lib = _lib.load()
+        if not (isinstance(H, torch.Tensor) and H.dim() == 2):
+            raise _lib.RgcnError("H must be a [V_src, d] tensor")
+        d = H.shape[1]
+        R = graph.n_relw // 2
+        _check_cuda_f32("H", H, (graph.V_src, d))
+        _check_cuda_f32("D_types_forward", Df, (R, d))
+        _check_cuda_f32("D_types_backward", Db, (R, d))
+        _check_cuda_f32("W_self", Wself, (d, d))
+        _check_cuda_f32("b", b, (d,))
+        mask = _mask_arg(drop_mask, graph.V_dst, d)
+        dev = H.device
+        out = torch.empty(graph.V_dst, d, dtype=torch.float32, device=dev)
+        nb = lib.rgcn_diag_workspace_bytes(graph.handle, d, 0)
+        if nb < 0:
+            _lib.check(int(nb), "rgcn_diag_workspace_bytes")
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_diag_forward(graph.handle, d, _ptr(H), _ptr(Df), _ptr(Db), _ptr(Wself), _ptr(b), _ptr(mask),
+                                   float(keep), int(bool(relu)), _ptr(out), _ptr(ws), ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_diag_forward")
+        ctx.graph, ctx.keep, ctx.relu, ctx.mask = graph, float(keep), bool(relu), mask
+        ctx.params = (Df, Db)   # the caller's tensor objects (slice norms are parked on them)
+        ctx.save_for_backward(H, Df, Db, Wself, out)
+        return out
+
+    @staticmethod
+    def backward(ctx, dOut):
+        lib = _lib.load()
+        H, Df, Db, Wself, out = ctx.saved_tensors
+        graph = ctx.graph
+        d = H.shape[1]
+        dOut = dOut.contiguous()
+        _check_cuda_f32("dOut", dOut, (graph.V_dst, d))
+        dev = H.device
+        dH = torch.empty_like(H)
+        dDf, dDb, dWself = torch.empty_like(Df), torch.empty_like(Db), torch.empty_like(Wself)
+        db = torch.empty(d, dtype=torch.float32, device=dev)
+        ss = torch.empty(2, dtype=torch.float32, device=dev) if _SLICE_NORMS else None
+        nb = lib.rgcn_diag_workspace_bytes(graph.handle, d, 1)
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_diag_backward(graph.handle, d, _ptr(H), _ptr(Df), _ptr(Db), _ptr(Wself), _ptr(ctx.mask),
+                                    ctx.keep, int(ctx.relu), _ptr(out), _ptr(dOut), _ptr(dH), _ptr(dDf), _ptr(dDb),
+                                    _ptr(dWself), _ptr(db), _ptr(ss), _ptr(ws), ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_diag_backward")
+        if ss is not None:
+            _add_slice_sumsq(ctx.params[0], ss[0])
+            _add_slice_sumsq(ctx.params[1], ss[1])
+        return dH, dDf, dDb, dWself, db, None, None, None, None
+
+
+def diag_layer(H, D_forward, D_backward, W_self, b, graph, drop_mask=None, keep=1.0, relu=True):
+    """Diagonal R-GCN layer (DiagGcn, gcn_diag.py): a message s -> o of relation r is D_dir[r] * H[s] (element-wise),
+    out = act(A_f m_f + A_b m_b + dropout(H @ W_self) + b).  D tables are [R, d]; differentiable in H and every
+    weight, b included.  With set_slice_norms(True) the backward also parks the IndexedSlices sum of squares of the
+    D gradients on D_forward / D_backward."""
+    return _DiagLayerFn.apply(H, D_forward, D_backward, W_self, b, graph, drop_mask, keep, relu)
+
+
 class _HighwayFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, c1, c2, W, b):

@@ -2,8 +2,9 @@
 ranking, basis layer
 (WN18 shape, BASELINE configs[2]; shipped gcn_basis.exp shape), block layer train-step graph, and the one-hot
 (UseInputTransform=No) first basis layer and the per-channel-coefficient basis layer (DiagonalCoefficients=Yes) at
-the same shapes next to the feature-input basis layer, and the highway
-skip connection next to the plain GEMM of its shape."""
+the same shapes next to the feature-input basis layer, the highway
+skip connection next to the plain GEMM of its shape, and the diagonal R-GCN layer (Name=gcn_diag) next to the basis
+layer and at bench.py's synthetic shape.  `python scripts/bench_secondary.py --gcn-diag` runs only that last section."""
 import json
 import subprocess
 import sys
@@ -37,6 +38,101 @@ def timeit(fn, n=10, warm=3):
 
 
 out = {}
+card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                      capture_output=True, text=True).stdout.strip()
+
+
+# ---- diagonal R-GCN layer (Name=gcn_diag) next to the basis layer, alternated in one run ----
+def gcn_diag_walk_bytes(tr, V, R, d):
+    """Algorithmic bytes of the two message walks (DESIGN.md 3).  Forward: per message the gathered H row and the
+    index, weight id and norm, M (4d + 12), plus the self-loop row read and the output row written, 8 V_dst d.
+    Backward: per message the gathered G row and the same 12 bytes, M (4d + 12), plus H read, dH read and written,
+    12 V_src d, plus one d-wide vector reduction into dD per (source, weight id) run, 4 d each."""
+    t = torch.as_tensor(tr, device=dev).long()
+    s, r, o = t[:, 0], t[:, 1], t[:, 2]
+    runs = torch.unique(torch.cat([s * (2 * R) + r, o * (2 * R) + R + r])).numel()
+    M = 2 * len(tr)
+    return M * (4 * d + 12) + 8 * V * d, M * (4 * d + 12) + 12 * V * d + runs * 4 * d, runs
+
+
+def gcn_diag_case(name, V, R, E, d, B=None, skewed=True, rounds=3):
+    """ops.diag_layer forward and forward + backward (ReLU on, no dropout mask, L2 flushed between calls), alternated
+    `rounds` times with ops.basis_layer at B bases when B is given; medians.  Stages from the library's event marks
+    in a separate profiled pass."""
+    g = torch.Generator(device=dev).manual_seed(0)
+    tr = synthetic_kg(V, R, E, seed=1234, skewed=skewed)
+    _lib.set_option("graph_views", 1)         # the diagonal layer walks the CSR views only
+    try:
+        gr = ops.Graph.from_device_triples(torch.as_tensor(tr, device=dev), V, R)
+    finally:
+        _lib.set_option("graph_views", 3)
+    H = torch.randn(V, d, device=dev, generator=g).requires_grad_(True)
+    dOut = torch.randn(V, d, device=dev, generator=g)
+    std = 3.0 / np.sqrt(2 * d)
+    wd = [torch.randn(R, d, device=dev, generator=g).requires_grad_(True) for _ in range(2)]
+    wd.append((torch.randn(d, d, device=dev, generator=g) * std).requires_grad_(True))
+    wd.append(torch.zeros(d, device=dev).requires_grad_(True))
+    fd = lambda: ops.diag_layer(H, wd[0], wd[1], wd[2], wd[3], gr, None, 1.0, True)
+    fns = {"gcn_diag": fd}
+    if B is not None:
+        gb = ops.Graph.from_device_triples(torch.as_tensor(tr, device=dev), V, R)
+        wb = [(torch.randn(d, B, d, device=dev, generator=g) * std).requires_grad_(True) for _ in range(2)]
+        wb += [torch.randn(R, B, device=dev, generator=g).requires_grad_(True) for _ in range(2)]
+        wb.append((torch.randn(d, d, device=dev, generator=g) * std).requires_grad_(True))
+        fns["basis"] = lambda: ops.basis_layer(H, wb[0], wb[1], wb[2], wb[3], wb[4], gb, None, 1.0, True)
+
+    def step(f):
+        H.grad = None
+        f().backward(dOut)
+
+    def fwd(f):
+        with torch.no_grad():
+            f()
+    ms = {k: {"fwd": [], "fwd_bwd": []} for k in fns}
+    for _ in range(rounds):
+        for k, f in fns.items():
+            ms[k]["fwd"].append(timeit(lambda: fwd(f), n=10))
+            ms[k]["fwd_bwd"].append(timeit(lambda: step(f), n=10))
+    med = {k: {p: float(np.median(v[p])) for p in v} for k, v in ms.items()}
+    _lib.profile_enable(True)
+    acc = {}
+    for _ in range(5):
+        flush.zero_()
+        step(fd)
+        torch.cuda.synchronize()
+        for nm, v in _lib.profile_read():
+            acc[nm] = acc.get(nm, 0.0) + v / 5
+    _lib.profile_enable(False)
+    by_f, by_b, runs = gcn_diag_walk_bytes(tr, V, R, d)
+    t_f, t_b = acc.get("diag_walk_fwd", 0.0), acc.get("diag_walk_bwd", 0.0)
+    res = {"V": V, "R": R, "E": E, "M": 2 * E, "d": d, "gpu": card, "medians_ms": med, "runs_ms": ms,
+           "bwd_source_weight_runs": runs, "fwd_walk_bytes_algorithmic": by_f, "bwd_walk_bytes_algorithmic": by_b,
+           "fwd_walk_TBps": by_f / t_f / 1e9 if t_f > 0 else None,
+           "bwd_walk_TBps": by_b / t_b / 1e9 if t_b > 0 else None,
+           "frac_of_3350_GBps": {"fwd_walk": by_f / t_f / 1e9 / 3.35 if t_f > 0 else None,
+                                 "bwd_walk": by_b / t_b / 1e9 / 3.35 if t_b > 0 else None},
+           "stages_ms": {k: round(v, 4) for k, v in acc.items()}}
+    if B is not None:
+        res["basis_B"] = B
+        res["ratio_to_basis"] = {p: med["gcn_diag"][p] / med["basis"][p] for p in ("fwd", "fwd_bwd")}
+    out[name] = res
+    del H, dOut, wd, fns, gr
+    torch.cuda.empty_cache()
+
+
+def gcn_diag_section():
+    gcn_diag_case("gcn_diag_fb15k237_d500 (vs basis B5)", 14541, 237, 272115, 500, B=5)
+    gcn_diag_case("gcn_diag_fb15k237_d500_trainstep_E15000 (vs basis B5)", 14541, 237, 15000, 500, B=5)
+    gcn_diag_case("gcn_diag_wn18_d200 (vs basis B2)", 40943, 18, 141442, 200, B=2)
+    # bench.py's synthetic workload at x0.5 (uniform endpoints); the block layer's step there is 386.6 ms (DESIGN 4)
+    gcn_diag_case("gcn_diag_synthetic_x0.5_V5M_E50M_d512", 5_000_000, 1000, 50_000_000, 512, skewed=False, rounds=2)
+
+
+if "--gcn-diag" in sys.argv:
+    gcn_diag_section()
+    print(json.dumps(out, indent=1))
+    sys.exit(0)
+
 # ---- DistMult: FB15k-237 train-step decoder shape: N = 330000 triples, d = 500 ----
 V, d, N = 14541, 500, 330000
 g = torch.Generator(device=dev).manual_seed(0)
@@ -288,4 +384,5 @@ def highway_case(name, V, d):
 
 highway_case("highway_fb15k237_V14541_d500", 14541, 500)
 highway_case("highway_V2M_d512", 2_000_000, 512)
+gcn_diag_section()
 print(json.dumps(out, indent=1))
