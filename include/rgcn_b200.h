@@ -395,6 +395,38 @@ int rgcn_highway_backward(const float* c1, const float* c2, const float* W, cons
                           int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Variational head of the variational encoders (Name=variational_embedding / variational_gcn_basis,
+ * model_builder.py:43-69, :186-254; extras/variational_encoding.py:14-31).  With l = log sigma:
+ *
+ *   z = mu + exp(l) * eps,    kl[0] = -0.0005 * sum over all V x w elements of (1 + 2 l - mu^2 - exp(2 l))
+ *
+ * Embedding variant (H == NULL, d == 0): mu = W_mu, l = W_sigma, both [V, w]; b_mu, b_sigma, P, dH, db_mu and
+ * db_sigma are not used and may be NULL.
+ * Gcn variant (H [V, d], d > 0): mu = H W_mu + b_mu, l = H W_sigma + b_sigma with W_mu, W_sigma [d, w] and b_mu,
+ * b_sigma [w]; one 3xTF32 GEMM over the interleaved weight computes both and writes P [V, 2w] = (mu, l) interleaved
+ * per element (P[v, 2j] = mu[v, j], P[v, 2j + 1] = l[v, j]), which the backward pass reads.
+ * eps, z, dz : [V, w].  eps is drawn by the caller (N(0, 1)).
+ * Backward, g = g_kl[0] (device memory, the incoming gradient of kl):
+ *   dmu = dz + 0.001 g mu,  dl = dz exp(l) eps + 0.001 g (exp(2 l) - 1);
+ *   embedding: dW_mu = dmu, dW_sigma = dl;  gcn: db = column sums of dmu / dl, dW = H^T dmu / H^T dl,
+ *   dH = dmu W_mu^T + dl W_sigma^T.  Every output is overwritten.
+ * kl and the db column sums are reduced in a fixed order (bitwise repeatable).
+ * Arguments are checked before any device work: null pointers, H == NULL while d != 0 (or the reverse), V < 0,
+ * d % 4 != 0 or w <= 0 or w % 4 != 0 are RGCN_ERR_INVALID, a short workspace RGCN_ERR_WORKSPACE, no device
+ * RGCN_ERR_NODEVICE.  rgcn_variational_workspace_bytes takes d = 0 for the embedding variant.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_variational_workspace_bytes(int64_t V, int32_t d, int32_t w, int backward);
+
+int rgcn_variational_forward(const float* H, int64_t V, int32_t d, int32_t w, const float* W_mu, const float* b_mu,
+                             const float* W_sigma, const float* b_sigma, const float* eps, float* z, float* P,
+                             float* kl, void* workspace, int64_t workspace_bytes, void* stream);
+
+int rgcn_variational_backward(const float* H, int64_t V, int32_t d, int32_t w, const float* W_mu,
+                              const float* W_sigma, const float* P, const float* eps, const float* dz,
+                              const float* g_kl, float* dH, float* dW_mu, float* db_mu, float* dW_sigma,
+                              float* db_sigma, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * DistMult triple scorer ("BilinearDiag", decoders/bilinear_diag.py:14-34, :63-69).
  *
  *   energy[n] = sum_k codes[X[n,0],k] * rel[X[n,1],k] * codes[X[n,2],k]

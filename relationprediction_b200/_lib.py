@@ -24,6 +24,7 @@ EXPORTED_SYMBOLS = [
     "rgcn_basis_diagcoef_workspace_bytes", "rgcn_basis_diagcoef_forward", "rgcn_basis_diagcoef_backward",
     "rgcn_diag_workspace_bytes", "rgcn_diag_forward", "rgcn_diag_backward",
     "rgcn_highway_workspace_bytes", "rgcn_highway_forward", "rgcn_highway_backward",
+    "rgcn_variational_workspace_bytes", "rgcn_variational_forward", "rgcn_variational_backward",
     "distmult_forward", "distmult_backward", "distmult_rank_workspace_bytes", "distmult_rank",
     "distmult_backward_slices", "rgcn_block_slice_sumsq_workspace_bytes", "rgcn_block_slice_sumsq",
     "rgcn_complex_forward", "rgcn_complex_backward", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_rank",
@@ -152,6 +153,14 @@ def _declare(lib):
     lib.rgcn_highway_forward.argtypes = [vp, vp, vp, vp, c_int64, c_int32, vp, vp, vp, c_int64, vp]
     lib.rgcn_highway_backward.restype = c_int
     lib.rgcn_highway_backward.argtypes = [vp, vp, vp, vp, vp, c_int64, c_int32, vp, vp, vp, vp, vp, c_int64, vp]
+    lib.rgcn_variational_workspace_bytes.restype = c_int64
+    lib.rgcn_variational_workspace_bytes.argtypes = [c_int64, c_int32, c_int32, c_int]
+    lib.rgcn_variational_forward.restype = c_int
+    lib.rgcn_variational_forward.argtypes = [vp, c_int64, c_int32, c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                             c_int64, vp]
+    lib.rgcn_variational_backward.restype = c_int
+    lib.rgcn_variational_backward.argtypes = [vp, c_int64, c_int32, c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                              vp, vp, c_int64, vp]
     lib.distmult_forward.restype = c_int
     lib.distmult_forward.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, vp, vp, vp, vp]
     lib.distmult_backward_slices.restype = c_int

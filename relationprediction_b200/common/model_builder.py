@@ -3,7 +3,8 @@
 Only the branches on the accelerated path are built: encoders `gcn_diag` (DiagGcn layers), `gcn_basis` (BasisGcn, or ConcatGcn
 when Concatenation=Yes, BasisGcnTimesDiag when DiagonalCoefficients=Yes; with UseInputTransform=No layer 0 is a one-hot
 BasisGcn; SkipConnections=Highway wraps every
-feature-input layer in a HighwayLayer) and `embedding`; decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
+feature-input layer in a HighwayLayer), `embedding`, and the variational encoders `variational_embedding` and
+`variational_gcn_basis` (a VariationalEncoding over two linear AffineTransform heads); decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag
 from ..decoders.complex import Complex
@@ -15,6 +16,7 @@ from ..encoders.message_gcns.gcn_diag import DiagGcn
 from ..encoders.relation_embedding import RelationEmbedding
 from ..extras.graph_representations import Representation
 from ..extras.highway_layer import HighwayLayer
+from ..extras.variational_encoding import VariationalEncoding
 
 
 def _flag(settings, key, default="No"):
@@ -69,6 +71,46 @@ def build_encoder(encoder_settings, triples):
         else:
             encoding = graph   # featureless: layer 0 reads one-hot entity input (model_builder.py:166-167)
         encoding = apply_basis_gcn(encoder_settings, encoding, internal_shape, layers)
+        if _flag(encoder_settings, 'UseOutputTransform') == "Yes":
+            encoding = AffineTransform(projection_shape, encoder_settings, next_component=encoding,
+                                       onehot_input=False, use_nonlinearity=False, use_bias=True)
+        return RelationEmbedding(relation_shape, encoder_settings, next_component=encoding)
+
+    if name == "variational_embedding":
+        # model_builder.py:43-69: two bias-free one-hot tables, mu = W_mu and log sigma = W_sigma
+        input_shape = [int(encoder_settings['EntityCount']), int(encoder_settings['CodeDimension'])]
+        mu = AffineTransform(input_shape, encoder_settings, onehot_input=True, use_bias=False, use_nonlinearity=False)
+        sigma = AffineTransform(input_shape, encoder_settings, onehot_input=True, use_bias=False,
+                                use_nonlinearity=False)
+        z = VariationalEncoding(input_shape, encoder_settings, mu_network=mu, sigma_network=sigma)
+        return RelationEmbedding(input_shape, encoder_settings, next_component=z)
+
+    if name == "variational_gcn_basis":
+        # model_builder.py:186-254: the gcn_basis trunk, two biased linear heads for mu and log sigma, the
+        # reparameterised code, then the optional output projection and RelationEmbedding
+        graph = Representation(triples, encoder_settings)
+        d_int = int(encoder_settings['InternalEncoderDimension'])
+        input_shape = [int(encoder_settings['EntityCount']), d_int]
+        internal_shape = [d_int, d_int]
+        projection_shape = [d_int, int(encoder_settings['CodeDimension'])]
+        relation_shape = [int(encoder_settings['EntityCount']), int(encoder_settings['CodeDimension'])]
+        layers = int(encoder_settings['NumberOfLayers'])
+        if _flag(encoder_settings, 'UseInputTransform') == "Yes":
+            encoding = AffineTransform(input_shape, encoder_settings, next_component=graph, onehot_input=True,
+                                       use_bias=True, use_nonlinearity=True)
+        elif _flag(encoder_settings, 'RandomInput') == "Yes" or _flag(encoder_settings, 'PartiallyRandomInput') == "Yes":
+            # the branch reads neither flag (:206-214) but apply_basis_gcn does: layer 0 would be a feature layer
+            # reading the graph object itself
+            raise NotImplementedError("UseInputTransform=No with RandomInput / PartiallyRandomInput: the reference's "
+                                      "variational_gcn_basis hands the graph object to a feature-input layer")
+        else:
+            encoding = graph
+        encoding = apply_basis_gcn(encoder_settings, encoding, internal_shape, layers)
+        mu = AffineTransform(projection_shape, encoder_settings, next_component=encoding, onehot_input=False,
+                             use_nonlinearity=False, use_bias=True)
+        sigma = AffineTransform(projection_shape, encoder_settings, next_component=encoding, onehot_input=False,
+                                use_nonlinearity=False, use_bias=True)
+        encoding = VariationalEncoding(input_shape, encoder_settings, mu_network=mu, sigma_network=sigma)
         if _flag(encoder_settings, 'UseOutputTransform') == "Yes":
             encoding = AffineTransform(projection_shape, encoder_settings, next_component=encoding,
                                        onehot_input=False, use_nonlinearity=False, use_bias=True)

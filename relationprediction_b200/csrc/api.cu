@@ -3,6 +3,7 @@
 // kernel, gemm_tf32x3.cu) -> warp-centric aggregation kernels.  No vendor-library compute anywhere.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <string>
@@ -1249,6 +1250,128 @@ extern "C" int rgcn_highway_backward(const float* c1, const float* c2, const flo
   // dW = c2^T dz (contraction over V)
   rc = launch_gemm_tn_tf32x3(c2, d, dz, d, dW, d, d, d, (int)V, /*accumulate=*/0, st);
   MARK("highway_dW_gemm");
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Variational head (extras/variational_encoding.py): d == 0 (H == NULL) is the embedding variant, mu and log sigma
+// are the [V, w] tables themselves; otherwise mu / log sigma = H W + b through one GEMM with interleaved weights.
+// ------------------------------------------------------------------------------------------------
+extern "C" int64_t rgcn_variational_workspace_bytes(int64_t V, int32_t d, int32_t w, int backward) {
+  if (V < 0 || V > 0x7fffffffLL || d < 0 || d % 4 != 0 || w <= 0 || w % 4 != 0) {
+    rgcn_set_error("rgcn_variational_workspace_bytes: need 0 <= V < 2^31, d >= 0, d % 4 == 0, w > 0, w % 4 == 0");
+    return RGCN_ERR_INVALID;
+  }
+  int64_t bytes = 0;
+  if (d == 0) {
+    if (!backward) bytes += align_up(var_emb_kl_parts(V, w) * 4);
+  } else if (!backward) {
+    bytes += align_up((int64_t)2 * (2 * w) * d * 4);                       // hi / lo planes of W_int^T
+    bytes += align_up(std::max<int64_t>(1, gemm_variational_kl_parts(V, w)) * 4);
+  } else {
+    bytes += align_up((int64_t)2 * d * (2 * w) * 4);                       // hi / lo planes of W_int
+    bytes += align_up(V * 2 * w * 4);                                      // dP
+    bytes += align_up((int64_t)d * 2 * w * 4);                             // dW_int
+    bytes += align_up(var_colsum_parts(V) * 2 * w * 4);                   // db parts
+  }
+  return bytes + 256;
+}
+
+static int variational_checks(bool ok, const float* H, int64_t V, int32_t d, int32_t w, int64_t workspace_bytes,
+                              int backward, const char* who) {
+  if (!ok || (H == nullptr) != (d == 0)) {
+    rgcn_set_error(std::string(who) + ": null pointer (H is NULL exactly when d == 0, the embedding variant)");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t need = rgcn_variational_workspace_bytes(V, d, w, backward);
+  if (need < 0) {
+    rgcn_set_error(std::string(who) + ": need 0 <= V < 2^31, d >= 0, d % 4 == 0, w > 0, w % 4 == 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  int n_dev = 0;
+  if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
+    cudaGetLastError();
+    rgcn_set_error(std::string(who) + ": no CUDA device");
+    return RGCN_ERR_NODEVICE;
+  }
+  return RGCN_OK;
+}
+
+extern "C" int rgcn_variational_forward(const float* H, int64_t V, int32_t d, int32_t w, const float* W_mu,
+                                        const float* b_mu, const float* W_sigma, const float* b_sigma,
+                                        const float* eps, float* z, float* P, float* kl, void* workspace,
+                                        int64_t workspace_bytes, void* stream) {
+  const bool gcn = d != 0;
+  int rc = variational_checks(W_mu && W_sigma && eps && z && kl && workspace && (!gcn || (b_mu && b_sigma && P)), H,
+                              V, d, w, workspace_bytes, 0, "rgcn_variational_forward");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (V == 0) return rgcn_check_cuda(cudaMemsetAsync(kl, 0, sizeof(float), st), "memset(kl)");
+  Carver ws(workspace, workspace_bytes);
+  MARK("start");
+  if (!gcn) {
+    float* part = ws.take<float>(var_emb_kl_parts(V, w));
+    rc = launch_var_emb_forward(W_mu, W_sigma, eps, V, w, z, part, st);
+    if (!rc) rc = launch_var_kl_reduce(part, var_emb_kl_parts(V, w), kl, st);
+    MARK("variational_emb_fwd");
+    return rc;
+  }
+  float* hi = ws.take<float>((int64_t)2 * 2 * w * d);
+  float* lo = hi + (size_t)2 * w * d;
+  float* part = ws.take<float>(gemm_variational_kl_parts(V, w));
+  rc = launch_gemm_split_b_interleave(W_mu, W_sigma, d, w, /*transposed=*/1, hi, lo, st);
+  if (!rc) rc = launch_gemm_variational_tf32x3(H, hi, lo, b_mu, b_sigma, eps, P, z, part, (int)V, d, w, st);
+  if (!rc) rc = launch_var_kl_reduce(part, gemm_variational_kl_parts(V, w), kl, st);
+  MARK("variational_gemm");
+  return rc;
+}
+
+extern "C" int rgcn_variational_backward(const float* H, int64_t V, int32_t d, int32_t w, const float* W_mu,
+                                         const float* W_sigma, const float* P, const float* eps, const float* dz,
+                                         const float* g_kl, float* dH, float* dW_mu, float* db_mu, float* dW_sigma,
+                                         float* db_sigma, void* workspace, int64_t workspace_bytes, void* stream) {
+  const bool gcn = d != 0;
+  int rc = variational_checks(W_mu && W_sigma && eps && dz && g_kl && dW_mu && dW_sigma && workspace &&
+                                  (!gcn || (P && dH && db_mu && db_sigma)),
+                              H, V, d, w, workspace_bytes, 1, "rgcn_variational_backward");
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  MARK("start");
+  if (!gcn) {
+    rc = launch_var_emb_backward(W_mu, W_sigma, eps, dz, g_kl, V, w, dW_mu, dW_sigma, st);
+    MARK("variational_emb_bwd");
+    return rc;
+  }
+  if (V == 0) {   // no rows: every gradient is zero
+    rc = rgcn_check_cuda(cudaMemsetAsync(dW_mu, 0, (size_t)d * w * 4, st), "memset(dW_mu)");
+    if (!rc) rc = rgcn_check_cuda(cudaMemsetAsync(dW_sigma, 0, (size_t)d * w * 4, st), "memset(dW_sigma)");
+    if (!rc) rc = rgcn_check_cuda(cudaMemsetAsync(db_mu, 0, (size_t)w * 4, st), "memset(db_mu)");
+    if (!rc) rc = rgcn_check_cuda(cudaMemsetAsync(db_sigma, 0, (size_t)w * 4, st), "memset(db_sigma)");
+    return rc;
+  }
+  Carver ws(workspace, workspace_bytes);
+  float* hi = ws.take<float>((int64_t)2 * d * 2 * w);
+  float* lo = hi + (size_t)d * 2 * w;
+  float* dP = ws.take<float>(V * 2 * w);
+  float* dWint = ws.take<float>((int64_t)d * 2 * w);
+  float* col_part = ws.take<float>(var_colsum_parts(V) * 2 * w);
+  rc = launch_var_prologue(P, eps, dz, g_kl, V, w, dP, col_part, st);
+  if (!rc) rc = launch_var_colsum_finish(col_part, var_colsum_parts(V), w, db_mu, db_sigma, st);
+  if (rc) return rc;
+  MARK("variational_prologue");
+  // dW_int = H^T dP (contraction over V), then split into the two tables
+  rc = launch_gemm_tn_tf32x3(H, d, dP, 2 * w, dWint, 2 * w, d, 2 * w, (int)V, /*accumulate=*/0, st);
+  if (!rc) rc = launch_var_deinterleave(dWint, d, w, dW_mu, dW_sigma, st);
+  if (rc) return rc;
+  MARK("variational_dW_gemm");
+  // dH = dP W_int^T: Bt = W_int [N = d, K = 2w]
+  rc = launch_gemm_split_b_interleave(W_mu, W_sigma, d, w, /*transposed=*/0, hi, lo, st);
+  if (!rc) rc = launch_gemm_tf32x3(dP, 2 * w, hi, lo, 2 * w, dH, d, (int)V, d, 2 * w, /*accumulate=*/0, st);
+  MARK("variational_dH_gemm");
   return rc;
 }
 

@@ -191,6 +191,21 @@ struct HighwayEpi {
   const float* c1;             // [M, ldc] the wrapped layer's output
   float* gate;                 // [M, ldc] g
 };
+// EPI = 3: VARIATIONAL epilogue (extras/variational_encoding.py:14-31): A = H [M, K], Bt the pre-split W_int^T whose
+// rows interleave the columns of W_mu and W_sigma (row 2j = W_mu[:, j], row 2j + 1 = W_sigma[:, j]), so each
+// accumulator pair (col, col + 1) = (2j, 2j + 1) is the (mu, log sigma) of element (row, j):
+//   mu = acc + b_mu[j],  l = acc' + b_sigma[j],  P[row, 2j .. 2j+1] = (mu, l)  (C, kept for the backward pass),
+//   z[row, j] = mu + exp(l) eps[row, j],
+// and every consumer warp writes kl_part[tile * 8 + warp] = sum of (1 + 2 l - mu^2 - exp(2 l)) over its elements,
+// summed in a fixed order (per thread, then a shuffle tree), so the KL reduced from the parts is bitwise repeatable.
+struct VarEpi {
+  const float* b_mu;           // [w]
+  const float* b_sigma;        // [w]
+  const float* eps;            // [M, w]
+  float* z;                    // [M, w]
+  float* kl_part;              // [tiles * 8]
+  int w;
+};
 template <int EPI>
 struct EpiArgs {
   using type = RankEpi;
@@ -198,6 +213,10 @@ struct EpiArgs {
 template <>
 struct EpiArgs<2> {
   using type = HighwayEpi;
+};
+template <>
+struct EpiArgs<3> {
+  using type = VarEpi;
 };
 
 // PERSISTENT: a CTA walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... (N tiles fastest, see below); the
@@ -353,6 +372,34 @@ __global__ void __launch_bounds__(N_THREADS, 1)
       consume_tile(smem_base, full_bar, empty_bar, ti * num_kb, num_kb, a_rows, big, small);
       const int r0 = m0 + wg * 64 + ((ctid >> 5) & 3) * 16 + (lane >> 2);
       const int c0 = n0 + 2 * (lane & 3);
+      if constexpr (EPI == 3) {
+        float kl = 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          if (row >= M) continue;
+          float* prow = C + (size_t)row * ldc;
+          const float* erow = re.eps + (size_t)row * re.w;
+          float* zrow = re.z + (size_t)row * re.w;
+          asm volatile("" : "+l"(erow), "+l"(zrow));   // no hoisting of the 16 pairs' loads ahead of use (spills)
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = c0 + 8 * j;
+            if (col < N) {  // col is even: the pair is (mu, log sigma) of element col / 2
+              const int e = col >> 1;
+              const float mu = big[4 * j + 2 * h] + small[4 * j + 2 * h] + __ldg(re.b_mu + e);
+              const float ls = big[4 * j + 2 * h + 1] + small[4 * j + 2 * h + 1] + __ldg(re.b_sigma + e);
+              *reinterpret_cast<float2*>(prow + col) = make_float2(mu, ls);
+              zrow[e] = mu + expf(ls) * __ldg(erow + e);
+              kl += 1.f + 2.f * ls - mu * mu - expf(2.f * ls);
+            }
+          }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) kl += __shfl_xor_sync(0xffffffffu, kl, o);
+        if (lane == 0) re.kl_part[(size_t)tile * 8 + (ctid >> 5)] = kl;
+        continue;
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int row = r0 + 8 * h;
@@ -605,6 +652,26 @@ __global__ void k_split_b(const float* __restrict__ B, int64_t ldb, int N, int K
   }
 }
 
+// The pre-split of the interleaved variational weight W_int [K = d, 2w] (column 2j = W_mu[:, j], column 2j + 1 =
+// W_sigma[:, j]; W_mu, W_sigma [d, w] row-major), made from the two tables directly (no interleaved copy):
+//   transposed = 1:  Bt = W_int^T [N = 2w, K = d]     (forward, P = H W_int)
+//   transposed = 0:  Bt = W_int   [N = d, K = 2w]     (backward, dH = dP W_int^T)
+__global__ void k_split_b_interleave(const float* __restrict__ Wmu, const float* __restrict__ Wsig, int d, int w,
+                                     int transposed, float* __restrict__ hi, float* __restrict__ lo) {
+  const int64_t total = (int64_t)2 * d * w;
+  const int K = transposed ? d : 2 * w;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int n = (int)(i / K), k = (int)(i % K);
+    const int row = transposed ? k : n, c = transposed ? n : k;   // W_int[row, c]
+    const float v = __ldg(((c & 1) ? Wsig : Wmu) + (size_t)row * w + (c >> 1));
+    float h, l;
+    split_tf32(v, h, l);
+    hi[i] = h;
+    lo[i] = l;
+  }
+}
+
 }  // namespace
 
 // SM count of the current device
@@ -722,6 +789,51 @@ int launch_gemm_highway_tf32x3(const float* c2, const float* Bt_hi, const float*
                                                          HighwayEpi{bias, c1, gate});
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<highway>");
+}
+
+int launch_gemm_split_b_interleave(const float* Wmu, const float* Wsig, int d, int w, int transposed, float* hi,
+                                   float* lo, cudaStream_t st) {
+  const int64_t total = (int64_t)2 * d * w;
+  if (total == 0) return RGCN_OK;
+  int blocks = (int)((total + 255) / 256);
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  k_split_b_interleave<<<blocks, 256, 0, st>>>(Wmu, Wsig, d, w, transposed, hi, lo);
+  ++g_rgcn_launches;
+  return rgcn_check_cuda(cudaGetLastError(), "k_split_b_interleave");
+}
+
+int64_t gemm_variational_kl_parts(int64_t M, int w) {
+  return ((M + BM - 1) / BM) * ((2 * (int64_t)w + BN - 1) / BN) * 8;
+}
+
+// Variational head GEMM (EPI = 3): P = H W_int + [b_mu, b_sigma] interleaved, z = mu + exp(l) eps, one KL part per
+// consumer warp and tile (gemm_variational_kl_parts of them).  H [M, d], P [M, 2w], eps / z [M, w], contiguous.
+int launch_gemm_variational_tf32x3(const float* H, const float* Bt_hi, const float* Bt_lo, const float* b_mu,
+                                   const float* b_sigma, const float* eps, float* P, float* z, float* kl_part, int M,
+                                   int d, int w, cudaStream_t st) {
+  if (M == 0) return RGCN_OK;
+  if (d <= 0 || d % 4 != 0 || w <= 0 || w % 2 != 0) {
+    rgcn_set_error("gemm_variational_tf32x3: d > 0, d % 4 == 0, w > 0, w % 2 == 0");
+    return RGCN_ERR_INVALID;
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  SMEM_BYTES),
+                             "cudaFuncSetAttribute(gemm variational smem)");
+    if (rc) return rc;
+    attr_set = true;
+  }
+  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((2 * w + BN - 1) / BN);
+  if (tiles > 0x7fffffffLL / 8) {
+    rgcn_set_error("gemm_variational_tf32x3: too many tiles");
+    return RGCN_ERR_INVALID;
+  }
+  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
+  k_gemm_tf32x3<3><<<grid, N_THREADS, SMEM_BYTES, st>>>(H, d, Bt_hi, Bt_lo, d, P, 2 * w, M, 2 * w, d, 0, (int)tiles,
+                                                         VarEpi{b_mu, b_sigma, eps, z, kl_part, w});
+  ++g_rgcn_launches;
+  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<variational>");
 }
 
 // C[M,N] (+)= A^T B, A [K,M] row-major, B [K,N] row-major (see k_gemm_tn_tf32x3)

@@ -165,6 +165,36 @@ int launch_gemm_highway_tf32x3(const float* c2, const float* Bt_hi, const float*
 int launch_highway_prologue(const float* c1, const float* c2, const float* g, const float* dY, int64_t V, int d,
                             float* dc1, float* dz, float* dc2, float* db, cudaStream_t st);
 
+// Variational head (extras/variational_encoding.py).  W_int [d, 2w] interleaves the columns of W_mu and W_sigma
+// [d, w]; its pre-split is made from the two tables: transposed = 1 gives Bt = W_int^T [2w, d], 0 gives W_int [d, 2w].
+int launch_gemm_split_b_interleave(const float* Wmu, const float* Wsig, int d, int w, int transposed, float* hi,
+                                   float* lo, cudaStream_t st);
+// KL parts written by launch_gemm_variational_tf32x3 for M rows
+int64_t gemm_variational_kl_parts(int64_t M, int w);
+// P = H W_int + (b_mu, b_sigma) interleaved [M, 2w], z = mu + exp(l) eps [M, w], KL parts of 1 + 2l - mu^2 - exp(2l)
+int launch_gemm_variational_tf32x3(const float* H, const float* Bt_hi, const float* Bt_lo, const float* b_mu,
+                                   const float* b_sigma, const float* eps, float* P, float* z, float* kl_part, int M,
+                                   int d, int w, cudaStream_t st);
+// variational.cu -- embedding variant forward (mu = Wmu, l = Wsig, [V, w]): z and var_emb_kl_parts(V, w) parts
+int64_t var_emb_kl_parts(int64_t V, int w);
+int launch_var_emb_forward(const float* Wmu, const float* Wsig, const float* eps, int64_t V, int w, float* z,
+                           float* kl_part, cudaStream_t st);
+// kl[0] = -0.0005 * sum of the n parts, summed in a fixed order
+int launch_var_kl_reduce(const float* kl_part, int64_t n, float* kl, cudaStream_t st);
+// embedding variant backward: dWmu = dz + 0.001 g mu, dWsig = dz exp(l) eps + 0.001 g (exp(2l) - 1), g = g_kl[0]
+int launch_var_emb_backward(const float* Wmu, const float* Wsig, const float* eps, const float* dz, const float* g_kl,
+                            int64_t V, int w, float* dWmu, float* dWsig, cudaStream_t st);
+// gcn variant backward prologue: dP [V, 2w] interleaved from P [V, 2w], eps, dz [V, w], g = g_kl[0]; col_part
+// [var_colsum_parts(V), 2w] the per-row-block column sums of dP
+int64_t var_colsum_parts(int64_t V);
+int launch_var_prologue(const float* P, const float* eps, const float* dz, const float* g_kl, int64_t V, int w,
+                        float* dP, float* col_part, cudaStream_t st);
+// db_mu[j] / db_sigma[j] = sum over the parts of col_part[:, 2j] / [:, 2j + 1], in part order
+int launch_var_colsum_finish(const float* col_part, int64_t parts, int w, float* db_mu, float* db_sigma,
+                             cudaStream_t st);
+// dW_mu[:, j] = dW_int[:, 2j], dW_sigma[:, j] = dW_int[:, 2j + 1]  (dW_int [d, 2w])
+int launch_var_deinterleave(const float* dWint, int d, int w, float* dWmu, float* dWsig, cudaStream_t st);
+
 // DistMult
 // queries + gold scores of the fused scorer/ranker: side 0 (subjects corrupted): Q[t] = rel[r] * codes[o], gold = s;
 // side 1 (objects corrupted): Q[t] = codes[s] * rel[r], gold = o.  gold_sig[t] = sigmoid(<Q[t], codes[gold]>)

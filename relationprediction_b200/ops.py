@@ -546,6 +546,76 @@ def highway(c1, c2, W, b):
     return _HighwayFn.apply(c1, c2, W, b)
 
 
+class _VariationalFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, H, W_mu, b_mu, W_sigma, b_sigma, eps):
+        lib = _lib.load()
+        if not (isinstance(W_mu, torch.Tensor) and W_mu.dim() == 2):
+            raise _lib.RgcnError("W_mu must be a 2-D tensor")
+        w = W_mu.shape[1]
+        _check_cuda_f32("eps", eps)
+        V = eps.shape[0]
+        _check_cuda_f32("eps", eps, (V, w))
+        if H is None:           # embedding variant: mu = W_mu, log sigma = W_sigma
+            d = 0
+            _check_cuda_f32("W_mu", W_mu, (V, w))
+            _check_cuda_f32("W_sigma", W_sigma, (V, w))
+        else:
+            d = W_mu.shape[0]
+            _check_cuda_f32("H", H, (V, d))
+            _check_cuda_f32("W_mu", W_mu, (d, w))
+            _check_cuda_f32("W_sigma", W_sigma, (d, w))
+            _check_cuda_f32("b_mu", b_mu, (w,))
+            _check_cuda_f32("b_sigma", b_sigma, (w,))
+        dev = eps.device
+        z = torch.empty(V, w, dtype=torch.float32, device=dev)
+        kl = torch.empty((), dtype=torch.float32, device=dev)
+        P = torch.empty(V, 2 * w, dtype=torch.float32, device=dev) if d else None
+        nb = lib.rgcn_variational_workspace_bytes(V, d, w, 0)
+        if nb < 0:
+            _lib.check(int(nb), "rgcn_variational_workspace_bytes")
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_variational_forward(_ptr(H), V, d, w, _ptr(W_mu), _ptr(b_mu if d else None), _ptr(W_sigma),
+                                          _ptr(b_sigma if d else None), _ptr(eps), _ptr(z), _ptr(P), _ptr(kl),
+                                          _ptr(ws), ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_variational_forward")
+        ctx.d = d
+        ctx.save_for_backward(H, W_mu, W_sigma, P, eps)
+        return z, kl
+
+    @staticmethod
+    def backward(ctx, dz, g_kl):
+        lib = _lib.load()
+        H, W_mu, W_sigma, P, eps = ctx.saved_tensors
+        d = ctx.d
+        V, w = eps.shape
+        dev = eps.device
+        dz = dz.contiguous()
+        _check_cuda_f32("dz", dz, (V, w))
+        g_kl = g_kl.reshape(1).contiguous()
+        dW_mu, dW_sigma = torch.empty_like(W_mu), torch.empty_like(W_sigma)
+        dH = torch.empty_like(H) if d else None
+        db_mu = torch.empty(w, dtype=torch.float32, device=dev) if d else None
+        db_sigma = torch.empty(w, dtype=torch.float32, device=dev) if d else None
+        nb = lib.rgcn_variational_workspace_bytes(V, d, w, 1)
+        ws = _workspace(nb, dev)
+        rc = lib.rgcn_variational_backward(_ptr(H), V, d, w, _ptr(W_mu), _ptr(W_sigma), _ptr(P), _ptr(eps), _ptr(dz),
+                                           _ptr(g_kl), _ptr(dH), _ptr(dW_mu), _ptr(db_mu), _ptr(dW_sigma),
+                                           _ptr(db_sigma), _ptr(ws), ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_variational_backward")
+        # the embedding variant's biases are never read: their gradient is None, as in the reference
+        return dH, dW_mu, db_mu, dW_sigma, db_sigma, None
+
+
+def variational(H, W_mu, b_mu, W_sigma, b_sigma, eps):
+    """Reparameterised codes and KL term of VariationalEncoding (extras/variational_encoding.py:14-31).  With H None
+    (variational_embedding) mu = W_mu and log sigma = W_sigma ([V, w]) and the biases are ignored; otherwise
+    mu = H @ W_mu + b_mu and log sigma = H @ W_sigma + b_sigma.  Returns (z, kl): z = mu + exp(log sigma) * eps and
+    kl = -0.0005 * sum(1 + 2 log sigma - mu^2 - exp(2 log sigma)).  One library call each way; differentiable in H and
+    every weight it reads."""
+    return _VariationalFn.apply(H, W_mu, b_mu, W_sigma, b_sigma, eps)
+
+
 def _triple_forward(ctx, entry, codes, rel, X, Y):
     """Forward of a triple scorer entry point with the distmult_forward argument list."""
     lib = _lib.load()

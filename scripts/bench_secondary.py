@@ -4,7 +4,9 @@ ranking, basis layer
 (UseInputTransform=No) first basis layer and the per-channel-coefficient basis layer (DiagonalCoefficients=Yes) at
 the same shapes next to the feature-input basis layer, the highway
 skip connection next to the plain GEMM of its shape, and the diagonal R-GCN layer (Name=gcn_diag) next to the basis
-layer and at bench.py's synthetic shape.  `python scripts/bench_secondary.py --gcn-diag` runs only that last section."""
+layer and at bench.py's synthetic shape.  `python scripts/bench_secondary.py --gcn-diag` runs only that last section;
+`--variational` runs only the variational head (both variants at the FB15k-237 shape) next to an unfused torch
+composition."""
 import json
 import subprocess
 import sys
@@ -130,6 +132,65 @@ def gcn_diag_section():
 
 if "--gcn-diag" in sys.argv:
     gcn_diag_section()
+    print(json.dumps(out, indent=1))
+    sys.exit(0)
+
+
+# ---- variational head (Name=variational_embedding / variational_gcn_basis) next to an unfused torch composition ----
+def variational_case(name, V, d, w, rounds=3):
+    """ops.variational forward and forward + backward (g = 1 on the KL term, L2 flushed between calls), alternated
+    `rounds` times with the same head written as separate torch ops (two fp32 matmuls, exp, multiply-add, the KL
+    reduction; autograd backward); medians.  d = 0 is the embedding variant (mu = W_mu, log sigma = W_sigma [V, w])."""
+    g = torch.Generator(device=dev).manual_seed(0)
+    r = lambda *s, sc=1.0: (torch.randn(*s, device=dev, generator=g) * sc).requires_grad_(True)
+    if d:
+        H, Wm, Ws = r(V, d), r(d, w, sc=1 / np.sqrt(d)), r(d, w, sc=0.5 / np.sqrt(d))
+    else:
+        H, Wm, Ws = None, r(V, w), r(V, w, sc=0.5)
+    bm, bs = r(w), r(w, sc=0.2)
+    eps, dz = torch.randn(V, w, device=dev, generator=g), torch.randn(V, w, device=dev, generator=g)
+
+    def unfused():
+        mu, ls = (H @ Wm + bm, H @ Ws + bs) if d else (Wm, Ws)
+        return mu + torch.exp(ls) * eps, -0.0005 * torch.sum(1 + 2 * ls - mu * mu - torch.exp(2 * ls))
+    fns = {"fused": lambda: ops.variational(H, Wm, bm, Ws, bs, eps), "unfused_torch": unfused}
+
+    def step(f):
+        z, kl = f()
+        torch.autograd.backward([z, kl], [dz, torch.ones((), device=dev)])
+
+    def fwd(f):
+        with torch.no_grad():
+            f()
+    with torch.no_grad():
+        zf, klf = fns["fused"]()
+        zu, klu = unfused()
+    ms = {k: {"fwd": [], "fwd_bwd": []} for k in fns}
+    for _ in range(rounds):
+        for k, f in fns.items():
+            ms[k]["fwd"].append(timeit(lambda: fwd(f), n=20))
+            ms[k]["fwd_bwd"].append(timeit(lambda: step(f), n=20))
+    med = {k: {p: float(np.median(v[p])) for p in v} for k, v in ms.items()}
+    _lib.profile_enable(True)
+    acc = {}
+    for _ in range(5):
+        flush.zero_()
+        step(fns["fused"])
+        torch.cuda.synchronize()
+        for nm, v in _lib.profile_read():
+            acc[nm] = acc.get(nm, 0.0) + v / 5
+    _lib.profile_enable(False)
+    out[name] = {"V": V, "d": d, "w": w, "gpu": card, "medians_ms": med, "runs_ms": ms,
+                 "speedup_vs_unfused": {p: med["unfused_torch"][p] / med["fused"][p] for p in ("fwd", "fwd_bwd")},
+                 "max_rel_z_vs_unfused": float((zf - zu).abs().max() / zu.abs().max()),
+                 "rel_kl_vs_unfused": float((klf - klu).abs() / klu.abs()),
+                 "stages_ms": {k: round(v, 4) for k, v in acc.items()}}
+    torch.cuda.empty_cache()
+
+
+if "--variational" in sys.argv:
+    variational_case("variational_gcn_fb15k237_V14541_d500_w500", 14541, 500, 500)
+    variational_case("variational_embedding_fb15k237_V14541_w500", 14541, 0, 500)
     print(json.dumps(out, indent=1))
     sys.exit(0)
 
