@@ -522,6 +522,34 @@ int rgcn_complex_rank(const float* codes, const float* rel, int32_t V, int32_t V
                       int64_t n, int side, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
                       int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Top-k entity prediction, fused: the k entities each query believes in most, without the [n, V] score matrix
+ * that predict_all_subject_scores / predict_all_object_scores (bilinear_diag.py:51-61, complex.py:77-106)
+ * materialise and Scorer.dump_all_scores (common/evaluation.py:391-408) writes out.  For every triple t of X:
+ *   side 0 (predict subjects): q = rel[r] * codes[o]   (ComplEx: the rgcn_complex_rank side-0 row)
+ *   side 1 (predict objects):  q = codes[s] * rel[r]   (ComplEx: the rgcn_complex_rank side-1 row)
+ * the predicted column of X is not read.  energy(t, v) = sum_k q[k] * codes[v, k] (3xTF32 GEMM); the score is
+ * sigmoid(energy) in float32.  ids[t, :] lists the entities in order of energy descending, the smaller id first on
+ * ties (the energy keeps its order where the float32 sigmoid saturates to 1); energies[t, :] are their energies.
+ * exclude_mask : uint32 [n, ceil(V/32)] device, bit v of row t = entity v never appears in row t (the known_mask
+ *                format of distmult_rank), or NULL.
+ * When fewer than k entities remain, the tail of the row is id -1, energy -inf.  1 <= k <= 128, else
+ * RGCN_ERR_INVALID.  ids int32 [n, k], energies float32 [n, k] device.  The result is bitwise repeatable.
+ * workspace  : rgcn_topk_workspace_bytes(V, d, n, k), linear in n (about 4 d + 8 k ceil(V/128) bytes per query; a
+ *              caller with many queries over many entities calls in chunks).  Its head holds the hi/lo split of
+ *              `codes` exactly as in distmult_rank's workspace: reuse_split != 0 skips re-splitting when the same
+ *              workspace (or a rank workspace of the same codes) is passed again with unchanged codes.
+ * Errors as distmult_rank: RGCN_ERR_INVALID (null pointers, d % 4 != 0, side, k), RGCN_ERR_WORKSPACE.
+ * rgcn_topk_workspace_bytes returns RGCN_ERR_INVALID (-1) on bad arguments.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_topk_workspace_bytes(int32_t V, int32_t d, int64_t n, int32_t k);
+int distmult_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                  int64_t n, int side, int32_t k, const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
+                  float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+int rgcn_complex_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                      int64_t n, int side, int32_t k, const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
+                      float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

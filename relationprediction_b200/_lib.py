@@ -28,6 +28,7 @@ EXPORTED_SYMBOLS = [
     "distmult_forward", "distmult_backward", "distmult_rank_workspace_bytes", "distmult_rank",
     "distmult_backward_slices", "rgcn_block_slice_sumsq_workspace_bytes", "rgcn_block_slice_sumsq",
     "rgcn_complex_forward", "rgcn_complex_backward", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_rank",
+    "rgcn_topk_workspace_bytes", "distmult_topk", "rgcn_complex_topk",
 ]
 
 RGCN_NORM_CANONICAL, RGCN_NORM_EXPLICIT, RGCN_NORM_NONE = 0, 1, 2
@@ -187,6 +188,12 @@ def _declare(lib):
     lib.rgcn_complex_rank.restype = c_int
     lib.rgcn_complex_rank.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, vp, c_int, vp, vp, vp,
                                       c_int64, vp]
+    lib.rgcn_topk_workspace_bytes.restype = c_int64
+    lib.rgcn_topk_workspace_bytes.argtypes = [c_int32, c_int32, c_int64, c_int32]
+    for name in ("distmult_topk", "rgcn_complex_topk"):
+        getattr(lib, name).restype = c_int
+        getattr(lib, name).argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, c_int32, vp, c_int, vp,
+                                       vp, vp, c_int64, vp]
 
 
 def load():

@@ -73,6 +73,21 @@ class Scorer(object):
     def register_model(self, model):
         self.model = model
 
+    def predict_top_k(self, triples, k, side, filtered=True):
+        """The k most likely entities for each triple through the model's fused top-k path (Model.predict_top_k):
+        side 0 predicts subjects, 1 objects.  filtered=True leaves out every entity that completes a triple of any
+        registered split -- the known_subject_triples / known_object_triples lists the filtered ranks use -- so only
+        new answers come back; filtered=False excludes nothing.  Returns numpy (ids, energies, scores), each [n, k]."""
+        triples = np.asarray(triples).reshape(-1, 3)
+        exclude = None
+        if filtered:
+            tl = triples.tolist()
+            if int(side) == 0:
+                exclude = [self.known_subject_triples.get((t[2], t[1]), []) for t in tl]
+            else:
+                exclude = [self.known_object_triples.get((t[0], t[1]), []) for t in tl]
+        return self.model.predict_top_k(triples, k, side, exclude)
+
     def compute_scores(self, triples, verbose=False):
         return self.compute_mrr_scores(triples, verbose)
 

@@ -1568,3 +1568,76 @@ extern "C" int rgcn_complex_rank(const float* codes, const float* rel, int32_t V
   return rank_with_queries(launch_complex_rank_prepare, codes, rel, V, d, X, n, side, known_mask, reuse_split,
                            raw_rank, filtered_rank, workspace, workspace_bytes, (cudaStream_t)stream);
 }
+
+// ------------------------------------------------------------------------------------------------
+// Top-k prediction over all entities, fused (DistMult and ComplEx)
+// ------------------------------------------------------------------------------------------------
+// The decoder-independent body of distmult_topk / rgcn_complex_topk: the hi/lo split of `codes` (unless reused),
+// the decoder's query rows, the scoring GEMM with its top-k epilogue (each row's best k of every 128-entity tile),
+// and the merge of those candidates.
+// Workspace layout: [hi V*d | lo V*d | Q n*d | cand n*ceil(V/128)*k (energy, id) pairs]; the head is the same as
+// rank_with_queries', so one workspace with its split serves both.
+static int64_t topk_per_row_bytes(int32_t V, int32_t d, int32_t k) {
+  return (int64_t)d * 4 + (int64_t)((V + 127) / 128) * k * 8;
+}
+
+extern "C" int64_t rgcn_topk_workspace_bytes(int32_t V, int32_t d, int64_t n, int32_t k) {
+  if (V <= 0 || d <= 0 || d % 4 != 0 || n < 0 || k < 1 || k > 128 ||
+      (n > 0 && topk_per_row_bytes(V, d, k) > ((int64_t)1 << 60) / n)) {
+    rgcn_set_error("rgcn_topk_workspace_bytes: bad arguments (need V > 0, d > 0, d % 4 == 0, n >= 0, 1 <= k <= 128)");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t tn = (V + 127) / 128;
+  return 2 * align_up((int64_t)V * d * 4) + align_up(n * d * 4) + align_up(n * tn * k * 8) + 256;
+}
+
+static int topk_with_queries(RankPrepareFn prepare, const char* who, const float* codes, const float* rel, int32_t V,
+                             int32_t Vrel, int32_t d, const int32_t* X, int64_t n, int side, int32_t k,
+                             const uint32_t* exclude_mask, int reuse_split, int32_t* ids, float* energies,
+                             void* workspace, int64_t workspace_bytes, cudaStream_t st) {
+  if (!codes || !rel || (n > 0 && (!X || !ids || !energies)) || !workspace || V <= 0 || Vrel <= 0 || d <= 0 ||
+      d % 4 != 0 || n < 0 || n > 0x7fffffffLL || (side != 0 && side != 1)) {
+    rgcn_set_error(std::string(who) + ": bad arguments (need non-null pointers, d % 4 == 0, side in {0,1})");
+    return RGCN_ERR_INVALID;
+  }
+  if (k < 1 || k > 128) {
+    rgcn_set_error(std::string(who) + ": k = " + std::to_string(k) + " is out of range (1 <= k <= 128)");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t need = rgcn_topk_workspace_bytes(V, d, n, k);
+  if (need < 0) return (int)need;
+  if (workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_topk_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  const int tn = (V + 127) / 128;
+  Carver ws(workspace, workspace_bytes);
+  float* hi = ws.take<float>((int64_t)V * d);
+  float* lo = ws.take<float>((int64_t)V * d);
+  float* Q = ws.take<float>(n * d);
+  uint2* cand = ws.take<uint2>(n * tn * k);
+  int rc = RGCN_OK;
+  if (!reuse_split) rc = launch_gemm_split_b(codes, d, V, d, /*transposed=*/0, hi, lo, st);
+  if (rc || n == 0) return rc;
+  rc = prepare(codes, rel, d, X, n, side, Q, nullptr, nullptr, st);
+  if (rc) return rc;
+  rc = launch_gemm_topk_tf32x3(Q, d, hi, lo, d, (int)n, V, d, exclude_mask, (V + 31) / 32, k, cand, st);
+  if (rc) return rc;
+  return launch_topk_merge(cand, n, tn * k, k, ids, energies, st);
+}
+
+extern "C" int distmult_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                             const int32_t* X, int64_t n, int side, int32_t k, const uint32_t* exclude_mask,
+                             int reuse_split, int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes,
+                             void* stream) {
+  return topk_with_queries(launch_distmult_rank_prepare, "distmult_topk", codes, rel, V, Vrel, d, X, n, side, k,
+                           exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_complex_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                 const int32_t* X, int64_t n, int side, int32_t k, const uint32_t* exclude_mask,
+                                 int reuse_split, int32_t* ids, float* energies, void* workspace,
+                                 int64_t workspace_bytes, void* stream) {
+  return topk_with_queries(launch_complex_rank_prepare, "rgcn_complex_topk", codes, rel, V, Vrel, d, X, n, side, k,
+                           exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+}

@@ -201,7 +201,6 @@ __global__ void __launch_bounds__(256)
       float kr[W], ki[W], br[W], bi[W], gr[W], gi[W], qr[W], qi[W];
       Vec<W>::load(ek + k, kr), Vec<W>::load(ek + h + k, ki);
       Vec<W>::load(rr + k, br), Vec<W>::load(rr + h + k, bi);
-      Vec<W>::load(eg + k, gr), Vec<W>::load(eg + h + k, gi);
 #pragma unroll
       for (int j = 0; j < W; ++j) {
         if (side == 0) {
@@ -211,13 +210,19 @@ __global__ void __launch_bounds__(256)
           qr[j] = fmaf(kr[j], br[j], -ki[j] * bi[j]);
           qi[j] = fmaf(ki[j], br[j], kr[j] * bi[j]);
         }
-        e = fmaf(qr[j], gr[j], e);
-        e = fmaf(qi[j], gi[j], e);
       }
       Vec<W>::store(q + k, qr), Vec<W>::store(q + h + k, qi);
+      if (gold_sig) {   // the top-k path asks for the query rows only: the predicted column of X is not read
+        Vec<W>::load(eg + k, gr), Vec<W>::load(eg + h + k, gi);
+#pragma unroll
+        for (int j = 0; j < W; ++j) {
+          e = fmaf(qr[j], gr[j], e);
+          e = fmaf(qi[j], gi[j], e);
+        }
+      }
     }
     e = warp_sum(e);
-    if (lane == 0) {
+    if (lane == 0 && gold_sig) {
       gold_sig[t] = 1.0f / (1.0f + expf(-e));
       gold_col[t] = gold;
     }

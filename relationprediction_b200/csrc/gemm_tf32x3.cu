@@ -206,6 +206,18 @@ struct VarEpi {
   float* kl_part;              // [tiles * 8]
   int w;
 };
+// EPI = 4: TOP-K epilogue (filtered top-k prediction over all entities, decoders/bilinear_diag.py:51-61 and
+// complex.py:77-106 without the [M, N] score matrix): row m of A is a query, row n of Bt an entity code.  For each
+// row the tile's best k eligible (energy, column) pairs -- energy descending, smaller column first on ties; columns
+// >= N and columns whose bit is set in `excl` are not eligible -- are written in that order to
+// cand[(row * tn + tile column) * k + p]; the tail past the eligible columns is (-inf, -1).  k <= BN.
+struct TopKEpi {
+  const uint32_t* excl;        // [M, words] bit v = entity v never appears in row m (or nullptr)
+  int words;                   // ceil(N / 32)
+  int k;                       // candidates per row and tile, 1 <= k <= BN
+  int tn;                      // N tiles
+  uint2* cand;                 // [M, tn, k] (energy bits, column)
+};
 template <int EPI>
 struct EpiArgs {
   using type = RankEpi;
@@ -217,6 +229,10 @@ struct EpiArgs<2> {
 template <>
 struct EpiArgs<3> {
   using type = VarEpi;
+};
+template <>
+struct EpiArgs<4> {
+  using type = TopKEpi;
 };
 
 // PERSISTENT: a CTA walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... (N tiles fastest, see below); the
@@ -372,6 +388,83 @@ __global__ void __launch_bounds__(N_THREADS, 1)
       consume_tile(smem_base, full_bar, empty_bar, ti * num_kb, num_kb, a_rows, big, small);
       const int r0 = m0 + wg * 64 + ((ctid >> 5) & 3) * 16 + (lane >> 2);
       const int c0 = n0 + 2 * (lane & 3);
+      if constexpr (EPI == 4) {
+        // The quad of lanes lane & ~3 holds rows r0 and r0 + 8 of the tile: 32 columns each per lane, value i
+        // (= 2 j + e) at column c0 + 8 j + e, so a lane's columns increase with i.  k rounds per row: every lane
+        // takes its best value not yet taken (strict > in i order: the smaller column wins a tie), the quad keeps
+        // the best of the four by two shuffles on (energy, column), and the lane that owned it marks it taken.
+        float v[2][32];
+        uint32_t left[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          left[h] = 0u;
+#pragma unroll
+          for (int cb = 0; cb < BN / 32; ++cb) {
+            const int chunk = n0 + 32 * cb;
+            const uint32_t xw =
+                (re.excl && row < M && chunk < N) ? __ldg(re.excl + (size_t)row * re.words + (chunk >> 5)) : 0u;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int j = 4 * cb + jj, i = 2 * j + e, col = c0 + 8 * j + e;
+                v[h][i] = big[4 * j + 2 * h + e] + small[4 * j + 2 * h + e];
+                if (row < M && col < N && !((xw >> (col & 31)) & 1u)) left[h] |= 1u << i;
+              }
+            }
+          }
+        }
+        // candidate p of row r0 + 8 h (formed at the store: a live pointer pair would spill)
+        auto slot = [&](int h, int p) {
+          return re.cand + ((size_t)(r0 + 8 * h) * re.tn + (size_t)(n0 / BN)) * re.k + p;
+        };
+        const bool writer = (lane & 3) == 0;
+        const uint2 none = make_uint2(__float_as_uint(-INFINITY), 0xffffffffu);
+        int p = 0;
+        for (; p < re.k; ++p) {
+          float be[2];
+          int bc[2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            int bi = -1;
+            be[h] = -INFINITY;
+#pragma unroll
+            for (int i = 0; i < 32; ++i)
+              if (((left[h] >> i) & 1u) && (bi < 0 || v[h][i] > be[h])) {
+                be[h] = v[h][i];
+                bi = i;
+              }
+            const int mine = bi < 0 ? 0x7fffffff : c0 + 8 * (bi >> 1) + (bi & 1);
+            bc[h] = mine;
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1) {
+              const float oe = __shfl_xor_sync(0xffffffffu, be[h], o);
+              const int oc = __shfl_xor_sync(0xffffffffu, bc[h], o);
+              if (oc != 0x7fffffff && (bc[h] == 0x7fffffff || oe > be[h] || (oe == be[h] && oc < bc[h]))) {
+                be[h] = oe;
+                bc[h] = oc;
+              }
+            }
+            if (bi >= 0 && bc[h] == mine) left[h] &= ~(1u << bi);
+          }
+          if (!__any_sync(0xffffffffu, bc[0] != 0x7fffffff || bc[1] != 0x7fffffff)) break;   // the warp's rows ran dry
+          if (writer) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              if (r0 + 8 * h < M)
+                *slot(h, p) = bc[h] == 0x7fffffff ? none : make_uint2(__float_as_uint(be[h]), (uint32_t)bc[h]);
+          }
+        }
+        if (writer) {
+          for (; p < re.k; ++p) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              if (r0 + 8 * h < M) *slot(h, p) = none;
+          }
+        }
+        continue;
+      }
       if constexpr (EPI == 3) {
         float kl = 0.f;
 #pragma unroll
@@ -760,6 +853,36 @@ int launch_gemm_rank_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
                                                          (int)tiles, re);
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<rank>");
+}
+
+// Scoring GEMM with the top-k epilogue (EPI = 4): queries Q [M,K] against the pre-split entity codes Bt [N,K]; each
+// row's best k eligible (energy, column) pairs of every N tile go to cand [M, ceil(N / BN), k].
+int launch_gemm_topk_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, const float* Bt_lo, int64_t ldb, int M,
+                            int N, int K, const uint32_t* excl, int words, int k, uint2* cand, cudaStream_t st) {
+  if (M == 0 || N == 0) return RGCN_OK;
+  if (K <= 0 || K % 4 != 0 || ldq % 4 != 0 || ldb % 4 != 0 || k < 1 || k > BN) {
+    rgcn_set_error("gemm_topk_tf32x3: K > 0; K and leading dimensions must be multiples of 4; 1 <= k <= 128");
+    return RGCN_ERR_INVALID;
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  SMEM_BYTES),
+                             "cudaFuncSetAttribute(gemm topk smem)");
+    if (rc) return rc;
+    attr_set = true;
+  }
+  const int tn = (N + BN - 1) / BN;
+  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * tn;
+  if (tiles > 0x7fffffffLL) {
+    rgcn_set_error("gemm_topk_tf32x3: too many tiles");
+    return RGCN_ERR_INVALID;
+  }
+  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
+  k_gemm_tf32x3<4><<<grid, N_THREADS, SMEM_BYTES, st>>>(Q, ldq, Bt_hi, Bt_lo, ldb, nullptr, 0, M, N, K, 0,
+                                                         (int)tiles, TopKEpi{excl, words, k, tn, cand});
+  ++g_rgcn_launches;
+  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<topk>");
 }
 
 // Highway gate GEMM with the blend epilogue (EPI = 2): z = c2 @ W + bias with W pre-split as Bt = W^T [d, d];

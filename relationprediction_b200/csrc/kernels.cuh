@@ -153,6 +153,16 @@ int launch_gemm_rank_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
                             int N, int K, const float* gold_sig, const int32_t* gold_col, const uint32_t* known,
                             int words, int32_t* raw_cnt, int32_t* known_cnt, cudaStream_t st);
 
+// Scoring GEMM with the top-k epilogue: for every row of Q and every 128-column tile of Bt, the tile's best k
+// eligible (energy, column) pairs -- energy descending, smaller column first on ties; excl bit set or column >= N:
+// not eligible -- in order in cand [M, ceil(N / 128), k] as (energy bits, column), the tail padded (-inf, -1).
+int launch_gemm_topk_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, const float* Bt_lo, int64_t ldb, int M,
+                            int N, int K, const uint32_t* excl, int words, int k, uint2* cand, cudaStream_t st);
+// topk.cu -- merge of those candidates: ids [n, k] / energies [n, k] of every row's best k, in the same order, the
+// tail past the row's eligible columns padded (-1, -inf)
+int launch_topk_merge(const uint2* cand, int64_t n, int per_row, int k, int32_t* ids, float* energies,
+                      cudaStream_t st);
+
 int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
                           int M, int N, int K, int accumulate, cudaStream_t st);
 
@@ -198,6 +208,7 @@ int launch_var_deinterleave(const float* dWint, int d, int w, float* dWmu, float
 // DistMult
 // queries + gold scores of the fused scorer/ranker: side 0 (subjects corrupted): Q[t] = rel[r] * codes[o], gold = s;
 // side 1 (objects corrupted): Q[t] = codes[s] * rel[r], gold = o.  gold_sig[t] = sigmoid(<Q[t], codes[gold]>)
+// (gold_sig == nullptr: Q only; the gold column of X is then not read)
 int launch_distmult_rank_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
                                  float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
 int launch_distmult_rank_finalize(const int32_t* raw_cnt, const int32_t* known_cnt, int64_t n, int32_t* raw_rank,

@@ -115,3 +115,29 @@ class BilinearDiag(Model):
                 out[2 * side].append(raw)
                 out[2 * side + 1].append(filt)
         return tuple(torch.cat(o).cpu().numpy().astype(np.int64) if o else np.zeros(0, np.int64) for o in out)
+
+    def top_k_all(self, triplets, k, side, exclude_lists=None, chunk=4096):
+        """The k entities of highest energy for every triple (side 0 predicts subjects, 1 objects; the predicted
+        column is not read), without the [n, V] score matrices of predict_all_subject_scores /
+        predict_all_object_scores (bilinear_diag.py:51-61): the encoder runs once, the codes are split once, and the
+        scoring GEMM keeps each row's best k in its epilogue.  exclude_lists[t] lists the entities row t may not
+        return (or None: none excluded).  Returns (ids int64 [n, k], energies float32 [n, k]); energy descending,
+        the smaller id first on ties; rows with fewer than k eligible entities end in (-1, -inf)."""
+        subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='test')
+        assert subject_codes is object_codes, "fused top-k prediction expects one shared entity code matrix"
+        codes, rel = subject_codes.contiguous(), relation_codes.contiguous()
+        ranker = self._ranker(codes, rel)
+        V = codes.shape[0]
+        tri = np.ascontiguousarray(np.asarray(triplets, dtype=np.int32).reshape(-1, 3))
+        ids, energies = [], []
+        for c0 in range(0, len(tri), chunk):
+            X = torch.as_tensor(tri[c0:c0 + chunk], device=codes.device)
+            mask = None
+            if exclude_lists is not None:
+                mask = torch.as_tensor(self.known_bit_mask(exclude_lists[c0:c0 + chunk], V), device=codes.device)
+            i, e = ranker.top_k(X, side, k, mask)
+            ids.append(i)
+            energies.append(e)
+        if not ids:
+            return np.zeros((0, k), np.int64), np.zeros((0, k), np.float32)
+        return torch.cat(ids).cpu().numpy().astype(np.int64), torch.cat(energies).cpu().numpy()

@@ -105,6 +105,28 @@ class Model(object):
         with torch.no_grad():
             return self.rank_all(triplets, known_subject_lists, known_object_lists)
 
+    def predict_top_k(self, triplets, k, side, exclude_lists=None):
+        """The k most likely entities for every triple under the decoder's fused top-k path (one encoder pass for
+        the whole set), fed like rank_all_entities.  side 0 predicts subjects, 1 objects; the predicted column of
+        `triplets` is not read but must hold an entity id.  exclude_lists[t] (optional) lists the entities row t
+        may not return.  Returns numpy (ids [n, k], energies [n, k], scores = float32 sigmoid(energies)); rows with
+        fewer than k eligible entities end in id -1, energy -inf, score 0."""
+        if not hasattr(self, 'top_k_all') or self.get_device().type != 'cuda':
+            raise NotImplementedError("%s has no fused top-k prediction on a CUDA device (DistMult and ComplEx "
+                                      "decoders on CUDA have one)" % type(self).__name__)
+        k, side = int(k), int(side)
+        if side not in (0, 1):
+            raise ValueError("side must be 0 (predict subjects) or 1 (predict objects), got %r" % (side,))
+        if not 1 <= k <= 128:
+            raise ValueError("k must be in [1, 128], got %d" % k)
+        triplets = np.asarray(triplets).reshape(-1, 3)
+        self._feed_test(getattr(self, 'test_graph', None), triplets[:1])
+        with torch.no_grad():
+            ids, energies = self.top_k_all(triplets, k, side, exclude_lists)
+        with np.errstate(over='ignore'):   # exp(+inf) of the padding: score 0
+            scores = (1.0 / (1.0 + np.exp(-energies.astype(np.float32)))).astype(np.float32)
+        return ids, energies, scores
+
     def register_for_test(self, triplets):
         self.test_graph = triplets
 

@@ -806,14 +806,57 @@ def block_aggregate_backward(X, W_forward, W_backward, G, graph, n_blocks, dWf=N
 
 class DistMultRanker(object):
     """Fused all-entity scoring + ranking over one entity code matrix (distmult_rank, include/rgcn_b200.h): the
-    hi/lo split of `codes` is made once and reused by every chunk / corruption side."""
-    _RANK, _WORKSPACE = "distmult_rank", "distmult_rank_workspace_bytes"
+    hi/lo split of `codes` is made once and reused by every chunk / corruption side, by rank and top_k alike (both
+    workspaces start with the split)."""
+    _RANK, _WORKSPACE, _TOPK = "distmult_rank", "distmult_rank_workspace_bytes", "distmult_topk"
+    # device bytes one top_k call may use beyond the split of `codes`; more queries than fit go in several calls
+    TOPK_CHUNK_BYTES = 1 << 30
 
     def __init__(self, codes, rel):
         _check_cuda_f32("codes", codes)
         _check_cuda_f32("relation table", rel)
         self.codes, self.rel = codes, rel
         self._ws, self._ws_n, self._split_ready = None, -1, False
+
+    def _check_rows(self, X, mask, name):
+        if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
+            raise _lib.RgcnError("X must be a contiguous CUDA int32 [n,3] tensor")
+        words = (self.codes.shape[0] + 31) // 32
+        if mask is not None and not (mask.is_cuda and mask.dtype == torch.int32
+                                     and mask.is_contiguous() and tuple(mask.shape) == (X.shape[0], words)):
+            raise _lib.RgcnError("%s must be a contiguous CUDA int32 [n, ceil(V/32)] tensor (bit masks)" % name)
+
+    def top_k(self, X, side, k, exclude_mask=None):
+        """The k entities of highest energy for every triple of X (int32 [n,3] CUDA; side 0 predicts subjects, 1
+        objects; the predicted column is not read), energy descending and the smaller id first on ties, never one
+        whose bit is set in exclude_mask (uint32 [n, ceil(V/32)] CUDA, as int32, or None).  Returns (ids int32
+        [n,k], energies float32 [n,k]) CUDA tensors; rows with fewer than k eligible entities end in (-1, -inf).
+        Queries go to the library in chunks whose workspace beyond the split stays under TOPK_CHUNK_BYTES."""
+        lib = _lib.load()
+        V, d = self.codes.shape
+        self._check_rows(X, exclude_mask, "exclude_mask")
+        k, n = int(k), X.shape[0]
+        split_bytes = lib.rgcn_topk_workspace_bytes(V, d, 0, k)
+        if split_bytes < 0:
+            _lib.check(int(split_bytes), "rgcn_topk_workspace_bytes")
+        per_row = lib.rgcn_topk_workspace_bytes(V, d, 1, k) - split_bytes
+        chunk = max(1, min(n, self.TOPK_CHUNK_BYTES // per_row))
+        dev = self.codes.device
+        nb = lib.rgcn_topk_workspace_bytes(V, d, chunk, k)
+        if self._ws is None or self._ws.numel() < nb:
+            self._ws, self._ws_n, self._split_ready = _workspace(nb, dev), -1, False
+        ids = torch.empty((n, k), dtype=torch.int32, device=dev)
+        energies = torch.empty((n, k), dtype=torch.float32, device=dev)
+        for c0 in range(0, max(n, 1), chunk):
+            c1 = min(n, c0 + chunk)
+            rc = getattr(lib, self._TOPK)(_ptr(self.codes), _ptr(self.rel), V, self.rel.shape[0], d, _ptr(X[c0:c1]),
+                                          c1 - c0, int(side), k,
+                                          _ptr(None if exclude_mask is None else exclude_mask[c0:c1]),
+                                          int(self._split_ready), _ptr(ids[c0:c1]), _ptr(energies[c0:c1]),
+                                          _ptr(self._ws), self._ws.numel(), _stream(dev))
+            _lib.check(rc, self._TOPK)
+            self._split_ready = True
+        return ids, energies
 
     def rank(self, X, side, known_mask=None):
         """X int32 [n,3] CUDA; side 0 = subjects corrupted, 1 = objects; known_mask uint32 [n, ceil(V/32)] CUDA or None.
@@ -846,4 +889,4 @@ class DistMultRanker(object):
 class ComplexRanker(DistMultRanker):
     """Fused all-entity scoring + ranking of the ComplEx decoder (rgcn_complex_rank): same interface and split reuse
     as DistMultRanker, the query rows are the complex products of complex.py:77-106."""
-    _RANK, _WORKSPACE = "rgcn_complex_rank", "rgcn_complex_rank_workspace_bytes"
+    _RANK, _WORKSPACE, _TOPK = "rgcn_complex_rank", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_topk"

@@ -103,6 +103,26 @@ def merge_settings(settings, n_entities, n_relations, n_train):
     return settings
 
 
+def build_chain(settings, splits, n_entities, n_relations, device):
+    """Encoder, decoder and Scorer of a run: the settings merged with the dataset sizes (train.py:69-86), the
+    model built by the factory on `device` with the train split as its graph, and every split registered with the
+    Scorer for the filtered metrics.  Returns (encoder, model, scorer)."""
+    train = splits['train']
+    merge_settings(settings, n_entities, n_relations, len(train))
+    encoder = model_builder.build_encoder(settings['Encoder'], train)
+    model = model_builder.build_decoder(encoder, settings['Decoder'])
+    model.set_device(device)
+    model.preprocess(train)
+    model.register_for_test(train)
+    model.initialize_train()
+
+    scorer = evaluation.Scorer(settings['Evaluation'])
+    for part in (train, splits['valid'], splits['test']):
+        scorer.register_data(part)
+    scorer.register_model(model)
+    return encoder, model, scorer
+
+
 def sample_edge_neighborhood_fast(triples, n_entities, sample_size):
     """The same sampler in the library (csrc/sampler.cu): Fenwick trees instead of an O(V) np.random.choice per
     draw (~5 s -> ~10 ms for 30 000 edges of FB15k-237); seeded from numpy's global stream."""
@@ -259,20 +279,8 @@ def main(argv=None):
     else:
         splits, entities, relations = load_dataset(args.dataset)
     train, valid, test = splits['train'], splits['valid'], splits['test']
-    merge_settings(settings, len(entities), len(relations), len(train))
+    encoder, model, scorer = build_chain(settings, splits, len(entities), len(relations), args.device)
     general, opt = settings['General'], settings['Optimizer']
-
-    encoder = model_builder.build_encoder(settings['Encoder'], train)
-    model = model_builder.build_decoder(encoder, settings['Decoder'])
-    model.set_device(args.device)
-    model.preprocess(train)
-    model.register_for_test(train)
-    model.initialize_train()
-
-    scorer = evaluation.Scorer(settings['Evaluation'])
-    for part in (train, valid, test):
-        scorer.register_data(part)
-    scorer.register_model(model)
 
     ns = auxilliaries.NegativeSampler(int(general['NegativeSampleRate']), len(entities))
     adj_list = [[] for _ in entities]

@@ -6,7 +6,8 @@ the same shapes next to the feature-input basis layer, the highway
 skip connection next to the plain GEMM of its shape, and the diagonal R-GCN layer (Name=gcn_diag) next to the basis
 layer and at bench.py's synthetic shape.  `python scripts/bench_secondary.py --gcn-diag` runs only that last section;
 `--variational` runs only the variational head (both variants at the FB15k-237 shape) next to an unfused torch
-composition."""
+composition; `--topk` runs only the fused top-k prediction at the FB15k-237 test shape next to the fused rank and an
+unfused torch top-k."""
 import json
 import subprocess
 import sys
@@ -18,6 +19,7 @@ import torch
 sys.path.insert(0, ".")
 from bench import synthetic_kg  # noqa: E402
 from relationprediction_b200 import _lib, ops  # noqa: E402
+from relationprediction_b200.decoders.bilinear_diag import BilinearDiag  # noqa: E402
 
 dev = torch.device("cuda", 0)
 flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
@@ -191,6 +193,81 @@ def variational_case(name, V, d, w, rounds=3):
 if "--variational" in sys.argv:
     variational_case("variational_gcn_fb15k237_V14541_d500_w500", 14541, 500, 500)
     variational_case("variational_embedding_fb15k237_V14541_w500", 14541, 0, 500)
+    print(json.dumps(out, indent=1))
+    sys.exit(0)
+
+# ---- top-k prediction (distmult_topk / rgcn_complex_topk) next to the fused rank and an unfused torch top-k ----
+def topk_case(name, ranker_cls, V, d, n, ks, chunk=4096, rounds=3):
+    """All n queries on both sides: the fused top-k, the fused rank of the same queries (rank_all's loop) and the
+    unfused torch path (q @ codes.T, masked fill, torch.topk; query rows formed by torch), alternated `rounds`
+    times, L2 flushed between calls; medians.  Every path gets the same random exclusion masks (~20 entities a
+    row).  Algorithmic bytes of the fused top-k: codes read once per 128-query M tile (hi + lo planes), the query
+    rows and masks, the candidate slab written and read back, the answers; flops 2 n V d x 3 (3xTF32)."""
+    g = torch.Generator(device=dev).manual_seed(0)
+    cd = torch.randn(V, d, device=dev, generator=g) * 0.3
+    rl = torch.randn(237, d, device=dev, generator=g)
+    Xq = torch.stack([torch.randint(0, V, (n,), device=dev, generator=g), torch.randint(0, 237, (n,), device=dev, generator=g),
+                      torch.randint(0, V, (n,), device=dev, generator=g)], 1).int().contiguous()
+    words = (V + 31) // 32
+    rng = np.random.RandomState(0)
+    excl = rng.randint(0, V, (n, 20))
+    mask = torch.as_tensor(BilinearDiag.known_bit_mask(list(excl), V), device=dev)
+    dense = torch.zeros(n, V, dtype=torch.bool, device=dev)
+    dense[torch.arange(n, device=dev).repeat_interleave(20), torch.as_tensor(excl.reshape(-1), device=dev)] = True
+    complex_ = ranker_cls is ops.ComplexRanker
+
+    def torch_q(X, side):
+        kept = cd[X[:, 2].long()] if side == 0 else cd[X[:, 0].long()]
+        b = rl[X[:, 1].long()]
+        if not complex_:
+            return b * kept
+        h = d // 2
+        kr, ki, br, bi = kept[:, :h], kept[:, h:], b[:, :h], b[:, h:]
+        if side == 0:
+            return torch.cat([br * kr + bi * ki, br * ki - bi * kr], 1)
+        return torch.cat([kr * br - ki * bi, ki * br + kr * bi], 1)
+
+    res = {"V": V, "d": d, "n": n, "gpu": card, "decoder": "complex" if complex_ else "distmult", "k": {}}
+    for k in ks:
+        def fused():
+            rk = ranker_cls(cd, rl)
+            for c0 in range(0, n, chunk):
+                for side in (0, 1):
+                    rk.top_k(Xq[c0:c0 + chunk], side, k, mask[c0:c0 + chunk])
+
+        def rank():
+            rk = ranker_cls(cd, rl)
+            for c0 in range(0, n, chunk):
+                for side in (0, 1):
+                    rk.rank(Xq[c0:c0 + chunk], side, mask[c0:c0 + chunk])
+
+        def unfused():
+            with torch.no_grad():
+                for c0 in range(0, n, chunk):
+                    for side in (0, 1):
+                        e = torch_q(Xq[c0:c0 + chunk], side) @ cd.T
+                        e.masked_fill_(dense[c0:c0 + chunk], float("-inf"))
+                        torch.topk(e, k, dim=1)
+        fns = {"fused_topk": fused, "fused_rank": rank, "unfused_torch_topk": unfused}
+        ms = {nm: [] for nm in fns}
+        for _ in range(rounds):
+            for nm, f in fns.items():
+                ms[nm].append(timeit(f, n=3, warm=1))
+        med = {nm: float(np.median(v)) for nm, v in ms.items()}
+        tn = (V + 127) // 128
+        by = 2 * (2 * n * V * d * 4 / 128) + 2 * n * (d * 4 + words * 4 + 2 * tn * k * 8 + k * 8)
+        fl = 2 * 2 * n * V * d * 3
+        res["k"][k] = {"medians_ms": med, "runs_ms": ms, "topk_over_rank": med["fused_topk"] / med["fused_rank"],
+                       "speedup_vs_unfused": med["unfused_torch_topk"] / med["fused_topk"],
+                       "bytes_algorithmic": by, "flops": fl, "topk_TFLOPs": fl / med["fused_topk"] / 1e9}
+    out[name] = res
+    del cd, rl, Xq, dense, mask
+    torch.cuda.empty_cache()
+
+
+if "--topk" in sys.argv:
+    for cls in (ops.DistMultRanker, ops.ComplexRanker):
+        topk_case("topk_fb15k237_%s_V14541_d500_n20466_both_sides" % cls.__name__, cls, 14541, 500, 20466, (1, 10, 100))
     print(json.dumps(out, indent=1))
     sys.exit(0)
 
