@@ -550,6 +550,50 @@ int rgcn_complex_topk(const float* codes, const float* rel, int32_t V, int32_t V
                       int64_t n, int side, int32_t k, const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
                       float* energies, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Relation prediction, fused: (h, ?, t) queries scored against every relation.  Both decoders' energies are linear
+ * in the relation row, so for every triple t = (h, r, t') of X
+ *   DistMult: q = codes[h] * codes[t']
+ *   ComplEx:  q = [hr tr + hi ti, hr ti - hi tr]    (h = codes[h], t = codes[t'], [real | imaginary] halves)
+ * and energy(t, r) = sum_k q[k] * rel[r, k] (3xTF32 GEMM) equals the decoder's energy of (h, r, t').
+ * Only the first R rows of `rel` are candidates: rows R..Vrel-1 (the R-GCN encoders keep a [V, d] relation table)
+ * are never scored, counted or returned.  1 <= R <= Vrel, else RGCN_ERR_INVALID.
+ *
+ * *_relation_rank: the ranking rules of distmult_rank with relations in place of entities:
+ *   raw_rank[t]      = #{r < R : sigmoid(energy(t, r)) >= sigmoid(energy(t, gold))}, gold = X[t, 1] in [0, R)
+ *   filtered_rank[t] = raw_rank[t] - #{known r with score >= gold} + 1   (only when filtered_rank != NULL)
+ *   known_mask : uint32 [n, ceil(R/32)] device, bit r of row t = (h, r, t') is a known triple; required for
+ *                filtered ranks.
+ *   workspace  : rgcn_relation_rank_workspace_bytes(R, d, n).
+ * *_relation_topk: the k relations of highest energy per row, energy descending, the smaller relation id first on
+ *   ties, never one whose bit is set in exclude_mask (uint32 [n, ceil(R/32)] device, or NULL); the tail of a row
+ *   with fewer than k eligible relations is id -1, energy -inf.  1 <= k <= 128.  The relation column of X is not
+ *   read.  ids int32 [n, k], energies float32 [n, k] device; bitwise repeatable.
+ *   workspace  : rgcn_relation_topk_workspace_bytes(R, d, n, k), linear in n.
+ * Both workspaces start with the hi/lo split of rel[0:R] in the same place, so reuse_split != 0 skips re-splitting
+ * when a relation workspace (rank or top-k) is passed again with an unchanged relation table.  The split is not that
+ * of the entity entry points: never pass an entity workspace with reuse_split != 0.
+ * Errors: RGCN_ERR_INVALID (null pointers, V <= 0, d % 4 != 0, R out of range, k out of range, filtered ranks
+ * without a known mask), RGCN_ERR_WORKSPACE.  The two *_workspace_bytes functions return RGCN_ERR_INVALID (-1) on
+ * bad arguments (R <= 0, d % 4 != 0, n < 0, k out of range).
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_relation_rank_workspace_bytes(int32_t R, int32_t d, int64_t n);
+int distmult_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                           const int32_t* X, int64_t n, const uint32_t* known_mask, int reuse_split,
+                           int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                           void* stream);
+int rgcn_complex_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                               const int32_t* X, int64_t n, const uint32_t* known_mask, int reuse_split,
+                               int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                               void* stream);
+int64_t rgcn_relation_topk_workspace_bytes(int32_t R, int32_t d, int64_t n, int32_t k);
+int distmult_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                           const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask, int reuse_split,
+                           int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+int rgcn_complex_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                               const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask, int reuse_split,
+                               int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -29,6 +29,8 @@ EXPORTED_SYMBOLS = [
     "distmult_backward_slices", "rgcn_block_slice_sumsq_workspace_bytes", "rgcn_block_slice_sumsq",
     "rgcn_complex_forward", "rgcn_complex_backward", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_rank",
     "rgcn_topk_workspace_bytes", "distmult_topk", "rgcn_complex_topk",
+    "rgcn_relation_rank_workspace_bytes", "distmult_relation_rank", "rgcn_complex_relation_rank",
+    "rgcn_relation_topk_workspace_bytes", "distmult_relation_topk", "rgcn_complex_relation_topk",
 ]
 
 RGCN_NORM_CANONICAL, RGCN_NORM_EXPLICIT, RGCN_NORM_NONE = 0, 1, 2
@@ -194,6 +196,18 @@ def _declare(lib):
         getattr(lib, name).restype = c_int
         getattr(lib, name).argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, c_int32, vp, c_int, vp,
                                        vp, vp, c_int64, vp]
+    lib.rgcn_relation_rank_workspace_bytes.restype = c_int64
+    lib.rgcn_relation_rank_workspace_bytes.argtypes = [c_int32, c_int32, c_int64]
+    lib.rgcn_relation_topk_workspace_bytes.restype = c_int64
+    lib.rgcn_relation_topk_workspace_bytes.argtypes = [c_int32, c_int32, c_int64, c_int32]
+    for name in ("distmult_relation_rank", "rgcn_complex_relation_rank"):
+        getattr(lib, name).restype = c_int
+        getattr(lib, name).argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, vp, c_int64, vp, c_int, vp, vp, vp,
+                                       c_int64, vp]
+    for name in ("distmult_relation_topk", "rgcn_complex_relation_topk"):
+        getattr(lib, name).restype = c_int
+        getattr(lib, name).argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, vp, c_int64, c_int32, vp, c_int,
+                                       vp, vp, vp, c_int64, vp]
 
 
 def load():

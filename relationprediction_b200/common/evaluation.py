@@ -52,10 +52,12 @@ class Scorer(object):
         self.settings = settings
         self.known_object_triples = {}
         self.known_subject_triples = {}
+        self.known_relation_triples = {}
         self.model = None
 
     def register_data(self, triples):
-        # de-duplicated lists, like extend_triple_dict (common/evaluation.py:232-245)
+        # de-duplicated lists, like extend_triple_dict (common/evaluation.py:232-245); known_relation_triples[(s, o)]
+        # lists the relations linking s to o, for the relation queries (s, ?, o)
         for s, r, o in np.asarray(triples).reshape(-1, 3).tolist():
             lo = self.known_object_triples.setdefault((s, r), [])
             if o not in lo:
@@ -63,6 +65,9 @@ class Scorer(object):
             ls = self.known_subject_triples.setdefault((o, r), [])
             if s not in ls:
                 ls.append(s)
+            lr = self.known_relation_triples.setdefault((s, o), [])
+            if r not in lr:
+                lr.append(r)
 
     def register_degrees(self, triples):  # kept for call compatibility (train.py:106); unused here
         pass
@@ -87,6 +92,29 @@ class Scorer(object):
             else:
                 exclude = [self.known_object_triples.get((t[0], t[1]), []) for t in tl]
         return self.model.predict_top_k(triples, k, side, exclude)
+
+    def predict_top_k_relations(self, triples, k, filtered=True):
+        """The k most likely relations for each (s, ?, o) pair of `triples` through the model's fused path
+        (Model.predict_top_k_relations; the relation column is not read).  filtered=True leaves out every relation
+        r with (s, r, o) in a registered split (known_relation_triples); filtered=False excludes nothing.  Returns
+        numpy (ids, energies, scores), each [n, k]."""
+        triples = np.asarray(triples).reshape(-1, 3)
+        exclude = None
+        if filtered:
+            exclude = [self.known_relation_triples.get((t[0], t[2]), []) for t in triples.tolist()]
+        return self.model.predict_top_k_relations(triples, k, exclude)
+
+    def compute_relation_mrr_scores(self, triples):
+        """Relation prediction metrics: each triple's relation ranked among all relations for its (s, o) pair by
+        the model's fused relation ranker, raw and filtered by known_relation_triples with the entity ranks' rules.
+        Returns an MrrScore (one rank per triple) whose summary prints the same Raw / Filtered table."""
+        triples = np.asarray(triples).reshape(-1, 3)
+        score = MrrScore()
+        known = [self.known_relation_triples.get((t[0], t[2]), []) for t in triples.tolist()]
+        raw, filt = self.model.rank_all_relations(triples, known)
+        score.raw_ranks.extend(np.asarray(raw).tolist())
+        score.filtered_ranks.extend(np.asarray(filt).tolist())
+        return score
 
     def compute_scores(self, triples, verbose=False):
         return self.compute_mrr_scores(triples, verbose)

@@ -1641,3 +1641,156 @@ extern "C" int rgcn_complex_topk(const float* codes, const float* rel, int32_t V
   return topk_with_queries(launch_complex_rank_prepare, "rgcn_complex_topk", codes, rel, V, Vrel, d, X, n, side, k,
                            exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
 }
+
+// ------------------------------------------------------------------------------------------------
+// Relation prediction over all relations, fused (DistMult and ComplEx): queries (h, ?, t)
+// ------------------------------------------------------------------------------------------------
+// Both decoders' energies are linear in the relation row, so a pair query is one row Q[t] (the decoder's relation
+// prepare kernel) and the energies of all relations are Q @ rel[0:R]^T: the entity-side scoring GEMM with its rank or
+// top-k epilogue, run with Bt = the hi/lo split of the first R relation rows and N = R.  Rows R..Vrel-1 of `rel` (the
+// R-GCN encoders keep a [V, d] relation table) are never split, scored, counted or returned.
+// Workspace layouts: rank [hi R*d | lo R*d | Q n*d | gold_sig n | gold_col n | raw_cnt n | known_cnt n] (that of
+// rank_with_queries with V = R), top-k [hi R*d | lo R*d | Q n*d | cand n*ceil(R/128)*k] (that of topk_with_queries);
+// one relation workspace with its split serves both, never the entity split.
+typedef int (*RelationPrepareFn)(const float*, const float*, int, const int32_t*, int64_t, float*, float*, int32_t*,
+                                 cudaStream_t);
+
+static bool relation_sizes_ok(int32_t R, int32_t d, int64_t n, int64_t per_row) {
+  return R > 0 && d > 0 && d % 4 == 0 && n >= 0 && (n == 0 || per_row <= ((int64_t)1 << 60) / n);
+}
+
+extern "C" int64_t rgcn_relation_rank_workspace_bytes(int32_t R, int32_t d, int64_t n) {
+  if (!relation_sizes_ok(R, d, n, (int64_t)d * 4 + 16)) {
+    rgcn_set_error("rgcn_relation_rank_workspace_bytes: bad arguments (need R > 0, d > 0, d % 4 == 0, n >= 0)");
+    return RGCN_ERR_INVALID;
+  }
+  return distmult_rank_workspace_bytes(R, d, n);
+}
+
+extern "C" int64_t rgcn_relation_topk_workspace_bytes(int32_t R, int32_t d, int64_t n, int32_t k) {
+  if (!relation_sizes_ok(R, d, n, 0) || k < 1 || k > 128 ||
+      (n > 0 && topk_per_row_bytes(R, d, k) > ((int64_t)1 << 60) / n)) {
+    rgcn_set_error("rgcn_relation_topk_workspace_bytes: bad arguments (need R > 0, d > 0, d % 4 == 0, n >= 0, "
+                   "1 <= k <= 128)");
+    return RGCN_ERR_INVALID;
+  }
+  return rgcn_topk_workspace_bytes(R, d, n, k);
+}
+
+// the argument checks shared by the four relation entry points (before any device work)
+static bool relation_args_ok(const char* who, const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                             int32_t R, int32_t d, const int32_t* X, int64_t n, const void* out1, const void* out2,
+                             const void* workspace) {
+  if (!codes || !rel || (n > 0 && (!X || !out1 || !out2)) || !workspace || V <= 0 || d <= 0 || d % 4 != 0 || n < 0 ||
+      n > 0x7fffffffLL) {
+    rgcn_set_error(std::string(who) + ": bad arguments (need non-null pointers, V > 0, d % 4 == 0)");
+    return false;
+  }
+  if (R < 1 || R > Vrel) {
+    rgcn_set_error(std::string(who) + ": R = " + std::to_string(R) + " relations, need 1 <= R <= Vrel = " +
+                   std::to_string(Vrel));
+    return false;
+  }
+  return true;
+}
+
+static int relation_rank(RelationPrepareFn prepare, const char* who, const float* codes, const float* rel, int32_t V,
+                         int32_t Vrel, int32_t R, int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
+                         int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
+                         int64_t workspace_bytes, cudaStream_t st) {
+  if (!relation_args_ok(who, codes, rel, V, Vrel, R, d, X, n, raw_rank, raw_rank, workspace)) return RGCN_ERR_INVALID;
+  if (filtered_rank && !known_mask) {
+    rgcn_set_error(std::string(who) + ": bad arguments (filtered ranks need a known mask)");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t need = rgcn_relation_rank_workspace_bytes(R, d, n);
+  if (need < 0) return (int)need;
+  if (workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_relation_rank_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  Carver ws(workspace, workspace_bytes);
+  float* hi = ws.take<float>((int64_t)R * d);
+  float* lo = ws.take<float>((int64_t)R * d);
+  float* Q = ws.take<float>(n * d);
+  float* gold_sig = ws.take<float>(n);
+  int32_t* gold_col = ws.take<int32_t>(n);
+  int32_t* raw_cnt = ws.take<int32_t>(n);
+  int32_t* known_cnt = ws.take<int32_t>(n);
+  int rc = RGCN_OK;
+  if (!reuse_split) rc = launch_gemm_split_b(rel, d, R, d, /*transposed=*/0, hi, lo, st);
+  if (rc || n == 0) return rc;
+  rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
+  if (rc) return rc;
+  rc = prepare(codes, rel, d, X, n, Q, gold_sig, gold_col, st);
+  if (rc) return rc;
+  rc = launch_gemm_rank_tf32x3(Q, d, hi, lo, d, (int)n, R, d, gold_sig, gold_col, known_mask, (R + 31) / 32, raw_cnt,
+                               known_cnt, st);
+  if (rc) return rc;
+  return launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
+}
+
+static int relation_topk(RelationPrepareFn prepare, const char* who, const float* codes, const float* rel, int32_t V,
+                         int32_t Vrel, int32_t R, int32_t d, const int32_t* X, int64_t n, int32_t k,
+                         const uint32_t* exclude_mask, int reuse_split, int32_t* ids, float* energies, void* workspace,
+                         int64_t workspace_bytes, cudaStream_t st) {
+  if (!relation_args_ok(who, codes, rel, V, Vrel, R, d, X, n, ids, energies, workspace)) return RGCN_ERR_INVALID;
+  if (k < 1 || k > 128) {
+    rgcn_set_error(std::string(who) + ": k = " + std::to_string(k) + " is out of range (1 <= k <= 128)");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t need = rgcn_relation_topk_workspace_bytes(R, d, n, k);
+  if (need < 0) return (int)need;
+  if (workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_relation_topk_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  const int tn = (R + 127) / 128;
+  Carver ws(workspace, workspace_bytes);
+  float* hi = ws.take<float>((int64_t)R * d);
+  float* lo = ws.take<float>((int64_t)R * d);
+  float* Q = ws.take<float>(n * d);
+  uint2* cand = ws.take<uint2>(n * tn * k);
+  int rc = RGCN_OK;
+  if (!reuse_split) rc = launch_gemm_split_b(rel, d, R, d, /*transposed=*/0, hi, lo, st);
+  if (rc || n == 0) return rc;
+  rc = prepare(codes, rel, d, X, n, Q, nullptr, nullptr, st);
+  if (rc) return rc;
+  rc = launch_gemm_topk_tf32x3(Q, d, hi, lo, d, (int)n, R, d, exclude_mask, (R + 31) / 32, k, cand, st);
+  if (rc) return rc;
+  return launch_topk_merge(cand, n, tn * k, k, ids, energies, st);
+}
+
+extern "C" int distmult_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                      int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
+                                      int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
+                                      int64_t workspace_bytes, void* stream) {
+  return relation_rank(launch_distmult_relation_prepare, "distmult_relation_rank", codes, rel, V, Vrel, R, d, X, n,
+                       known_mask, reuse_split, raw_rank, filtered_rank, workspace, workspace_bytes,
+                       (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_complex_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                          int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
+                                          int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
+                                          int64_t workspace_bytes, void* stream) {
+  return relation_rank(launch_complex_relation_prepare, "rgcn_complex_relation_rank", codes, rel, V, Vrel, R, d, X, n,
+                       known_mask, reuse_split, raw_rank, filtered_rank, workspace, workspace_bytes,
+                       (cudaStream_t)stream);
+}
+
+extern "C" int distmult_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                      int32_t d, const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask,
+                                      int reuse_split, int32_t* ids, float* energies, void* workspace,
+                                      int64_t workspace_bytes, void* stream) {
+  return relation_topk(launch_distmult_relation_prepare, "distmult_relation_topk", codes, rel, V, Vrel, R, d, X, n, k,
+                       exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_complex_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                          int32_t d, const int32_t* X, int64_t n, int32_t k,
+                                          const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
+                                          float* energies, void* workspace, int64_t workspace_bytes, void* stream) {
+  return relation_topk(launch_complex_relation_prepare, "rgcn_complex_relation_topk", codes, rel, V, Vrel, R, d, X, n,
+                       k, exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+}

@@ -229,6 +229,53 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// ---- fused all-relation scoring + ranking / top-k: pair queries (h, ?, t) ----------------------------------------
+// The energy of complex.py:38-41, (hr rr) . tr + (hi rr) . ti + (hr ri) . ti - (hi ri) . tr, is linear in the
+// relation row [rr | ri]:  e = rr . (hr tr + hi ti) + ri . (hr ti - hi tr),  so
+//   Q = [hr tr + hi ti, hr ti - hi tr],  gold = r,  gold_sig[t] = sigmoid(<Q[t], rel[r]>)
+// (gold_sig == nullptr: Q only; the relation column of X is then not read).
+template <int W>
+__global__ void __launch_bounds__(256)
+    k_complex_relation_prepare(const float* __restrict__ codes, const float* __restrict__ rel, int d,
+                               const int32_t* __restrict__ X, int64_t n, float* __restrict__ Q,
+                               float* __restrict__ gold_sig, int32_t* __restrict__ gold_col) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int h = d >> 1;
+  for (int64_t t = (int64_t)blockIdx.x * 8 + warp; t < n; t += (int64_t)gridDim.x * 8) {
+    const int s = __ldg(X + 3 * t), o = __ldg(X + 3 * t + 2);
+    const int r = gold_sig ? __ldg(X + 3 * t + 1) : 0;
+    const float* eh = codes + (size_t)s * d;
+    const float* et = codes + (size_t)o * d;
+    const float* rr = rel + (size_t)r * d;
+    float* q = Q + (size_t)t * d;
+    float e = 0.f;
+    for (int k = lane * W; k < h; k += 32 * W) {
+      float hr[W], hi[W], tr[W], ti[W], br[W], bi[W], qr[W], qi[W];
+      Vec<W>::load(eh + k, hr), Vec<W>::load(eh + h + k, hi);
+      Vec<W>::load(et + k, tr), Vec<W>::load(et + h + k, ti);
+#pragma unroll
+      for (int j = 0; j < W; ++j) {
+        qr[j] = fmaf(hr[j], tr[j], hi[j] * ti[j]);
+        qi[j] = fmaf(hr[j], ti[j], -hi[j] * tr[j]);
+      }
+      Vec<W>::store(q + k, qr), Vec<W>::store(q + h + k, qi);
+      if (gold_sig) {
+        Vec<W>::load(rr + k, br), Vec<W>::load(rr + h + k, bi);
+#pragma unroll
+        for (int j = 0; j < W; ++j) {
+          e = fmaf(qr[j], br[j], e);
+          e = fmaf(qi[j], bi[j], e);
+        }
+      }
+    }
+    e = warp_sum(e);
+    if (lane == 0 && gold_sig) {
+      gold_sig[t] = 1.0f / (1.0f + expf(-e));
+      gold_col[t] = r;
+    }
+  }
+}
+
 int check_launch(const char* what) {
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), what);
@@ -285,4 +332,14 @@ int launch_complex_rank_prepare(const float* codes, const float* rel, int d, con
     k_complex_rank_prepare<2><<<blocks_for_triples(n), 256, 0, st>>>(codes, rel, d, X, n, side, Q, gold_sig,
                                                                      gold_col);
   return check_launch("k_complex_rank_prepare");
+}
+
+int launch_complex_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n,
+                                    float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st) {
+  if (n == 0) return RGCN_OK;
+  if (d % 8 == 0)
+    k_complex_relation_prepare<4><<<blocks_for_triples(n), 256, 0, st>>>(codes, rel, d, X, n, Q, gold_sig, gold_col);
+  else
+    k_complex_relation_prepare<2><<<blocks_for_triples(n), 256, 0, st>>>(codes, rel, d, X, n, Q, gold_sig, gold_col);
+  return check_launch("k_complex_relation_prepare");
 }

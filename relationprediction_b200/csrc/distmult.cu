@@ -174,6 +174,44 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// ---- fused all-relation scoring + ranking / top-k: pair queries (h, ?, t) ----------------------------------------
+// The energy is linear in the relation row: e(h, r, t) = <codes[h] * codes[t], rel[r]>, so Q[t] = codes[h] * codes[t]
+// is scored against every relation row by the same GEMM.  gold_sig[t] = sigmoid(<Q[t], rel[r]>), gold_col[t] = r
+// (gold_sig == nullptr: Q only; the relation column of X is then not read).
+__global__ void __launch_bounds__(256)
+    k_relation_prepare(const float* __restrict__ codes, const float* __restrict__ rel, int d,
+                       const int32_t* __restrict__ X, int64_t n, float* __restrict__ Q, float* __restrict__ gold_sig,
+                       int32_t* __restrict__ gold_col) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int d4 = d >> 2;
+  for (int64_t t = (int64_t)blockIdx.x * 8 + warp; t < n; t += (int64_t)gridDim.x * 8) {
+    const int s = __ldg(X + 3 * t), o = __ldg(X + 3 * t + 2);
+    const int r = gold_sig ? __ldg(X + 3 * t + 1) : 0;
+    const float4* eh = reinterpret_cast<const float4*>(codes + (size_t)s * d);
+    const float4* et = reinterpret_cast<const float4*>(codes + (size_t)o * d);
+    const float4* rr = reinterpret_cast<const float4*>(rel + (size_t)r * d);
+    float4* q = reinterpret_cast<float4*>(Q + (size_t)t * d);
+    float e = 0.f;
+    for (int i = lane; i < d4; i += 32) {
+      const float4 a = __ldg(eh + i), b = __ldg(et + i);
+      const float4 p = make_float4(a.x * b.x, a.y * b.y, a.z * b.z, a.w * b.w);
+      q[i] = p;
+      if (gold_sig) {
+        const float4 c = __ldg(rr + i);
+        e = fmaf(p.x, c.x, e);
+        e = fmaf(p.y, c.y, e);
+        e = fmaf(p.z, c.z, e);
+        e = fmaf(p.w, c.w, e);
+      }
+    }
+    e = warp_sum(e);
+    if (lane == 0 && gold_sig) {
+      gold_sig[t] = 1.0f / (1.0f + expf(-e));
+      gold_col[t] = r;
+    }
+  }
+}
+
 // raw rank = #{score >= gold}; filtered rank = raw - #{known with score >= gold} + 1 (common/evaluation.py:148-152)
 __global__ void k_rank_finalize(const int32_t* __restrict__ raw_cnt, const int32_t* __restrict__ known_cnt, int64_t n,
                                 int32_t* __restrict__ raw_rank, int32_t* __restrict__ filtered_rank) {
@@ -228,6 +266,13 @@ int launch_distmult_rank_prepare(const float* codes, const float* rel, int d, co
   if (n == 0) return RGCN_OK;
   k_rank_prepare<<<blocks_for_triples(n), 256, 0, st>>>(codes, rel, d, X, n, side, Q, gold_sig, gold_col);
   return check_launch("k_rank_prepare");
+}
+
+int launch_distmult_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n,
+                                     float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st) {
+  if (n == 0) return RGCN_OK;
+  k_relation_prepare<<<blocks_for_triples(n), 256, 0, st>>>(codes, rel, d, X, n, Q, gold_sig, gold_col);
+  return check_launch("k_relation_prepare");
 }
 
 int launch_distmult_rank_finalize(const int32_t* raw_cnt, const int32_t* known_cnt, int64_t n, int32_t* raw_rank,

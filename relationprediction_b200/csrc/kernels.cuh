@@ -211,6 +211,10 @@ int launch_var_deinterleave(const float* dWint, int d, int w, float* dWmu, float
 // (gold_sig == nullptr: Q only; the gold column of X is then not read)
 int launch_distmult_rank_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
                                  float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
+// relation queries (h, ?, t): Q[t] = codes[h] * codes[t], gold = r, gold_sig[t] = sigmoid(<Q[t], rel[r]>)
+// (gold_sig == nullptr: Q only; the relation column of X is then not read)
+int launch_distmult_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n,
+                                     float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
 int launch_distmult_rank_finalize(const int32_t* raw_cnt, const int32_t* known_cnt, int64_t n, int32_t* raw_rank,
                                   int32_t* filtered_rank, cudaStream_t st);
 int launch_distmult_forward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N,
@@ -231,3 +235,7 @@ int launch_complex_backward(const float* codes, const float* rel, int d, const i
 // gold = o.  gold_sig[t] = sigmoid(<Q[t], codes[gold]>)
 int launch_complex_rank_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
                                 float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
+// relation queries (h, ?, t): Q[t] = [hr tr + hi ti, hr ti - hi tr], gold = r, gold_sig[t] = sigmoid(<Q[t], rel[r]>)
+// (gold_sig == nullptr: Q only; the relation column of X is then not read)
+int launch_complex_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n,
+                                    float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);

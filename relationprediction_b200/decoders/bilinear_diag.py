@@ -51,7 +51,7 @@ class BilinearDiag(Model):
         return ops.distmult
 
     def _ranker(self, codes, rel):
-        return ops.DistMultRanker(codes, rel)
+        return ops.DistMultRanker(codes, rel, self.relation_count)
 
     def compute_codes(self, mode='train'):
         """(e1s, rs, e2s) row gathers (bilinear_diag.py:14-24) -- only the all-entity scoring GEMMs
@@ -136,6 +136,53 @@ class BilinearDiag(Model):
             if exclude_lists is not None:
                 mask = torch.as_tensor(self.known_bit_mask(exclude_lists[c0:c0 + chunk], V), device=codes.device)
             i, e = ranker.top_k(X, side, k, mask)
+            ids.append(i)
+            energies.append(e)
+        if not ids:
+            return np.zeros((0, k), np.int64), np.zeros((0, k), np.float32)
+        return torch.cat(ids).cpu().numpy().astype(np.int64), torch.cat(energies).cpu().numpy()
+
+    # ---- relation queries (h, ?, t): library entries distmult_relation_rank / distmult_relation_topk ----
+    def _relation_ranker(self):
+        """The ranker over the test-mode codes, with R = RelationCount relation candidates (rows 0..R-1 of the
+        relation table)."""
+        subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='test')
+        assert subject_codes is object_codes, "fused relation prediction expects one shared entity code matrix"
+        return self._ranker(subject_codes.contiguous(), relation_codes.contiguous())
+
+    def rank_relations_all(self, triplets, known_relation_lists, chunk=4096):
+        """Raw and filtered ranks of every triple's relation among the RelationCount relations for its (head, tail)
+        pair, with the counting rules of rank_all; known_relation_lists[t] lists the relations r with (h, r, t) in
+        any split.  One encoder pass, one split of the relation table.  Returns (raw, filtered) int64 arrays."""
+        ranker = self._relation_ranker()
+        dev = ranker.codes.device
+        tri = np.ascontiguousarray(np.asarray(triplets, dtype=np.int32).reshape(-1, 3))
+        raw, filt = [], []
+        for c0 in range(0, len(tri), chunk):
+            X = torch.as_tensor(tri[c0:c0 + chunk], device=dev)
+            mask = torch.as_tensor(self.known_bit_mask(known_relation_lists[c0:c0 + chunk], self.relation_count),
+                                   device=dev)
+            r, f = ranker.rank_relations(X, mask)
+            raw.append(r)
+            filt.append(f)
+        return tuple(torch.cat(o).cpu().numpy().astype(np.int64) if o else np.zeros(0, np.int64) for o in (raw, filt))
+
+    def top_k_relations_all(self, triplets, k, exclude_lists=None, chunk=4096):
+        """The k relations of highest energy for every (head, ?, tail) pair of `triplets` (the relation column is
+        not read), among the RelationCount relations.  exclude_lists[t] lists the relations row t may not return (or
+        None).  Returns (ids int64 [n, k], energies float32 [n, k]); energy descending, the smaller id first on
+        ties; rows with fewer than k eligible relations end in (-1, -inf)."""
+        ranker = self._relation_ranker()
+        dev = ranker.codes.device
+        tri = np.ascontiguousarray(np.asarray(triplets, dtype=np.int32).reshape(-1, 3))
+        ids, energies = [], []
+        for c0 in range(0, len(tri), chunk):
+            X = torch.as_tensor(tri[c0:c0 + chunk], device=dev)
+            mask = None
+            if exclude_lists is not None:
+                mask = torch.as_tensor(self.known_bit_mask(exclude_lists[c0:c0 + chunk], self.relation_count),
+                                       device=dev)
+            i, e = ranker.top_k_relations(X, k, mask)
             ids.append(i)
             energies.append(e)
         if not ids:

@@ -18,7 +18,7 @@ class Complex(BilinearDiag):
         return ops.complex_score   # energies (:38-41), reduce_mean(weighted CE, pos_weight 1) (:43-45), L2 (:108-114)
 
     def _ranker(self, codes, rel):
-        return ops.ComplexRanker(codes, rel)
+        return ops.ComplexRanker(codes, rel, self.relation_count)
 
     def extract_real_and_imaginary(self, composite_vector):
         """(:71-75) columns [0, h) and [h, 2h) with h = int(dimension / 2)."""

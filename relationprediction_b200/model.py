@@ -127,6 +127,44 @@ class Model(object):
             scores = (1.0 / (1.0 + np.exp(-energies.astype(np.float32)))).astype(np.float32)
         return ids, energies, scores
 
+    def _relation_triplets(self, hook, triplets, check_relations):
+        if not hasattr(self, hook) or self.get_device().type != 'cuda':
+            raise NotImplementedError("%s has no fused relation prediction on a CUDA device (DistMult and ComplEx "
+                                      "decoders on CUDA have one)" % type(self).__name__)
+        triplets = np.asarray(triplets).reshape(-1, 3)
+        if len(triplets):
+            ent = triplets[:, [0, 2]]
+            if ent.min() < 0 or ent.max() >= self.entity_count:
+                raise ValueError("entity ids must be in [0, %d)" % self.entity_count)
+            if check_relations and (triplets[:, 1].min() < 0 or triplets[:, 1].max() >= self.relation_count):
+                raise ValueError("relation ids must be in [0, %d)" % self.relation_count)
+        self._feed_test(getattr(self, 'test_graph', None), triplets[:1])
+        return triplets
+
+    def rank_all_relations(self, triplets, known_relation_lists):
+        """Ranks of every triple's relation among the RelationCount relations for its (head, tail) pair, through the
+        decoder's fused relation ranker (one encoder pass for the whole set), fed like rank_all_entities.
+        known_relation_lists[t] lists the relations r with (head, r, tail) known; the filtered rank leaves them out
+        as the entity ranks do.  Returns numpy (raw, filtered) int64 [n]."""
+        triplets = self._relation_triplets('rank_relations_all', triplets, check_relations=True)
+        with torch.no_grad():
+            return self.rank_relations_all(triplets, known_relation_lists)
+
+    def predict_top_k_relations(self, triplets, k, exclude_lists=None):
+        """The k most likely relations for every (head, ?, tail) pair of `triplets` (the relation column is not
+        read) under the decoder's fused path, fed like predict_top_k.  exclude_lists[t] (optional) lists the
+        relations row t may not return.  Returns numpy (ids [n, k], energies [n, k], scores = float32
+        sigmoid(energies)); rows with fewer than k eligible relations end in id -1, energy -inf, score 0."""
+        k = int(k)
+        if not 1 <= k <= 128:
+            raise ValueError("k must be in [1, 128], got %d" % k)
+        triplets = self._relation_triplets('top_k_relations_all', triplets, check_relations=False)
+        with torch.no_grad():
+            ids, energies = self.top_k_relations_all(triplets, k, exclude_lists)
+        with np.errstate(over='ignore'):   # exp(+inf) of the padding: score 0
+            scores = (1.0 / (1.0 + np.exp(-energies.astype(np.float32)))).astype(np.float32)
+        return ids, energies, scores
+
     def register_for_test(self, triplets):
         self.test_graph = triplets
 

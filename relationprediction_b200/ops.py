@@ -809,14 +809,21 @@ class DistMultRanker(object):
     hi/lo split of `codes` is made once and reused by every chunk / corruption side, by rank and top_k alike (both
     workspaces start with the split)."""
     _RANK, _WORKSPACE, _TOPK = "distmult_rank", "distmult_rank_workspace_bytes", "distmult_topk"
-    # device bytes one top_k call may use beyond the split of `codes`; more queries than fit go in several calls
+    _REL_RANK, _REL_TOPK = "distmult_relation_rank", "distmult_relation_topk"
+    # device bytes one top_k / top_k_relations / rank_relations call may use beyond the split of its table; more
+    # queries than fit go in several calls
     TOPK_CHUNK_BYTES = 1 << 30
 
-    def __init__(self, codes, rel):
+    def __init__(self, codes, rel, relation_count=None):
+        """relation_count = R, the candidates of the relation queries: rows 0..R-1 of `rel` (default: all rows).
+        The R-GCN encoders' relation table has V rows of which only the first R are trained."""
         _check_cuda_f32("codes", codes)
         _check_cuda_f32("relation table", rel)
         self.codes, self.rel = codes, rel
+        self.relation_count = rel.shape[0] if relation_count is None else int(relation_count)
         self._ws, self._ws_n, self._split_ready = None, -1, False
+        # the relation queries keep their own workspace: its head is the split of rel[0:R], not of `codes`
+        self._rel_ws, self._rel_split_ready = None, False
 
     def _check_rows(self, X, mask, name):
         if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
@@ -885,8 +892,74 @@ class DistMultRanker(object):
         self._split_ready = True
         return raw, filt
 
+    # ---- relation queries (h, ?, t) over rel[0:R] (distmult_relation_rank / distmult_relation_topk) ----
+    def _relation_calls(self, X, mask, name, workspace_bytes):
+        """Checks X and the [n, ceil(R/32)] mask, sizes the relation workspace for chunks of at most
+        TOPK_CHUNK_BYTES beyond the split, and yields (c0, c1) per chunk; the split is marked ready after each."""
+        lib = _lib.load()
+        R, d = self.relation_count, self.codes.shape[1]
+        if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
+            raise _lib.RgcnError("X must be a contiguous CUDA int32 [n,3] tensor")
+        n, words = X.shape[0], (R + 31) // 32
+        if mask is not None and not (mask.is_cuda and mask.dtype == torch.int32
+                                     and mask.is_contiguous() and tuple(mask.shape) == (n, words)):
+            raise _lib.RgcnError("%s must be a contiguous CUDA int32 [n, ceil(R/32)] tensor (bit masks)" % name)
+        split_bytes = workspace_bytes(0)
+        if split_bytes < 0:
+            _lib.check(int(split_bytes), "relation workspace bytes")
+        chunk = max(1, min(n, self.TOPK_CHUNK_BYTES // max(1, workspace_bytes(1) - split_bytes)))
+        nb = workspace_bytes(chunk)
+        if self._rel_ws is None or self._rel_ws.numel() < nb:
+            self._rel_ws, self._rel_split_ready = _workspace(nb, self.codes.device), False
+        for c0 in range(0, max(n, 1), chunk):
+            yield c0, min(n, c0 + chunk)
+            self._rel_split_ready = True
+
+    def rank_relations(self, X, known_mask=None):
+        """Ranks of the relation X[t, 1] in [0, R) among all R relations for the pair (X[t, 0], X[t, 2]), by the
+        rules of rank: raw = #{r : score_r >= gold score}, filtered = raw - #{known r with score >= gold} + 1.
+        X int32 [n,3] CUDA; known_mask uint32 [n, ceil(R/32)] CUDA (as int32) or None.  Returns (raw_rank,
+        filtered_rank or None) int32 CUDA tensors."""
+        lib = _lib.load()
+        R, d = self.relation_count, self.codes.shape[1]
+        dev = self.codes.device
+        n = X.shape[0]
+        raw = torch.empty(n, dtype=torch.int32, device=dev)
+        filt = torch.empty(n, dtype=torch.int32, device=dev) if known_mask is not None else None
+        fn = getattr(lib, self._REL_RANK)
+        for c0, c1 in self._relation_calls(X, known_mask, "known_mask",
+                                           lambda m: lib.rgcn_relation_rank_workspace_bytes(R, d, m)):
+            rc = fn(_ptr(self.codes), _ptr(self.rel), self.codes.shape[0], self.rel.shape[0], R, d, _ptr(X[c0:c1]),
+                    c1 - c0, _ptr(None if known_mask is None else known_mask[c0:c1]), int(self._rel_split_ready),
+                    _ptr(raw[c0:c1]), _ptr(None if filt is None else filt[c0:c1]), _ptr(self._rel_ws),
+                    self._rel_ws.numel(), _stream(dev))
+            _lib.check(rc, self._REL_RANK)
+        return raw, filt
+
+    def top_k_relations(self, X, k, exclude_mask=None):
+        """The k relations of rel[0:R] of highest energy for every pair (X[t, 0], ?, X[t, 2]) (the relation column
+        is not read), energy descending and the smaller id first on ties, never one whose bit is set in
+        exclude_mask (uint32 [n, ceil(R/32)] CUDA, as int32, or None).  Returns (ids int32 [n,k], energies float32
+        [n,k]) CUDA tensors; rows with fewer than k eligible relations end in (-1, -inf)."""
+        lib = _lib.load()
+        R, d, k = self.relation_count, self.codes.shape[1], int(k)
+        dev = self.codes.device
+        n = X.shape[0]
+        ids = torch.empty((n, k), dtype=torch.int32, device=dev)
+        energies = torch.empty((n, k), dtype=torch.float32, device=dev)
+        fn = getattr(lib, self._REL_TOPK)
+        for c0, c1 in self._relation_calls(X, exclude_mask, "exclude_mask",
+                                           lambda m: lib.rgcn_relation_topk_workspace_bytes(R, d, m, k)):
+            rc = fn(_ptr(self.codes), _ptr(self.rel), self.codes.shape[0], self.rel.shape[0], R, d, _ptr(X[c0:c1]),
+                    c1 - c0, k, _ptr(None if exclude_mask is None else exclude_mask[c0:c1]),
+                    int(self._rel_split_ready), _ptr(ids[c0:c1]), _ptr(energies[c0:c1]), _ptr(self._rel_ws),
+                    self._rel_ws.numel(), _stream(dev))
+            _lib.check(rc, self._REL_TOPK)
+        return ids, energies
+
 
 class ComplexRanker(DistMultRanker):
     """Fused all-entity scoring + ranking of the ComplEx decoder (rgcn_complex_rank): same interface and split reuse
     as DistMultRanker, the query rows are the complex products of complex.py:77-106."""
     _RANK, _WORKSPACE, _TOPK = "rgcn_complex_rank", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_topk"
+    _REL_RANK, _REL_TOPK = "rgcn_complex_relation_rank", "rgcn_complex_relation_topk"

@@ -1,4 +1,4 @@
-"""Top-k entity prediction from a trained checkpoint:
+"""Top-k entity and relation prediction from a trained checkpoint:
 
   python -m relationprediction_b200.predict --settings X.exp --dataset DIR | --dataset-npz F --checkpoint PATH
                                             --queries FILE --k K [--raw] --out FILE
@@ -8,15 +8,17 @@ every query of FILE, one per line:
 
   head<TAB>relation<TAB>?      the K most likely tails
   ?<TAB>relation<TAB>tail      the K most likely heads
+  head<TAB>?<TAB>tail          the K most likely relations linking head to tail
 
 Names come from the dataset's entities.dict / relations.dict; with --dataset-npz they are numeric ids.  By default
-the answers leave out every entity that completes a triple of the train, valid or test split (the filtered setting
-of the evaluation); --raw keeps them.  The output has one line per answer:
+the answers leave out every entity (or relation) that completes a triple of the train, valid or test split (the
+filtered setting of the evaluation); --raw keeps them.  The output has one line per answer:
 
-  query_index<TAB>position<TAB>entity<TAB>score
+  query_index<TAB>position<TAB>answer<TAB>score
 
 query_index counts the queries from 0 in file order, position counts from 1, and score is the model's sigmoid
-score.  A query with fewer than K eligible entities gets fewer lines."""
+score.  The answer is an entity name, or a relation name for a relation query.  A query with fewer than K eligible
+answers gets fewer lines."""
 import argparse
 
 import numpy as np
@@ -30,9 +32,9 @@ class QueryError(ValueError):
 
 
 def parse_queries(lines, entity_ids, relation_ids):
-    """[(s, r, o, side)] with the unknown end as -1 and side 0 = predict the head, 1 = predict the tail.
-    entity_ids / relation_ids map names to ids.  Blank lines are skipped; anything else malformed raises
-    QueryError naming the line."""
+    """[(s, r, o, side)] with the unknown field as -1 and side 0 = predict the head, 1 = predict the tail,
+    2 = predict the relation.  entity_ids / relation_ids map names to ids.  Blank lines are skipped; anything else
+    malformed raises QueryError naming the line."""
     out = []
     for no, line in enumerate(lines, 1):
         line = line.rstrip("\r\n")
@@ -40,10 +42,16 @@ def parse_queries(lines, entity_ids, relation_ids):
             continue
         f = [x.strip() for x in line.split("\t")]
         if len(f) != 3:
-            raise QueryError("line %d: expected head<TAB>relation<TAB>? or ?<TAB>relation<TAB>tail, got %r"
-                             % (no, line))
-        if (f[0] == "?") == (f[2] == "?"):
-            raise QueryError("line %d: exactly one of head and tail must be '?', got %r" % (no, line))
+            raise QueryError("line %d: expected head<TAB>relation<TAB>?, ?<TAB>relation<TAB>tail or "
+                             "head<TAB>?<TAB>tail, got %r" % (no, line))
+        if f.count("?") != 1:
+            raise QueryError("line %d: exactly one of head, relation and tail must be '?', got %r" % (no, line))
+        if f[1] == "?":
+            for name in (f[0], f[2]):
+                if name not in entity_ids:
+                    raise QueryError("line %d: unknown entity %r" % (no, name))
+            out.append((entity_ids[f[0]], -1, entity_ids[f[2]], 2))
+            continue
         if f[1] not in relation_ids:
             raise QueryError("line %d: unknown relation %r" % (no, f[1]))
         side = 0 if f[0] == "?" else 1
@@ -56,17 +64,23 @@ def parse_queries(lines, entity_ids, relation_ids):
 
 
 def answer(scorer, queries, k, filtered):
-    """[(query_index, position, entity id, score)] for the parsed queries, through Scorer.predict_top_k: one call
-    per side.  The unknown end is given the known entity's id (the fused path does not read it)."""
+    """[(query_index, position, answer id, score)] for the parsed queries: entity queries through
+    Scorer.predict_top_k, one call per side, and relation queries (side 2, answer = a relation id) through
+    Scorer.predict_top_k_relations, one call.  The unknown field is given an id in range (the fused paths do not
+    read it): the known entity's for an entity query, 0 for a relation query."""
     rows = []
-    for side in (0, 1):
+    for side in (0, 1, 2):
         idx = [i for i, q in enumerate(queries) if q[3] == side]
         if not idx:
             continue
         tri = np.array([queries[i][:3] for i in idx], dtype=np.int64)
-        unknown = 0 if side == 0 else 2
-        tri[:, unknown] = tri[:, 2 - unknown]
-        ids, _, scores = scorer.predict_top_k(tri, k, side, filtered=filtered)
+        if side == 2:
+            tri[:, 1] = 0
+            ids, _, scores = scorer.predict_top_k_relations(tri, k, filtered=filtered)
+        else:
+            unknown = 0 if side == 0 else 2
+            tri[:, unknown] = tri[:, 2 - unknown]
+            ids, _, scores = scorer.predict_top_k(tri, k, side, filtered=filtered)
         for j, qi in enumerate(idx):
             for p in range(ids.shape[1]):
                 if ids[j, p] < 0:
@@ -78,17 +92,19 @@ def answer(scorer, queries, k, filtered):
 
 def main(argv=None):
     ap = argparse.ArgumentParser(description="Predict the K most likely entities for (head, relation, ?) and "
-                                             "(?, relation, tail) queries with a trained model.")
+                                             "(?, relation, tail) queries, and the K most likely relations for "
+                                             "(head, ?, tail) queries, with a trained model.")
     ap.add_argument("--settings", required=True)
     ap.add_argument("--dataset", default=None, help="directory with train/valid/test.txt + the two .dict files")
     ap.add_argument("--dataset-npz", default=None, help="the same data packed by scripts/pack_dataset.py "
                                                         "(queries then name entities and relations by id)")
     ap.add_argument("--checkpoint", required=True, help="a file written by Model.save (PREFIX-N.pt)")
-    ap.add_argument("--queries", required=True, help="one query per line: head<TAB>relation<TAB>? or "
-                                                     "?<TAB>relation<TAB>tail")
+    ap.add_argument("--queries", required=True, help="one query per line: head<TAB>relation<TAB>?, "
+                                                     "?<TAB>relation<TAB>tail or head<TAB>?<TAB>tail")
     ap.add_argument("--k", type=int, required=True, help="answers per query, 1 <= K <= 128")
-    ap.add_argument("--raw", action="store_true", help="keep entities that complete a known triple")
-    ap.add_argument("--out", required=True, help="output file: query_index<TAB>position<TAB>entity<TAB>score")
+    ap.add_argument("--raw", action="store_true", help="keep entities (relations) that complete a known triple")
+    ap.add_argument("--out", required=True, help="output file: query_index<TAB>position<TAB>answer<TAB>score, the "
+                                                "answer an entity, or a relation for head<TAB>?<TAB>tail")
     ap.add_argument("--device", default="cuda:0")
     args = ap.parse_args(argv)
     if (args.dataset is None) == (args.dataset_npz is None):
@@ -101,12 +117,12 @@ def main(argv=None):
         splits, entities, relations = driver.load_dataset_npz(args.dataset_npz)
         ent_names = {str(i): i for i in entities}
         rel_names = {str(i): i for i in relations}
-        name_of = str
+        name_of = rel_name_of = str
     else:
         splits, entities, relations = driver.load_dataset(args.dataset)
         ent_names = {v: i for i, v in entities.items()}
         rel_names = {v: i for i, v in relations.items()}
-        name_of = entities.__getitem__
+        name_of, rel_name_of = entities.__getitem__, relations.__getitem__
     with open(args.queries) as fh:
         try:
             queries = parse_queries(fh, ent_names, rel_names)
@@ -117,8 +133,9 @@ def main(argv=None):
     model.load(args.checkpoint)
     rows = answer(scorer, queries, args.k, filtered=not args.raw)
     with open(args.out, "w") as fh:
-        for qi, pos, ent, score in rows:
-            fh.write("%d\t%d\t%s\t%.9g\n" % (qi, pos, name_of(ent), score))
+        for qi, pos, ans, score in rows:
+            name = rel_name_of(ans) if queries[qi][3] == 2 else name_of(ans)
+            fh.write("%d\t%d\t%s\t%.9g\n" % (qi, pos, name, score))
     return rows
 
 

@@ -231,6 +231,10 @@ def main(argv=None):
                     help="keep the validation passes but never stop on them (only --max-iterations / --time-budget)")
     ap.add_argument("--final-eval", type=int, default=None, metavar="N",
                     help="after training rank the first N test triples (0 = all) and print one JSON line")
+    ap.add_argument("--relation-metrics", action="store_true",
+                    help="also rank every test triple's relation among all relations for its (head, tail) pair and "
+                         "report Raw / Filtered MRR and H@1/3/10 for relation prediction after the entity metrics "
+                         "(DistMult and ComplEx decoders on CUDA)")
     ap.add_argument("--set", action="append", default=[], metavar="Section.Key=Value",
                     help="override one settings entry after the file is read, e.g. "
                          "--set Encoder.NumberOfBasisFunctions=2 (repeatable)")
@@ -410,6 +414,9 @@ def main(argv=None):
             score = scorer.compute_scores(valid).get_summary().results['Filtered']['MRR']
             print("Validation filtered MRR at iteration %d: %f" % (it, score))
             scorer.compute_scores(test).get_summary().pretty_print()
+            if args.relation_metrics:
+                print("Relation prediction:")
+                scorer.compute_relation_mrr_scores(test).get_summary().pretty_print()
             if stopper.update(it, score) and not args.no_early_stopping:
                 break
         if save_every is not None and it % save_every == 0:
@@ -422,12 +429,17 @@ def main(argv=None):
         t0 = time.time()
         res = scorer.compute_scores(part).get_summary().results
         keep = ('MRR', 'H@1', 'H@3', 'H@10')
-        print(json.dumps({"iterations": it, "train_seconds": round(train_seconds, 2),
-                          "ms_per_iteration": round(train_seconds / max(it, 1) * 1e3, 3),
-                          "last_avg_train_loss": last_avg, "test_triples": int(len(part)),
-                          "eval_seconds": round(time.time() - t0, 2),
-                          "raw": {k: float(v) for k, v in res['Raw'].items() if k in keep},
-                          "filtered": {k: float(v) for k, v in res['Filtered'].items() if k in keep}}))
+        line = {"iterations": it, "train_seconds": round(train_seconds, 2),
+                "ms_per_iteration": round(train_seconds / max(it, 1) * 1e3, 3),
+                "last_avg_train_loss": last_avg, "test_triples": int(len(part)),
+                "eval_seconds": round(time.time() - t0, 2),
+                "raw": {k: float(v) for k, v in res['Raw'].items() if k in keep},
+                "filtered": {k: float(v) for k, v in res['Filtered'].items() if k in keep}}
+        if args.relation_metrics:
+            rel = scorer.compute_relation_mrr_scores(part).get_summary().results
+            line["relation"] = {"raw": {k: float(v) for k, v in rel['Raw'].items() if k in keep},
+                                "filtered": {k: float(v) for k, v in rel['Filtered'].items() if k in keep}}
+        print(json.dumps(line))
     return model, scorer
 
 
