@@ -523,6 +523,33 @@ int rgcn_complex_rank(const float* codes, const float* rel, int32_t V, int32_t V
                       int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Ensemble ranking, fused (R-GCN+): the weighted sum of two models' scores (the reference's tools/ensemble.py
+ * --method weighted_sum over Scorer.dump_all_scores files), without either [n, V] score matrix.  A member is a
+ * DistMult or ComplEx decoder (decoder_x = RGCN_DECODER_*) over its own codes [V, d_x] and relation table
+ * [Vrel_x, d_x]; both members share the V entities, their widths may differ.  For every triple t of X:
+ *   s_X(t, v) = the float32 sigmoid score of member X's rank entry point (distmult_rank / rgcn_complex_rank)
+ *   c(t, v)   = w s_A(t, v) + (1 - w) s_B(t, v)       in float64, separately rounded products and sum,
+ *               1 - w formed once in double (the reference tool's Python arithmetic, bit for bit)
+ *   G(t)      = w g_A(t) + (1 - w) g_B(t), g_X the member's gold score
+ *   raw_rank[t]      = #{ v : c(t, v) >= G(t) }   (the gold entity counts itself)
+ *   filtered_rank[t] = raw_rank[t] - #{ v in known(t) : c(t, v) >= G(t) } + 1
+ * known_mask, side, X and the outputs as in distmult_rank.  weight = w must be finite and in [0, 1].
+ * workspace  : rgcn_ensemble_rank_workspace_bytes(V, d_a, d_b, n); its head holds the hi/lo splits of codes_a and
+ *              codes_b: reuse_split != 0 skips both when the same workspace is passed again with unchanged codes.
+ * Errors, before any device work: RGCN_ERR_INVALID (unknown decoder kind, d_x % 4 != 0, bad weight, null pointers,
+ * side, filtered ranks without a known mask), RGCN_ERR_WORKSPACE.  The *_workspace_bytes function returns
+ * RGCN_ERR_INVALID (-1) on bad arguments.
+ * ---------------------------------------------------------------------------------------------- */
+#define RGCN_DECODER_DISTMULT 0
+#define RGCN_DECODER_COMPLEX 1
+int64_t rgcn_ensemble_rank_workspace_bytes(int32_t V, int32_t d_a, int32_t d_b, int64_t n);
+int rgcn_ensemble_rank(int32_t decoder_a, const float* codes_a, const float* rel_a, int32_t Vrel_a, int32_t d_a,
+                       int32_t decoder_b, const float* codes_b, const float* rel_b, int32_t Vrel_b, int32_t d_b,
+                       int32_t V, double weight, const int32_t* X, int64_t n, int side, const uint32_t* known_mask,
+                       int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
+                       int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Top-k entity prediction, fused: the k entities each query believes in most, without the [n, V] score matrix
  * that predict_all_subject_scores / predict_all_object_scores (bilinear_diag.py:51-61, complex.py:77-106)
  * materialise and Scorer.dump_all_scores (common/evaluation.py:391-408) writes out.  For every triple t of X:

@@ -5,7 +5,7 @@ loudly.  (The oracle under /oracle is test infrastructure and is never imported 
 """
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "librgcn_b200.so")
@@ -31,7 +31,10 @@ EXPORTED_SYMBOLS = [
     "rgcn_topk_workspace_bytes", "distmult_topk", "rgcn_complex_topk",
     "rgcn_relation_rank_workspace_bytes", "distmult_relation_rank", "rgcn_complex_relation_rank",
     "rgcn_relation_topk_workspace_bytes", "distmult_relation_topk", "rgcn_complex_relation_topk",
+    "rgcn_ensemble_rank_workspace_bytes", "rgcn_ensemble_rank",
 ]
+
+RGCN_DECODER_DISTMULT, RGCN_DECODER_COMPLEX = 0, 1
 
 RGCN_NORM_CANONICAL, RGCN_NORM_EXPLICIT, RGCN_NORM_NONE = 0, 1, 2
 
@@ -208,6 +211,11 @@ def _declare(lib):
         getattr(lib, name).restype = c_int
         getattr(lib, name).argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, vp, c_int64, c_int32, vp, c_int,
                                        vp, vp, vp, c_int64, vp]
+    lib.rgcn_ensemble_rank_workspace_bytes.restype = c_int64
+    lib.rgcn_ensemble_rank_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int64]
+    lib.rgcn_ensemble_rank.restype = c_int
+    lib.rgcn_ensemble_rank.argtypes = [c_int32, vp, vp, c_int32, c_int32, c_int32, vp, vp, c_int32, c_int32, c_int32,
+                                       c_double, vp, c_int64, c_int, vp, c_int, vp, vp, vp, c_int64, vp]
 
 
 def load():

@@ -1570,6 +1570,96 @@ extern "C" int rgcn_complex_rank(const float* codes, const float* rel, int32_t V
 }
 
 // ------------------------------------------------------------------------------------------------
+// Ensemble ranking (R-GCN+), fused: two members' scores combined by a weighted sum in float64
+// ------------------------------------------------------------------------------------------------
+// Workspace layout: [hi_A V*d_A | lo_A V*d_A | hi_B V*d_B | lo_B V*d_B | Q_A n*d_A | Q_A lo n*d_A | Q_B n*d_B |
+// Q_B lo n*d_B | gold_sig_A n | gold_sig_B n | gold_col n | raw_cnt n | known_cnt n].  Q_X holds the member's query
+// rows (its rank prepare kernel) and then, split in place, their TF32 hi part.
+static RankPrepareFn ensemble_prepare(int32_t decoder) {
+  if (decoder == RGCN_DECODER_DISTMULT) return launch_distmult_rank_prepare;
+  if (decoder == RGCN_DECODER_COMPLEX) return launch_complex_rank_prepare;
+  return nullptr;
+}
+
+extern "C" int64_t rgcn_ensemble_rank_workspace_bytes(int32_t V, int32_t d_a, int32_t d_b, int64_t n) {
+  if (V <= 0 || d_a <= 0 || d_a % 4 != 0 || d_b <= 0 || d_b % 4 != 0 || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_ensemble_rank_workspace_bytes: bad arguments (need V > 0, d > 0, d % 4 == 0, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  return 2 * align_up((int64_t)V * d_a * 4) + 2 * align_up((int64_t)V * d_b * 4) + 2 * align_up(n * d_a * 4) +
+         2 * align_up(n * d_b * 4) + 5 * align_up(n * 4) + 256;
+}
+
+extern "C" int rgcn_ensemble_rank(int32_t decoder_a, const float* codes_a, const float* rel_a, int32_t Vrel_a,
+                                  int32_t d_a, int32_t decoder_b, const float* codes_b, const float* rel_b,
+                                  int32_t Vrel_b, int32_t d_b, int32_t V, double weight, const int32_t* X, int64_t n,
+                                  int side, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
+                                  int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream) {
+  const RankPrepareFn prep_a = ensemble_prepare(decoder_a), prep_b = ensemble_prepare(decoder_b);
+  if (!prep_a || !prep_b) {
+    rgcn_set_error("rgcn_ensemble_rank: unknown decoder kind (RGCN_DECODER_DISTMULT or RGCN_DECODER_COMPLEX)");
+    return RGCN_ERR_INVALID;
+  }
+  if (d_a <= 0 || d_a % 4 != 0 || d_b <= 0 || d_b % 4 != 0) {
+    rgcn_set_error("rgcn_ensemble_rank: bad arguments (need d % 4 == 0 for both members)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!(weight >= 0.0 && weight <= 1.0)) {   // also refuses NaN
+    rgcn_set_error("rgcn_ensemble_rank: bad arguments (the weight must be finite and in [0, 1])");
+    return RGCN_ERR_INVALID;
+  }
+  if (!codes_a || !rel_a || !codes_b || !rel_b || (n > 0 && (!X || !raw_rank)) || !workspace || V <= 0 ||
+      Vrel_a <= 0 || Vrel_b <= 0 || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_ensemble_rank: bad arguments (null pointer or bad size)");
+    return RGCN_ERR_INVALID;
+  }
+  if (side != 0 && side != 1) {
+    rgcn_set_error("rgcn_ensemble_rank: bad arguments (side in {0,1})");
+    return RGCN_ERR_INVALID;
+  }
+  if (filtered_rank && !known_mask) {
+    rgcn_set_error("rgcn_ensemble_rank: bad arguments (filtered ranks need a known mask)");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_ensemble_rank_workspace_bytes(V, d_a, d_b, n)) {
+    rgcn_set_error("rgcn_ensemble_rank: workspace too small (rgcn_ensemble_rank_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver ws(workspace, workspace_bytes);
+  float* hi_a = ws.take<float>((int64_t)V * d_a);
+  float* lo_a = ws.take<float>((int64_t)V * d_a);
+  float* hi_b = ws.take<float>((int64_t)V * d_b);
+  float* lo_b = ws.take<float>((int64_t)V * d_b);
+  float* q_a = ws.take<float>(n * d_a);
+  float* ql_a = ws.take<float>(n * d_a);
+  float* q_b = ws.take<float>(n * d_b);
+  float* ql_b = ws.take<float>(n * d_b);
+  float* gs_a = ws.take<float>(n);
+  float* gs_b = ws.take<float>(n);
+  int32_t* gold_col = ws.take<int32_t>(n);
+  int32_t* raw_cnt = ws.take<int32_t>(n);
+  int32_t* known_cnt = ws.take<int32_t>(n);
+  int rc = RGCN_OK;
+  if (!reuse_split) {
+    rc = launch_gemm_split_b(codes_a, d_a, V, d_a, /*transposed=*/0, hi_a, lo_a, st);
+    if (!rc) rc = launch_gemm_split_b(codes_b, d_b, V, d_b, /*transposed=*/0, hi_b, lo_b, st);
+  }
+  if (rc || n == 0) return rc;
+  rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
+  if (!rc) rc = prep_a(codes_a, rel_a, d_a, X, n, side, q_a, gs_a, gold_col, st);
+  if (!rc) rc = prep_b(codes_b, rel_b, d_b, X, n, side, q_b, gs_b, gold_col, st);   // the same gold column
+  if (!rc) rc = launch_split_trunc(q_a, ql_a, n * d_a, st);
+  if (!rc) rc = launch_split_trunc(q_b, ql_b, n * d_b, st);
+  if (rc) return rc;
+  rc = launch_gemm_ensemble_rank_tf32x3(q_a, ql_a, hi_a, lo_a, gs_a, d_a, q_b, ql_b, hi_b, lo_b, gs_b, d_b, (int)n, V,
+                                        weight, 1.0 - weight, gold_col, known_mask, (V + 31) / 32, raw_cnt, known_cnt,
+                                        st);
+  if (rc) return rc;
+  return launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
+}
+
+// ------------------------------------------------------------------------------------------------
 // Top-k prediction over all entities, fused (DistMult and ComplEx)
 // ------------------------------------------------------------------------------------------------
 // The decoder-independent body of distmult_topk / rgcn_complex_topk: the hi/lo split of `codes` (unless reused),

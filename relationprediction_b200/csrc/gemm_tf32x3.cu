@@ -765,6 +765,251 @@ __global__ void k_split_b_interleave(const float* __restrict__ Wmu, const float*
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// ENSEMBLE RANKING (R-GCN+: the weighted sum of two models' scores, tools/ensemble.py `weighted_sum`): every tile
+// runs the K blocks of member A (Q_A [M, K_A] against codes_A [N, K_A]) and then those of member B into separate
+// accumulators; the epilogue forms each member's float32 sigmoid score as RankEpi does, combines them in float64,
+//   c = w s_A + (1 - w) s_B   (separately rounded multiplies and add: the reference tool's Python arithmetic),
+// and counts c >= G into raw_cnt / known_cnt by RankEpi's rules, G = w g_A + (1 - w) g_B.  [M, N] is never written.
+//
+// Tile 128 x 64 (wgmma.m64n64k8): two members x (hi*hi, cross terms) x 64 x 64 / 128 threads = 128 accumulator
+// registers per consumer thread, the count of the 128 x 128 single-model kernel.  Both operands come pre-split
+// (the codes by round-to-nearest as for k_gemm_tf32x3, the query rows by the same truncation its producer applies),
+// so the producer only issues asynchronous copies, EN_LOOKAHEAD blocks ahead.  A stage is Q hi/lo (2 x 16 KB) and
+// code hi/lo (2 x 8 KB); four stages fit.  Each output element sees the K steps of its member in the order of the
+// single-model kernel, so w = 1 (w = 0) reproduces member A's (B's) fused ranks.
+// ------------------------------------------------------------------------------------------------
+constexpr int EN_BN = 64;
+constexpr int EN_STAGES = 4;
+constexpr int EN_LOOKAHEAD = 2;                                    // blocks in flight ahead of the one published
+constexpr int EN_Q_BYTES = BM * BK * 4;                            // 16 KB (Q_hi, Q_lo)
+constexpr int EN_C_BYTES = EN_BN * BK * 4;                         // 8 KB (code_hi, code_lo)
+constexpr int EN_STAGE_BYTES = 2 * EN_Q_BYTES + 2 * EN_C_BYTES;    // 48 KB
+constexpr int EN_SMEM_BYTES = EN_STAGES * EN_STAGE_BYTES + 1024;
+constexpr int EN_FRAG = EN_BN / 2;                                 // accumulator registers per thread and array
+static_assert(EN_SMEM_BYTES <= 227 * 1024, "ensemble kernel exceeds the shared memory of a block");
+static_assert(EN_LOOKAHEAD < EN_STAGES, "the lookahead needs a free stage");
+
+struct EnsMember {
+  const float* q_hi;           // [M, K] query rows, split by truncation
+  const float* q_lo;
+  const float* c_hi;           // [N, K] entity codes, split by round-to-nearest
+  const float* c_lo;
+  const float* gold_sig;       // [M] sigmoid(energy of the gold entity)
+  int K;                       // K % 4 == 0; the leading dimension of all four planes
+};
+struct EnsEpi {
+  EnsMember a, b;
+  double w, omw;               // weight of A and 1 - w (formed once on the host, in double)
+  const int32_t* gold_col;     // [M]
+  const uint32_t* known;       // [M, words] or nullptr
+  int words;
+  int32_t* raw_cnt;            // [M] += #{v : c_v >= G}
+  int32_t* known_cnt;          // [M] += #{known v : c_v >= G}
+};
+
+// d[64 rows of this warpgroup x 64] (+)= A(desc) * B(desc)^T, TF32 inputs, fp32 accumulators
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[EN_FRAG], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+      "%23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
+}
+__device__ __forceinline__ void fence_acc64(float (&d)[EN_FRAG]) {
+#pragma unroll
+  for (int i = 0; i < EN_FRAG; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// consume_tile for the 128 x 64 stages of the ensemble kernel: k-blocks g0 .. g0 + num_kb - 1 of the CTA's stage
+// sequence into (big, small), the MMAs of a K step in the order of consume_tile
+__device__ __forceinline__ void ens_consume(uint32_t smem_base, uint64_t* full_bar, uint64_t* empty_bar, int g0,
+                                            int num_kb, uint32_t a_rows, float (&big)[EN_FRAG],
+                                            float (&small)[EN_FRAG]) {
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int g = g0 + kb;
+    const int s = g % EN_STAGES;
+    mbar_wait(&full_bar[s], (uint32_t)(g / EN_STAGES) & 1u);
+    const uint32_t a_hi = smem_base + s * EN_STAGE_BYTES + a_rows, a_lo = a_hi + EN_Q_BYTES;
+    const uint32_t b_hi = smem_base + s * EN_STAGE_BYTES + 2 * EN_Q_BYTES, b_lo = b_hi + EN_C_BYTES;
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+    for (int kk = 0; kk < BK / 8; ++kk) {
+      const uint64_t dah = make_desc(a_hi + kk * 32), dal = make_desc(a_lo + kk * 32);
+      const uint64_t dbh = make_desc(b_hi + kk * 32), dbl = make_desc(b_lo + kk * 32);
+      const uint32_t acc = (kb == 0 && kk == 0) ? 0u : 1u;
+      wgmma_tf32_n64(small, dal, dbh, acc);
+      wgmma_tf32_n64(small, dah, dbl, 1u);
+      wgmma_tf32_n64(big, dah, dbh, acc);
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    fence_acc64(big);
+    fence_acc64(small);
+    mbar_arrive(&empty_bar[s]);
+  }
+}
+
+// Persistent like k_gemm_tf32x3 (N tiles fastest); a tile is num_kb_a + num_kb_b consecutive k-blocks of the CTA's
+// stage sequence.
+__global__ void __launch_bounds__(N_THREADS, 1)
+    k_gemm_ensemble_rank(int M, int N, int n_tiles, EnsEpi re) {
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t full_bar[EN_STAGES], empty_bar[EN_STAGES];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int tn = (N + EN_BN - 1) / EN_BN;
+  const int nkb_a = (re.a.K + BK - 1) / BK, nkb_b = (re.b.K + BK - 1) / BK, nkb = nkb_a + nkb_b;
+  const int n_mine = (n_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int total_g = n_mine * nkb;
+
+  if (tid == 0) init_barriers<EN_STAGES>(full_bar, empty_bar);
+  __syncthreads();
+
+  if (tid < N_PRODUCERS) {
+    // ================= producer warpgroup: asynchronous copies only =================
+    const int c = tid & 7;                     // 16 B chunk within the 128 B K-row
+    const int rbase = tid >> 3;                // tile rows rbase + 16 i
+    const uint32_t soff = swz(rbase, c);
+    int i_tile = (int)blockIdx.x, i_kb = 0, stage = 0;
+    auto issue = [&]() {                       // copies the next block of the sequence into `stage`
+      const bool mb = i_kb >= nkb_a;
+      const float* qh = mb ? re.b.q_hi : re.a.q_hi;
+      const float* ql = mb ? re.b.q_lo : re.a.q_lo;
+      const float* ch = mb ? re.b.c_hi : re.a.c_hi;
+      const float* cl = mb ? re.b.c_lo : re.a.c_lo;
+      const int K = mb ? re.b.K : re.a.K;
+      const int k = (mb ? i_kb - nkb_a : i_kb) * BK + c * 4;
+      const bool col_ok = k < K;               // K % 4 == 0: a 16 B chunk is entirely valid or entirely padding
+      const int m0 = (i_tile / tn) * BM, n0 = (i_tile % tn) * EN_BN;
+      const uint32_t st = smem_base + stage * EN_STAGE_BYTES + soff;
+#pragma unroll
+      for (int i = 0; i < BM / 16; ++i) {
+        const int row = m0 + rbase + 16 * i;
+        const bool ok = col_ok && row < M;
+        const size_t o = ok ? (size_t)row * K + k : 0;
+        cp_async16(st + 2048 * i, qh + o, ok ? 16u : 0u);
+        cp_async16(st + EN_Q_BYTES + 2048 * i, ql + o, ok ? 16u : 0u);
+      }
+#pragma unroll
+      for (int i = 0; i < EN_BN / 16; ++i) {
+        const int row = n0 + rbase + 16 * i;
+        const bool ok = col_ok && row < N;
+        const size_t o = ok ? (size_t)row * K + k : 0;
+        cp_async16(st + 2 * EN_Q_BYTES + 2048 * i, ch + o, ok ? 16u : 0u);
+        cp_async16(st + 2 * EN_Q_BYTES + EN_C_BYTES + 2048 * i, cl + o, ok ? 16u : 0u);
+      }
+      asm volatile("cp.async.commit_group;" ::: "memory");
+      stage = stage + 1 == EN_STAGES ? 0 : stage + 1;
+      if (++i_kb == nkb) {
+        i_kb = 0;
+        i_tile += (int)gridDim.x;
+      }
+    };
+    // block g goes to stage g % EN_STAGES in use round g / EN_STAGES; the copies of blocks g + 1 .. g + EN_LOOKAHEAD
+    // are in flight while block g is published.  One commit group per block (empty past the end) keeps the count.
+    for (int g = 0; g < EN_LOOKAHEAD; ++g) {
+      if (g < total_g) {
+        mbar_wait(&empty_bar[g % EN_STAGES], ((uint32_t)(g / EN_STAGES) & 1u) ^ 1u);
+        issue();
+      } else {
+        asm volatile("cp.async.commit_group;" ::: "memory");
+      }
+    }
+    for (int g = 0; g < total_g; ++g) {
+      const int gn = g + EN_LOOKAHEAD;
+      if (gn < total_g) {
+        mbar_wait(&empty_bar[gn % EN_STAGES], ((uint32_t)(gn / EN_STAGES) & 1u) ^ 1u);
+        issue();
+      } else {
+        asm volatile("cp.async.commit_group;" ::: "memory");
+      }
+      asm volatile("cp.async.wait_group %0;" ::"n"(EN_LOOKAHEAD) : "memory");   // block g has landed
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");             // generic-proxy writes -> tensor core
+      mbar_arrive(&full_bar[g % EN_STAGES]);
+    }
+  } else {
+    // ================= consumer warpgroups =================
+    // accumulator fragment of wgmma m64n64: register 4j + 2h + e holds row 16 * (warp % 4) + lane / 4 + 8 h and
+    // column 8 j + 2 (lane % 4) + e of the warpgroup's 64 x 64 block
+    const int ctid = tid - N_PRODUCERS;
+    const int wg = ctid >> 7;
+    const uint32_t a_rows = (uint32_t)(wg * 64 * 128);
+    float big_a[EN_FRAG], small_a[EN_FRAG], big_b[EN_FRAG], small_b[EN_FRAG];
+    for (int ti = 0; ti < n_mine; ++ti) {
+      const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+      const int m0 = (tile / tn) * BM, n0 = (tile % tn) * EN_BN;
+      ens_consume(smem_base, full_bar, empty_bar, ti * nkb, nkb_a, a_rows, big_a, small_a);
+      ens_consume(smem_base, full_bar, empty_bar, ti * nkb + nkb_a, nkb_b, a_rows, big_b, small_b);
+      const int r0 = m0 + wg * 64 + ((ctid >> 5) & 3) * 16 + (lane >> 2);
+      const int c0 = n0 + 2 * (lane & 3);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = r0 + 8 * h;
+        int raw = 0, kn = 0;
+        if (row < M) {
+          const double G = __dadd_rn(__dmul_rn(re.w, (double)__ldg(re.a.gold_sig + row)),
+                                     __dmul_rn(re.omw, (double)__ldg(re.b.gold_sig + row)));
+          const int gold_c = __ldg(re.gold_col + row);
+#pragma unroll
+          for (int cb = 0; cb < EN_BN / 32; ++cb) {
+            const int chunk = n0 + 32 * cb;
+            const uint32_t kw =
+                (re.known && chunk < N) ? __ldg(re.known + (size_t)row * re.words + (chunk >> 5)) : 0u;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * cb + jj;
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int col = c0 + 8 * j + e, r = 4 * j + 2 * h + e;
+                const float sa = sigmoid_ref(big_a[r] + small_a[r]);
+                const float sb = sigmoid_ref(big_b[r] + small_b[r]);
+                const double cv = __dadd_rn(__dmul_rn(re.w, (double)sa), __dmul_rn(re.omw, (double)sb));
+                if (col < N && (cv >= G || col == gold_c)) {   // the gold entity always counts
+                  ++raw;
+                  kn += (int)((kw >> (col & 31)) & 1u);
+                }
+              }
+            }
+          }
+        }
+        raw += __shfl_xor_sync(0xffffffffu, raw, 1);
+        raw += __shfl_xor_sync(0xffffffffu, raw, 2);
+        kn += __shfl_xor_sync(0xffffffffu, kn, 1);
+        kn += __shfl_xor_sync(0xffffffffu, kn, 2);
+        if ((lane & 3) == 0 && row < M) {
+          if (raw) atomicAdd(re.raw_cnt + row, raw);
+          if (kn) atomicAdd(re.known_cnt + row, kn);
+        }
+      }
+    }
+  }
+}
+
+// In-place truncation split of [count] floats (count % 4 == 0, 16 B aligned): a -> hi (kept in a) and lo, the split
+// the k_gemm_tf32x3 producer applies to its streamed operand
+__global__ void k_split_trunc(float* __restrict__ a, float* __restrict__ lo, int64_t count4) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < count4; i += (int64_t)gridDim.x * blockDim.x) {
+    float4 v = reinterpret_cast<float4*>(a)[i], h, l;
+    split_tf32_trunc(v.x, h.x, l.x);
+    split_tf32_trunc(v.y, h.y, l.y);
+    split_tf32_trunc(v.z, h.z, l.z);
+    split_tf32_trunc(v.w, h.w, l.w);
+    reinterpret_cast<float4*>(a)[i] = h;
+    reinterpret_cast<float4*>(lo)[i] = l;
+  }
+}
+
 }  // namespace
 
 // SM count of the current device
@@ -883,6 +1128,47 @@ int launch_gemm_topk_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
                                                          (int)tiles, TopKEpi{excl, words, k, tn, cand});
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<topk>");
+}
+
+int launch_split_trunc(float* a, float* lo, int64_t count, cudaStream_t st) {
+  if (count == 0) return RGCN_OK;
+  const int64_t count4 = count / 4;
+  int blocks = (int)std::min<int64_t>((count4 + 255) / 256, 132 * 8);
+  k_split_trunc<<<blocks, 256, 0, st>>>(a, lo, count4);
+  ++g_rgcn_launches;
+  return rgcn_check_cuda(cudaGetLastError(), "k_split_trunc");
+}
+
+// Two-member ranking GEMM (see k_gemm_ensemble_rank); the counts accumulate (+=) into raw_cnt / known_cnt.
+int launch_gemm_ensemble_rank_tf32x3(const float* qa_hi, const float* qa_lo, const float* ca_hi, const float* ca_lo,
+                                     const float* gold_sig_a, int Ka, const float* qb_hi, const float* qb_lo,
+                                     const float* cb_hi, const float* cb_lo, const float* gold_sig_b, int Kb, int M,
+                                     int N, double w, double omw, const int32_t* gold_col, const uint32_t* known,
+                                     int words, int32_t* raw_cnt, int32_t* known_cnt, cudaStream_t st) {
+  if (M == 0 || N == 0) return RGCN_OK;
+  if (Ka <= 0 || Ka % 4 != 0 || Kb <= 0 || Kb % 4 != 0) {
+    rgcn_set_error("gemm_ensemble_rank_tf32x3: K > 0 and K % 4 == 0 for both members");
+    return RGCN_ERR_INVALID;
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_ensemble_rank, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  EN_SMEM_BYTES),
+                             "cudaFuncSetAttribute(gemm ensemble smem)");
+    if (rc) return rc;
+    attr_set = true;
+  }
+  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((N + EN_BN - 1) / EN_BN);
+  if (tiles > 0x7fffffffLL) {
+    rgcn_set_error("gemm_ensemble_rank_tf32x3: too many tiles");
+    return RGCN_ERR_INVALID;
+  }
+  EnsEpi re{{qa_hi, qa_lo, ca_hi, ca_lo, gold_sig_a, Ka}, {qb_hi, qb_lo, cb_hi, cb_lo, gold_sig_b, Kb}, w, omw,
+            gold_col, known, words, raw_cnt, known_cnt};
+  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
+  k_gemm_ensemble_rank<<<grid, N_THREADS, EN_SMEM_BYTES, st>>>(M, N, (int)tiles, re);
+  ++g_rgcn_launches;
+  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_ensemble_rank");
 }
 
 // Highway gate GEMM with the blend epilogue (EPI = 2): z = c2 @ W + bias with W pre-split as Bt = W^T [d, d];

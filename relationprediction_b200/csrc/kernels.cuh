@@ -163,6 +163,18 @@ int launch_gemm_topk_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
 int launch_topk_merge(const uint2* cand, int64_t n, int per_row, int k, int32_t* ids, float* energies,
                       cudaStream_t st);
 
+// In-place truncation split of `count` floats (count % 4 == 0): a becomes the TF32 hi part, lo the remainder's --
+// the split the scoring GEMM's producer applies to the query rows
+int launch_split_trunc(float* a, float* lo, int64_t count, cudaStream_t st);
+// Ensemble ranking GEMM (R-GCN+): per member X the query rows q_X [M, K_X] (truncation split) against the entity
+// codes c_X [N, K_X] (round-to-nearest split); c = w s_A + (1 - w) s_B in float64 of the two float32 sigmoid scores,
+// G the same of the gold sigmoids; raw_cnt / known_cnt += the counts of c >= G (the gold column always counts).
+int launch_gemm_ensemble_rank_tf32x3(const float* qa_hi, const float* qa_lo, const float* ca_hi, const float* ca_lo,
+                                     const float* gold_sig_a, int Ka, const float* qb_hi, const float* qb_lo,
+                                     const float* cb_hi, const float* cb_lo, const float* gold_sig_b, int Kb, int M,
+                                     int N, double w, double omw, const int32_t* gold_col, const uint32_t* known,
+                                     int words, int32_t* raw_cnt, int32_t* known_cnt, cudaStream_t st);
+
 int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
                           int M, int N, int K, int accumulate, cudaStream_t st);
 

@@ -142,13 +142,18 @@ class BilinearDiag(Model):
             return np.zeros((0, k), np.int64), np.zeros((0, k), np.float32)
         return torch.cat(ids).cpu().numpy().astype(np.int64), torch.cat(energies).cpu().numpy()
 
+    def test_ranker(self):
+        """The decoder's fused ranker (ops.DistMultRanker / ops.ComplexRanker) over the test-mode codes of the fed
+        inputs: one encoder pass.  The ensemble ranker (ops.EnsembleRanker) combines two of these."""
+        subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='test')
+        assert subject_codes is object_codes, "fused ranking expects one shared entity code matrix"
+        return self._ranker(subject_codes.contiguous(), relation_codes.contiguous())
+
     # ---- relation queries (h, ?, t): library entries distmult_relation_rank / distmult_relation_topk ----
     def _relation_ranker(self):
         """The ranker over the test-mode codes, with R = RelationCount relation candidates (rows 0..R-1 of the
         relation table)."""
-        subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='test')
-        assert subject_codes is object_codes, "fused relation prediction expects one shared entity code matrix"
-        return self._ranker(subject_codes.contiguous(), relation_codes.contiguous())
+        return self.test_ranker()
 
     def rank_relations_all(self, triplets, known_relation_lists, chunk=4096):
         """Raw and filtered ranks of every triple's relation among the RelationCount relations for its (head, tail)

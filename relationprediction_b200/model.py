@@ -105,6 +105,15 @@ class Model(object):
         with torch.no_grad():
             return self.rank_all(triplets, known_subject_lists, known_object_lists)
 
+    def entity_ranker(self, triplets):
+        """The head decoder's fused ranker over the test codes (ops.DistMultRanker / ops.ComplexRanker), fed like
+        rank_all_entities: one encoder pass in test mode.  None for decoders without one or off CUDA."""
+        if not self.supports_fused_ranking() or not hasattr(self, 'test_ranker'):
+            return None
+        self._feed_test(getattr(self, 'test_graph', None), np.asarray(triplets).reshape(-1, 3)[:1])
+        with torch.no_grad():
+            return self.test_ranker()
+
     def predict_top_k(self, triplets, k, side, exclude_lists=None):
         """The k most likely entities for every triple under the decoder's fused top-k path (one encoder pass for
         the whole set), fed like rank_all_entities.  side 0 predicts subjects, 1 objects; the predicted column of

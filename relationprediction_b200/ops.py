@@ -810,6 +810,7 @@ class DistMultRanker(object):
     workspaces start with the split)."""
     _RANK, _WORKSPACE, _TOPK = "distmult_rank", "distmult_rank_workspace_bytes", "distmult_topk"
     _REL_RANK, _REL_TOPK = "distmult_relation_rank", "distmult_relation_topk"
+    DECODER = _lib.RGCN_DECODER_DISTMULT   # the decoder kind of the ensemble entry point (rgcn_ensemble_rank)
     # device bytes one top_k / top_k_relations / rank_relations call may use beyond the split of its table; more
     # queries than fit go in several calls
     TOPK_CHUNK_BYTES = 1 << 30
@@ -963,3 +964,53 @@ class ComplexRanker(DistMultRanker):
     as DistMultRanker, the query rows are the complex products of complex.py:77-106."""
     _RANK, _WORKSPACE, _TOPK = "rgcn_complex_rank", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_topk"
     _REL_RANK, _REL_TOPK = "rgcn_complex_relation_rank", "rgcn_complex_relation_topk"
+    DECODER = _lib.RGCN_DECODER_COMPLEX
+
+
+class EnsembleRanker(object):
+    """Fused ranking under the weighted sum of two members' scores (R-GCN+; rgcn_ensemble_rank): member A scored by
+    ranker_a with weight w, member B by ranker_b with 1 - w, combined in float64.  The members are DistMultRanker /
+    ComplexRanker objects over the same V entities; their code widths may differ.  The ensemble keeps its own
+    workspace, whose head holds both members' hi/lo splits, made once and reused by every later call."""
+
+    def __init__(self, ranker_a, ranker_b, weight):
+        for name, r in (("ranker_a", ranker_a), ("ranker_b", ranker_b)):
+            if not isinstance(r, DistMultRanker):
+                raise TypeError("%s must be a DistMultRanker or ComplexRanker, got %s" % (name, type(r).__name__))
+        if ranker_a.codes.shape[0] != ranker_b.codes.shape[0]:
+            raise ValueError("the members rank different entity sets (%d and %d entities)"
+                             % (ranker_a.codes.shape[0], ranker_b.codes.shape[0]))
+        if ranker_a.codes.device != ranker_b.codes.device:
+            raise ValueError("the members live on different devices (%s and %s)"
+                             % (ranker_a.codes.device, ranker_b.codes.device))
+        weight = float(weight)
+        if not 0.0 <= weight <= 1.0:   # also refuses NaN
+            raise ValueError("the weight must be in [0, 1], got %r" % weight)
+        self.a, self.b, self.weight = ranker_a, ranker_b, weight
+        self._ws, self._ws_n, self._split_ready = None, -1, False
+
+    def rank(self, X, side, known_mask=None):
+        """As DistMultRanker.rank, with c = w s_A + (1 - w) s_B in place of the single score.  X int32 [n,3] CUDA;
+        side 0 = subjects corrupted, 1 = objects; known_mask uint32 [n, ceil(V/32)] CUDA (as int32) or None.
+        Returns (raw_rank, filtered_rank or None) int32 CUDA tensors."""
+        lib = _lib.load()
+        a, b = self.a, self.b
+        V, d_a = a.codes.shape
+        d_b = b.codes.shape[1]
+        a._check_rows(X, known_mask, "known_mask")
+        n = X.shape[0]
+        dev = a.codes.device
+        if self._ws is None or n > self._ws_n:
+            nb = lib.rgcn_ensemble_rank_workspace_bytes(V, d_a, d_b, n)
+            if nb < 0:
+                _lib.check(int(nb), "rgcn_ensemble_rank_workspace_bytes")
+            self._ws, self._ws_n, self._split_ready = _workspace(nb, dev), n, False
+        raw = torch.empty(n, dtype=torch.int32, device=dev)
+        filt = torch.empty(n, dtype=torch.int32, device=dev) if known_mask is not None else None
+        rc = lib.rgcn_ensemble_rank(a.DECODER, _ptr(a.codes), _ptr(a.rel), a.rel.shape[0], d_a,
+                                    b.DECODER, _ptr(b.codes), _ptr(b.rel), b.rel.shape[0], d_b,
+                                    V, self.weight, _ptr(X), n, int(side), _ptr(known_mask), int(self._split_ready),
+                                    _ptr(raw), _ptr(filt), _ptr(self._ws), self._ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_ensemble_rank")
+        self._split_ready = True
+        return raw, filt
