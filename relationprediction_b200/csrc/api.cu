@@ -88,7 +88,32 @@ int slabs_for(int d) {
   return (d + nv * 128 - 1) / (nv * 128);
 }
 
-int common_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
+// ---- argument checks ------------------------------------------------------------------------------------------------
+// The block and basis entry points check the graph first.  The one-hot, per-channel and diagonal ones check shape,
+// pointers and workspace first (nothing there touches the device, so those errors read the same for a host-only
+// graph), then the graph.
+
+int shape_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
+  if (!g || d <= 0 || d % 4 != 0 || B <= 0) {
+    rgcn_set_error(std::string(who) + ": need a graph, d > 0, d % 4 == 0, B > 0");
+    return RGCN_ERR_INVALID;
+  }
+  return RGCN_OK;
+}
+
+// the views a code path walks must have been built (rgcn_set_option("graph_views", ...))
+int need_views(const rgcn_graph_t* g, bool csr, bool rel, const char* who) {
+  if ((csr && !g->has_csr) || (rel && !g->has_rel)) {
+    rgcn_set_error(std::string(who) + ": the graph was prepared without the " + (csr && !g->has_csr ? "CSR" : "weight-id-major") +
+                   " views this path needs (option graph_views)");
+    return RGCN_ERR_INVALID;
+  }
+  return RGCN_OK;
+}
+
+// A graph on a device with 2R weight ids and the views (csr, rel) the path walks.  The layer entry points (self_loop)
+// also need V_src >= V_dst: the self-loop term reads H rows [0, V_dst).
+int graph_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who, bool self_loop, bool csr, bool rel) {
   if (!g) {
     rgcn_set_error(std::string(who) + ": null graph");
     return RGCN_ERR_INVALID;
@@ -105,27 +130,99 @@ int common_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) 
     rgcn_set_error(std::string(who) + ": graph weight-id count must be 2R");
     return RGCN_ERR_INVALID;
   }
-  return RGCN_OK;
-}
-
-// the views a code path walks must have been built (rgcn_set_option("graph_views", ...))
-int need_views(const rgcn_graph_t* g, bool csr, bool rel, const char* who) {
-  if ((csr && !g->has_csr) || (rel && !g->has_rel)) {
-    rgcn_set_error(std::string(who) + ": the graph was prepared without the " + (csr && !g->has_csr ? "CSR" : "weight-id-major") +
-                   " views this path needs (option graph_views)");
-    return RGCN_ERR_INVALID;
-  }
-  return RGCN_OK;
-}
-
-int layer_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
-  int rc = common_checks(g, d, B, who);
-  if (rc) return rc;
-  if (g->V_src < g->V_dst) {  // the self-loop term reads H rows [0, V_dst)
+  if (self_loop && g->V_src < g->V_dst) {
     rgcn_set_error(std::string(who) + ": layer entry points need V_src >= V_dst (messages-only graphs go through rgcn_block_aggregate)");
     return RGCN_ERR_INVALID;
   }
+  return need_views(g, csr, rel, who);
+}
+
+int block_size_checks(int32_t d, int32_t B, const char* who) {
+  if (d % B != 0) {
+    rgcn_set_error(std::string(who) + ": d must be a multiple of B (gcn_basis_concat.py:15)");
+    return RGCN_ERR_INVALID;
+  }
   return RGCN_OK;
+}
+
+int pointer_checks(bool pointers_ok, float keep, const char* who) {
+  if (!pointers_ok || keep <= 0.f) {
+    rgcn_set_error(std::string(who) + (pointers_ok ? ": keep <= 0" : ": null pointer"));
+    return RGCN_ERR_INVALID;
+  }
+  return RGCN_OK;
+}
+
+int workspace_checks(int64_t workspace_bytes, int64_t need, const char* who) {
+  if (workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  return RGCN_OK;
+}
+
+// ---- layer frame: the host steps the layer entry points share ------------------------------------------------------
+
+// The split-row scratch of a destination-major walk (partial rows of the rows whose messages span several work items)
+// and its arrival counters, carved from the workspace and zeroed.
+int split_scratch(Carver& ws, int64_t n_split, int d, float*& scratch, int*& counters, cudaStream_t st) {
+  const int slabs = slabs_for(d);
+  scratch = ws.take<float>(n_split * d);
+  counters = ws.take<int>(n_split * slabs);
+  if (n_split == 0) return RGCN_OK;
+  return rgcn_check_cuda(cudaMemsetAsync(scratch, 0, (char*)(counters + n_split * slabs) - (char*)scratch, st),
+                         "memset(scratch)");
+}
+
+// [C_f; C_b]: the coefficient rows indexed by weight id, forward relations first; `count` floats per direction
+int concat_coefficients(const float* Cf, const float* Cb, int64_t count, float* Ccat, cudaStream_t st) {
+  int rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat, Cf, (size_t)count * 4, cudaMemcpyDeviceToDevice, st), "copy Cf");
+  if (!rc)
+    rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat + count, Cb, (size_t)count * 4, cudaMemcpyDeviceToDevice, st), "copy Cb");
+  return rc;
+}
+
+int split_coefficients(const float* dCcat, int64_t count, float* dCf, float* dCb, cudaStream_t st) {
+  int rc = rgcn_check_cuda(cudaMemcpyAsync(dCf, dCcat, (size_t)count * 4, cudaMemcpyDeviceToDevice, st), "copy dCf");
+  if (!rc)
+    rc = rgcn_check_cuda(cudaMemcpyAsync(dCb, dCcat + count, (size_t)count * 4, cudaMemcpyDeviceToDevice, st), "copy dCb");
+  return rc;
+}
+
+// out = H[0:V_dst] W_self, then out *= mask / keep when a mask is given (a walk that applies the mask passes none)
+int self_loop_forward(const rgcn_graph_t* g, int d, const float* H, const float* Wself, const uint8_t* mask, float keep,
+                      float* out, float* split_ws, cudaStream_t st) {
+  int rc = gemm_any(st, split_ws, false, false, g->V_dst, d, d, H, d, Wself, d, 0.f, out, d);
+  if (rc) return rc;
+  return launch_mask_relu(out, mask, 1.0f / keep, 0, (int64_t)g->V_dst * d, st);
+}
+
+// G = dOut * relu'(out);  dS = G * mask / keep  (dropout is on the self loop only).  G and dS come in as workspace
+// slices; without a mask dS is G.  With neither a ReLU nor a mask there is nothing to apply (the node-sharded layers
+// pass the already masked gradient): both are dOut, read in place instead of copied into the workspace (20 GB read +
+// 20 GB written at the full benchmark size).
+int grad_prologue(const float* dOut, const float* out, const uint8_t* mask, float keep, int relu, int64_t n, float*& G,
+                  float*& dS, cudaStream_t st) {
+  if (!relu && !mask) {
+    G = dS = const_cast<float*>(dOut);
+    return RGCN_OK;
+  }
+  if (!mask) dS = G;
+  return launch_grad_prologue(dOut, out, mask, 1.0f / keep, relu, n, G, dS, st);
+}
+
+// dW_self = H[0:V_dst]^T dS, then dH[0:V_dst] = dS W_self^T; the halo rows of dH start at zero.  dW_mark, when given,
+// names the profile stage of the dW_self GEMM.
+int self_loop_backward(const rgcn_graph_t* g, int d, const float* H, const float* dS, const float* Wself, float* dWself,
+                       float* dH, float* split_ws, const char* dW_mark, cudaStream_t st) {
+  int rc = gemm_any(st, split_ws, true, false, d, d, g->V_dst, H, d, dS, d, 0.f, dWself, d);
+  if (rc) return rc;
+  if (dW_mark) prof_mark(dW_mark, st);
+  rc = gemm_any(st, split_ws, false, true, g->V_dst, d, d, dS, d, Wself, d, 0.f, dH, d);
+  if (rc || g->V_src == g->V_dst) return rc;
+  return rgcn_check_cuda(
+      cudaMemsetAsync(dH + (size_t)g->V_dst * d, 0, (size_t)(g->V_src - g->V_dst) * d * sizeof(float), st),
+      "memset(dH halo)");
 }
 
 AggLaunch make_agg(const CsrSide& side, const float* X, int ldx, int d, float* scratch,
@@ -152,26 +249,66 @@ AggLaunch make_agg(const CsrSide& side, const float* X, int ldx, int d, float* s
 // -1 = auto: 3 where it applies, else 1 where it applies, else 0
 static int g_block_algo = -1;
 
-// 3 = weight-id-major with TMA-staged gathers (block_staged.cu) where the block size supports it
-static bool use_staged(int d, int s) {
+// The block message walk of one call, chosen once: weight-id major (`rel`; with TMA-staged gathers where the block size
+// supports them, `staged`) or destination-major, and whether the weight-id-major dH walk also produces dW (`fused`).
+struct BlockWalk {
+  bool rel, staged, fused;
+};
+
+static BlockWalk choose_block_walk(int d, int s) {
   int algo = g_block_algo;
   if (const char* e = std::getenv("RGCN_BLOCK_ALGO")) algo = std::atoi(e);
-  return (algo == 3 || algo == -1) && block_stg_supported(d, s);
+  BlockWalk w;
+  w.rel = algo != 0 && block_rel_supported(d, s);
+  w.staged = (algo == 3 || algo == -1) && block_stg_supported(d, s);
+  w.fused = w.rel && block_rel_fuse_dw_supported(d, s) && !std::getenv("RGCN_NO_FUSE_DW");
+  return w;
 }
 
-static int launch_block_relmajor(const WorkItem* items, int n_items, const int32_t* r_row, const int32_t* r_nbr,
-                                 const float* r_norm, const float* X, int ldx, int d, int s, const float* Wt,
+static int launch_block_relmajor(const BlockWalk& w, const RelSide& side, const float* X, int d, int s, const float* Wt,
                                  float* out, const float* Hrow, int ldh, float* dWt, cudaStream_t st) {
-  if (use_staged(d, s))
-    return launch_block_stg(items, n_items, r_row, r_nbr, r_norm, X, ldx, d, s, Wt, out, Hrow, ldh, dWt, st);
-  return launch_block_rel(items, n_items, r_row, r_nbr, r_norm, X, ldx, d, s, Wt, out, Hrow, ldh, dWt, st);
+  return (w.staged ? launch_block_stg : launch_block_rel)(side.d_items, (int)side.n_items, side.d_row, side.d_nbr,
+                                                          side.d_norm, X, d, d, s, Wt, out, Hrow, ldh, dWt, st);
 }
 
-static bool use_rel_major(int d, int s) {
-  int algo = g_block_algo;
-  if (const char* e = std::getenv("RGCN_BLOCK_ALGO")) algo = std::atoi(e);
-  if (algo == 0) return false;
-  return block_rel_supported(d, s);
+// out[dst] += sum_m norm_m W[relw_m] . X[src_m], with the layer's epilogue: the dropout mask on the self-loop term
+// already in `out` (mask, inv_keep) and the ReLU.  The weight-id-major walks accumulate with vector reductions, so they
+// apply the mask before the walk and leave the ReLU to the caller; the destination-major walk applies both.  scratch
+// and counters: the zeroed split-row scratch of by_dst (split_scratch), read by the destination-major walk only.
+static int block_walk_forward(const rgcn_graph_t* g, const BlockWalk& w, int d, int s, const float* X, const float* Wt,
+                              float* out, const uint8_t* mask, float inv_keep, int relu, float* scratch, int* counters,
+                              cudaStream_t st) {
+  if (w.rel) {
+    int rc = launch_mask_relu(out, mask, inv_keep, 0, (int64_t)g->V_dst * d, st);
+    if (rc) return rc;
+    return launch_block_relmajor(w, g->by_rel, X, d, s, Wt, out, nullptr, 0, nullptr, st);
+  }
+  return launch_block_agg(make_agg(g->by_dst, X, d, d, scratch, counters), s, Wt, out, mask, inv_keep, relu, st);
+}
+
+// dX[src] (+)= sum_m norm_m W[relw_m]^T G[dst_m] with the transposed table Wtt; dX starts at zero when zero_dX, else it
+// holds the self-loop gradient.  dWt is zeroed and, when the walk is fused, accumulates dW in the same walk.  scratch
+// and counters: the zeroed split-row scratch of by_src, read by the destination-major walk only.
+static int block_walk_backward(const rgcn_graph_t* g, const BlockWalk& w, int d, int s, const float* X, const float* G,
+                               const float* Wtt, float* dX, bool zero_dX, float* dWt, float* scratch, int* counters,
+                               cudaStream_t st) {
+  int rc = RGCN_OK;
+  if (zero_dX) rc = rgcn_check_cuda(cudaMemsetAsync(dX, 0, (size_t)g->V_src * d * sizeof(float), st), "memset(dX)");
+  if (rc) return rc;
+  rc = rgcn_check_cuda(cudaMemsetAsync(dWt, 0, (size_t)g->n_relw * s * d * sizeof(float), st), "memset(dWt)");
+  if (rc) return rc;
+  if (w.rel)
+    return launch_block_relmajor(w, g->by_rel_src, G, d, s, Wtt, dX, w.fused ? X : nullptr, d, w.fused ? dWt : nullptr,
+                                 st);
+  return launch_block_agg(make_agg(g->by_src, G, d, d, scratch, counters), s, Wtt, dX, nullptr, 1.f, 0, st);
+}
+
+// dW[w] = sum_{m: relw_m = w} norm_m G[dst_m] (x)_block X[src_m], unless the dH walk produced it
+static int block_walk_dw(const rgcn_graph_t* g, const BlockWalk& w, int d, int s, const float* X, const float* G,
+                         float* dWt, cudaStream_t st) {
+  if (w.fused) return RGCN_OK;
+  return launch_block_dw(g->by_rel.d_items, (int)g->by_rel.n_items, g->by_rel.d_row, g->by_rel.d_nbr,
+                         g->by_rel.d_norm, X, d, G, d, d, s, dWt, st);
 }
 
 extern "C" int rgcn_set_option(const char* name, int64_t value) {
@@ -283,67 +420,41 @@ extern "C" int rgcn_block_forward(const rgcn_graph_t* g, int32_t d, int32_t B, c
                                   const float* Wf, const float* Wb, const float* Wself,
                                   const uint8_t* drop_mask, float keep, int relu, float* out,
                                   void* workspace, int64_t workspace_bytes, void* stream) {
-  int rc = layer_checks(g, d, B, "rgcn_block_forward");
+  const char* who = "rgcn_block_forward";
+  int rc = graph_checks(g, d, B, who, true, false, false);
+  if (!rc) rc = block_size_checks(d, B, who);
+  if (!rc) rc = pointer_checks(H && Wf && Wb && Wself && out && workspace, keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_block_workspace_bytes(g, d, B, 0), who);
   if (rc) return rc;
-  if (d % B != 0) {
-    rgcn_set_error("rgcn_block_forward: d must be a multiple of B (gcn_basis_concat.py:15)");
-    return RGCN_ERR_INVALID;
-  }
-  if (!H || !Wf || !Wb || !Wself || !out || !workspace || keep <= 0.f) {
-    rgcn_set_error("rgcn_block_forward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_block_workspace_bytes(g, d, B, 0)) {
-    rgcn_set_error("rgcn_block_forward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
   if (rc) return rc;
   const int s = d / B, R = g->n_relw / 2;
-  {
-    const bool relm = use_rel_major(d, s);
-    rc = need_views(g, !relm, relm, "rgcn_block_forward");
-    if (rc) return rc;
-  }
-  const int slabs = slabs_for(d);
-  const int64_t n_split = g->by_dst.n_split;
+  const BlockWalk walk = choose_block_walk(d, s);
+  rc = need_views(g, !walk.rel, walk.rel, who);
+  if (rc) return rc;
   Carver ws(workspace, workspace_bytes);
   float* split_ws = ws.take<float>((int64_t)2 * d * d);
   float* Wt = ws.take<float>((int64_t)g->n_relw * s * d);
-  float* scratch = ws.take<float>(n_split * d);
-  int* counters = ws.take<int>(n_split * slabs);
 
   MARK("start");
   rc = launch_block_relayout(Wf, Wb, R, B, s, /*transpose=*/0, Wt, st);
   if (rc) return rc;
   MARK("block_relayout");
-  if (n_split > 0) {
-    rc = rgcn_check_cuda(
-        cudaMemsetAsync(scratch, 0, (char*)(counters + n_split * slabs) - (char*)scratch, st),
-        "memset(scratch)");
-    if (rc) return rc;
-  }
-  // self-loop term S = H[0:V_dst] @ W_self written straight into `out` (gcn_basis_concat.py:65-66)
-  rc = gemm_any(st, split_ws, false, false, g->V_dst, d, d, H, d, Wself, d, 0.f, out, d);
+  float* scratch;
+  int* counters;
+  rc = split_scratch(ws, g->by_dst.n_split, d, scratch, counters, st);
+  if (rc) return rc;
+  // self-loop term S = H[0:V_dst] @ W_self written straight into `out` (gcn_basis_concat.py:65-66); the walk applies
+  // the dropout mask to it
+  rc = self_loop_forward(g, d, H, Wself, nullptr, keep, out, split_ws, st);
   if (rc) return rc;
   MARK("gemm_self_loop");
-  if (use_rel_major(d, s)) {
-    // out = dropout(S);  out[dst] += W_r . sum(norm x)  (L2 vector reductions);  out = relu(out)
-    rc = launch_mask_relu(out, drop_mask, 1.0f / keep, 0, (int64_t)g->V_dst * d, st);
-    if (rc) return rc;
-    rc = launch_block_relmajor(g->by_rel.d_items, (int)g->by_rel.n_items, g->by_rel.d_row,
-                          g->by_rel.d_nbr, g->by_rel.d_norm, H, d, d, s, Wt, out, nullptr, 0, nullptr,
-                          st);
-    if (rc) return rc;
-    MARK("block_agg_fwd");
-    rc = launch_mask_relu(out, nullptr, 1.f, relu, (int64_t)g->V_dst * d, st);
-    MARK("relu_epilogue");
-    return rc;
-  }
-  AggLaunch a = make_agg(g->by_dst, H, d, d, scratch, counters);
-  rc = launch_block_agg(a, s, Wt, out, drop_mask, 1.0f / keep, relu, st);
+  rc = block_walk_forward(g, walk, d, s, H, Wt, out, drop_mask, 1.0f / keep, relu, scratch, counters, st);
   MARK("block_agg_fwd");
+  if (rc || !walk.rel) return rc;
+  rc = launch_mask_relu(out, nullptr, 1.f, relu, (int64_t)g->V_dst * d, st);
+  MARK("relu_epilogue");
   return rc;
 }
 
@@ -353,32 +464,21 @@ extern "C" int rgcn_block_backward(const rgcn_graph_t* g, int32_t d, int32_t B, 
                                    const float* dOut, float* dH, float* dWf, float* dWb,
                                    float* dWself, void* workspace, int64_t workspace_bytes,
                                    void* stream) {
-  int rc = layer_checks(g, d, B, "rgcn_block_backward");
+  const char* who = "rgcn_block_backward";
+  int rc = graph_checks(g, d, B, who, true, false, false);
+  if (!rc) rc = block_size_checks(d, B, who);
+  if (!rc)
+    rc = pointer_checks(H && Wf && Wb && Wself && dOut && dH && dWf && dWb && dWself && workspace && (!relu || out),
+                        keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_block_workspace_bytes(g, d, B, 1), who);
   if (rc) return rc;
-  if (d % B != 0) {
-    rgcn_set_error("rgcn_block_backward: d must be a multiple of B");
-    return RGCN_ERR_INVALID;
-  }
-  if (!H || !Wf || !Wb || !Wself || !dOut || !dH || !dWf || !dWb || !dWself || !workspace ||
-      (relu && !out) || keep <= 0.f) {
-    rgcn_set_error("rgcn_block_backward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_block_workspace_bytes(g, d, B, 1)) {
-    rgcn_set_error("rgcn_block_backward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
   if (rc) return rc;
   const int s = d / B, R = g->n_relw / 2;
-  {
-    const bool relm = use_rel_major(d, s);
-    rc = need_views(g, !relm, true, "rgcn_block_backward");
-    if (rc) return rc;
-  }
-  const int slabs = slabs_for(d);
-  const int64_t n_split = g->by_src.n_split;
+  const BlockWalk walk = choose_block_walk(d, s);
+  rc = need_views(g, !walk.rel, true, who);
+  if (rc) return rc;
   const int64_t wt = (int64_t)g->n_relw * s * d;
   Carver ws(workspace, workspace_bytes);
   float* split_ws = ws.take<float>((int64_t)2 * d * d);
@@ -386,69 +486,31 @@ extern "C" int rgcn_block_backward(const rgcn_graph_t* g, int32_t d, int32_t B, 
   float* dWt = ws.take<float>(wt);
   float* G = ws.take<float>((int64_t)g->V_dst * d);
   float* dS = ws.take<float>((int64_t)g->V_dst * d);
-  float* scratch = ws.take<float>(n_split * d);
-  int* counters = ws.take<int>(n_split * slabs);
-  if (!drop_mask) dS = G;
 
-  // G = dOut * relu'(out);  dS = G * mask / keep   (message_gcn.py:64 dropout is on the self loop only)
   MARK("start");
-  if (!relu && !drop_mask) {
-    // nothing to apply (the node-sharded layers pass the already masked gradient): read dOut in place instead of
-    // copying it into the workspace (20 GB read + 20 GB written at the full benchmark size)
-    G = dS = const_cast<float*>(dOut);
-  } else {
-    rc = launch_grad_prologue(dOut, out, drop_mask, 1.0f / keep, relu, (int64_t)g->V_dst * d, G, dS, st);
-    if (rc) return rc;
-  }
+  rc = grad_prologue(dOut, out, drop_mask, keep, relu, (int64_t)g->V_dst * d, G, dS, st);  // message_gcn.py:64
+  if (rc) return rc;
   MARK("grad_prologue");
-  // dW_self = H[0:V_dst]^T dS
-  rc = gemm_any(st, split_ws, true, false, d, d, g->V_dst, H, d, dS, d, 0.f, dWself, d);
+  rc = self_loop_backward(g, d, H, dS, Wself, dWself, dH, split_ws, "gemm_dWself", st);
   if (rc) return rc;
-  MARK("gemm_dWself");
-  // dH[0:V_dst] = dS W_self^T ; halo rows start at zero
-  rc = gemm_any(st, split_ws, false, true, g->V_dst, d, d, dS, d, Wself, d, 0.f, dH, d);
-  if (rc) return rc;
-  if (g->V_src > g->V_dst) {
-    rc = rgcn_check_cuda(cudaMemsetAsync(dH + (size_t)g->V_dst * d, 0,
-                                         (size_t)(g->V_src - g->V_dst) * d * sizeof(float), st),
-                         "memset(dH halo)");
-    if (rc) return rc;
-  }
   MARK("gemm_dH_self");
   // dH[u] += sum_{m: src_m = u} norm_m W[relw_m]^T G[dst_m]   (same kernel, transposed table)
   rc = launch_block_relayout(Wf, Wb, R, B, s, /*transpose=*/1, Wtt, st);
   if (rc) return rc;
   MARK("block_relayout_T");
-  if (n_split > 0) {
-    rc = rgcn_check_cuda(
-        cudaMemsetAsync(scratch, 0, (char*)(counters + n_split * slabs) - (char*)scratch, st),
-        "memset(scratch)");
-    if (rc) return rc;
-  }
-  // dW accumulates in the j-major layout (zeroed first); when the block size allows, the dH pass
-  // produces it in the same walk (one round of gathers for the whole backward of the messages)
-  rc = rgcn_check_cuda(cudaMemsetAsync(dWt, 0, wt * sizeof(float), st), "memset(dWt)");
+  float* scratch;
+  int* counters;
+  rc = split_scratch(ws, g->by_src.n_split, d, scratch, counters, st);
   if (rc) return rc;
-  const bool rel = use_rel_major(d, s);
-  const bool fused = rel && block_rel_fuse_dw_supported(d, s) && !std::getenv("RGCN_NO_FUSE_DW");
-  if (rel) {
-    rc = launch_block_relmajor(g->by_rel_src.d_items, (int)g->by_rel_src.n_items, g->by_rel_src.d_row,
-                          g->by_rel_src.d_nbr, g->by_rel_src.d_norm, G, d, d, s, Wtt, dH,
-                          fused ? H : nullptr, d, fused ? dWt : nullptr, st);
-  } else {
-    AggLaunch a = make_agg(g->by_src, G, d, d, scratch, counters);
-    rc = launch_block_agg(a, s, Wtt, dH, nullptr, 1.f, 0, st);
-  }
+  // dW accumulates in the j-major layout; when the block size allows, the dH pass produces it in the same walk (one
+  // round of gathers for the whole backward of the messages)
+  rc = block_walk_backward(g, walk, d, s, H, G, Wtt, dH, false, dWt, scratch, counters, st);
   if (rc) return rc;
   MARK("block_agg_dH");
-  // dW[w] = sum_{m: relw_m = w} norm_m G[dst_m] (x)_block H[src_m]
-  if (!fused) {
-    rc = launch_block_dw(g->by_rel.d_items, (int)g->by_rel.n_items, g->by_rel.d_row,
-                         g->by_rel.d_nbr, g->by_rel.d_norm, H, d, G, d, d, s, dWt, st);
-    if (rc) return rc;
-  }
+  rc = block_walk_dw(g, walk, d, s, H, G, dWt, st);
+  if (rc) return rc;
   MARK("block_dW");
-  rc = launch_block_unlayout(dWt, R, B, s, dWf, dWb, 0, fused ? 1 : 0, st);
+  rc = launch_block_unlayout(dWt, R, B, s, dWf, dWb, 0, walk.fused ? 1 : 0, st);
   MARK("block_unlayout");
   return rc;
 }
@@ -473,47 +535,28 @@ extern "C" int64_t rgcn_block_aggregate_workspace_bytes(const rgcn_graph_t* g, i
 extern "C" int rgcn_block_aggregate(const rgcn_graph_t* g, int32_t d, int32_t B, const float* X,
                                     const float* Wf, const float* Wb, float* out, void* workspace,
                                     int64_t workspace_bytes, void* stream) {
-  int rc = common_checks(g, d, B, "rgcn_block_aggregate");
+  const char* who = "rgcn_block_aggregate";
+  int rc = graph_checks(g, d, B, who, false, false, false);
+  if (!rc) rc = block_size_checks(d, B, who);
+  if (!rc) rc = pointer_checks(X && Wf && Wb && out && workspace, 1.f, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_block_aggregate_workspace_bytes(g, d, B, 0), who);
   if (rc) return rc;
-  if (d % B != 0 || !X || !Wf || !Wb || !out || !workspace) {
-    rgcn_set_error("rgcn_block_aggregate: bad arguments");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_block_aggregate_workspace_bytes(g, d, B, 0)) {
-    rgcn_set_error("rgcn_block_aggregate: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
   if (rc) return rc;
   const int s = d / B, R = g->n_relw / 2;
-  {
-    const bool relm = use_rel_major(d, s);
-    rc = need_views(g, !relm, relm, "rgcn_block_aggregate");
-    if (rc) return rc;
-  }
-  const int slabs = slabs_for(d);
-  const int64_t n_split = g->by_dst.n_split;
+  const BlockWalk walk = choose_block_walk(d, s);
+  rc = need_views(g, !walk.rel, walk.rel, who);
+  if (rc) return rc;
   Carver ws(workspace, workspace_bytes);
   float* Wt = ws.take<float>((int64_t)g->n_relw * s * d);
-  float* scratch = ws.take<float>(n_split * d);
-  int* counters = ws.take<int>(n_split * slabs);
   MARK("start");
+  float* scratch;
+  int* counters;
   rc = launch_block_relayout(Wf, Wb, R, B, s, 0, Wt, st);
+  if (!rc) rc = split_scratch(ws, g->by_dst.n_split, d, scratch, counters, st);
   if (rc) return rc;
-  if (use_rel_major(d, s)) {
-    rc = launch_block_relmajor(g->by_rel.d_items, (int)g->by_rel.n_items, g->by_rel.d_row, g->by_rel.d_nbr,
-                          g->by_rel.d_norm, X, d, d, s, Wt, out, nullptr, 0, nullptr, st);
-  } else {
-    if (n_split > 0) {
-      rc = rgcn_check_cuda(
-          cudaMemsetAsync(scratch, 0, (char*)(counters + n_split * slabs) - (char*)scratch, st),
-          "memset(scratch)");
-      if (rc) return rc;
-    }
-    AggLaunch a = make_agg(g->by_dst, X, d, d, scratch, counters);
-    rc = launch_block_agg(a, s, Wt, out, nullptr, 1.f, 0, st);  // out = out + sum (in-place epilogue)
-  }
+  rc = block_walk_forward(g, walk, d, s, X, Wt, out, nullptr, 1.f, 0, scratch, counters, st);  // out = out + sum
   MARK("block_aggregate");
   return rc;
 }
@@ -523,64 +566,33 @@ extern "C" int rgcn_block_aggregate_backward(const rgcn_graph_t* g, int32_t d, i
                                              const float* G, float* dX, float* dWf, float* dWb,
                                              int accumulate_dW, void* workspace,
                                              int64_t workspace_bytes, void* stream) {
-  int rc = common_checks(g, d, B, "rgcn_block_aggregate_backward");
+  const char* who = "rgcn_block_aggregate_backward";
+  int rc = graph_checks(g, d, B, who, false, false, false);
+  if (!rc) rc = block_size_checks(d, B, who);
+  if (!rc) rc = pointer_checks(X && Wf && Wb && G && dX && dWf && dWb && workspace, 1.f, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_block_aggregate_workspace_bytes(g, d, B, 1), who);
   if (rc) return rc;
-  if (d % B != 0 || !X || !Wf || !Wb || !G || !dX || !dWf || !dWb || !workspace) {
-    rgcn_set_error("rgcn_block_aggregate_backward: bad arguments");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_block_aggregate_workspace_bytes(g, d, B, 1)) {
-    rgcn_set_error("rgcn_block_aggregate_backward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
   if (rc) return rc;
   const int s = d / B, R = g->n_relw / 2;
-  {
-    const bool relm = use_rel_major(d, s);
-    rc = need_views(g, !relm, true, "rgcn_block_aggregate_backward");
-    if (rc) return rc;
-  }
-  const int slabs = slabs_for(d);
-  const int64_t n_split = g->by_src.n_split;
+  const BlockWalk walk = choose_block_walk(d, s);
+  rc = need_views(g, !walk.rel, true, who);
+  if (rc) return rc;
   const int64_t wt = (int64_t)g->n_relw * s * d;
   Carver ws(workspace, workspace_bytes);
   float* Wtt = ws.take<float>(wt);
   float* dWt = ws.take<float>(wt);
-  float* scratch = ws.take<float>(n_split * d);
-  int* counters = ws.take<int>(n_split * slabs);
   MARK("start");
+  float* scratch;
+  int* counters;
   rc = launch_block_relayout(Wf, Wb, R, B, s, 1, Wtt, st);
+  if (!rc) rc = split_scratch(ws, g->by_src.n_split, d, scratch, counters, st);
+  if (!rc) rc = block_walk_backward(g, walk, d, s, X, G, Wtt, dX, true, dWt, scratch, counters, st);
+  if (!rc) rc = block_walk_dw(g, walk, d, s, X, G, dWt, st);
   if (rc) return rc;
-  rc = rgcn_check_cuda(cudaMemsetAsync(dX, 0, (size_t)g->V_src * d * sizeof(float), st), "memset(dX)");
-  if (rc) return rc;
-  rc = rgcn_check_cuda(cudaMemsetAsync(dWt, 0, wt * sizeof(float), st), "memset(dWt)");
-  if (rc) return rc;
-  const bool rel = use_rel_major(d, s);
-  const bool fused = rel && block_rel_fuse_dw_supported(d, s) && !std::getenv("RGCN_NO_FUSE_DW");
-  if (rel) {
-    rc = launch_block_relmajor(g->by_rel_src.d_items, (int)g->by_rel_src.n_items, g->by_rel_src.d_row,
-                          g->by_rel_src.d_nbr, g->by_rel_src.d_norm, G, d, d, s, Wtt, dX,
-                          fused ? X : nullptr, d, fused ? dWt : nullptr, st);
-  } else {
-    if (n_split > 0) {
-      rc = rgcn_check_cuda(
-          cudaMemsetAsync(scratch, 0, (char*)(counters + n_split * slabs) - (char*)scratch, st),
-          "memset(scratch)");
-      if (rc) return rc;
-    }
-    AggLaunch a = make_agg(g->by_src, G, d, d, scratch, counters);
-    rc = launch_block_agg(a, s, Wtt, dX, nullptr, 1.f, 0, st);
-  }
-  if (rc) return rc;
-  if (!fused) {
-    rc = launch_block_dw(g->by_rel.d_items, (int)g->by_rel.n_items, g->by_rel.d_row, g->by_rel.d_nbr,
-                         g->by_rel.d_norm, X, d, G, d, d, s, dWt, st);
-    if (rc) return rc;
-  }
   MARK("block_aggregate_bwd");
-  return launch_block_unlayout(dWt, R, B, s, dWf, dWb, accumulate_dW, fused ? 1 : 0, st);
+  return launch_block_unlayout(dWt, R, B, s, dWf, dWb, accumulate_dW, walk.fused ? 1 : 0, st);
 }
 
 // dst[rows[i], :] += src[i, :] (rows unique): unpack of the returned halo gradients, one peer segment per call
@@ -636,18 +648,11 @@ extern "C" int rgcn_basis_forward(const rgcn_graph_t* g, int32_t d, int32_t B, c
                                   const float* Cb, const float* Wself, const uint8_t* drop_mask,
                                   float keep, int relu, float* out, float* saved, void* workspace,
                                   int64_t workspace_bytes, void* stream) {
-  int rc = layer_checks(g, d, B, "rgcn_basis_forward");
+  const char* who = "rgcn_basis_forward";
+  int rc = graph_checks(g, d, B, who, true, true, false);
+  if (!rc) rc = pointer_checks(H && Vf && Vb && Cf && Cb && Wself && out && saved && workspace, keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_basis_workspace_bytes(g, d, B, 0), who);
   if (rc) return rc;
-  rc = need_views(g, true, false, "rgcn_basis_forward");
-  if (rc) return rc;
-  if (!H || !Vf || !Vb || !Cf || !Cb || !Wself || !out || !saved || !workspace || keep <= 0.f) {
-    rgcn_set_error("rgcn_basis_forward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_basis_workspace_bytes(g, d, B, 0)) {
-    rgcn_set_error("rgcn_basis_forward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
   if (rc) return rc;
@@ -656,8 +661,7 @@ extern "C" int rgcn_basis_forward(const rgcn_graph_t* g, int32_t d, int32_t B, c
   Carver ws(workspace, workspace_bytes);
   float* Ccat = ws.take<float>((int64_t)g->n_relw * B);
   float* split_ws = ws.take<float>((int64_t)2 * d * d * B);
-  rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat, Cf, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy Cf");
-  if (!rc) rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat + (size_t)R * B, Cb, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy Cb");
+  rc = concat_coefficients(Cf, Cb, (int64_t)R * B, Ccat, st);
   if (rc) return rc;
   MARK("start");
   // Agg[v][dir][k*B+b] = sum_m norm_m C[relw_m,b] H[src_m,k]
@@ -667,9 +671,7 @@ extern "C" int rgcn_basis_forward(const rgcn_graph_t* g, int32_t d, int32_t B, c
   rc = launch_basis_agg(a, Ccat, B, g->n_relw, /*layout=*/0, saved, st);
   if (rc) return rc;
   MARK("basis_agg_fwd");
-  rc = gemm_any(st, split_ws, false, false, g->V_dst, d, d, H, d, Wself, d, 0.f, out, d);
-  if (rc) return rc;
-  rc = launch_mask_relu(out, drop_mask, 1.0f / keep, 0, (int64_t)g->V_dst * d, st);
+  rc = self_loop_forward(g, d, H, Wself, drop_mask, keep, out, split_ws, st);
   if (rc) return rc;
   // out += Agg_f @ Vf.reshape(d*B, d) + Agg_b @ Vb.reshape(d*B, d)    (gcn_basis.py:60-68 re-associated)
   rc = gemm_any(st, split_ws, false, false, g->V_dst, d, dB, saved, 2 * dB, Vf, d, 1.f, out, d);
@@ -689,19 +691,14 @@ extern "C" int rgcn_basis_backward(const rgcn_graph_t* g, int32_t d, int32_t B, 
                                    const float* dOut, float* dH, float* dVf, float* dVb, float* dCf,
                                    float* dCb, float* dWself, void* workspace,
                                    int64_t workspace_bytes, void* stream) {
-  int rc = layer_checks(g, d, B, "rgcn_basis_backward");
+  const char* who = "rgcn_basis_backward";
+  int rc = graph_checks(g, d, B, who, true, true, false);
+  if (!rc)
+    rc = pointer_checks(H && Vf && Vb && Cf && Cb && Wself && saved && dOut && dH && dVf && dVb && dCf && dCb &&
+                            dWself && workspace && (!relu || out),
+                        keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_basis_workspace_bytes(g, d, B, 1), who);
   if (rc) return rc;
-  rc = need_views(g, true, false, "rgcn_basis_backward");
-  if (rc) return rc;
-  if (!H || !Vf || !Vb || !Cf || !Cb || !Wself || !saved || !dOut || !dH || !dVf || !dVb || !dCf ||
-      !dCb || !dWself || !workspace || (relu && !out) || keep <= 0.f) {
-    rgcn_set_error("rgcn_basis_backward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_basis_workspace_bytes(g, d, B, 1)) {
-    rgcn_set_error("rgcn_basis_backward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
   if (rc) return rc;
@@ -715,24 +712,13 @@ extern "C" int rgcn_basis_backward(const rgcn_graph_t* g, int32_t d, int32_t B, 
   float* dS = ws.take<float>((int64_t)g->V_dst * d);
   float* dAgg = ws.take<float>((int64_t)g->V_dst * 2 * dB);
   float* P = ws.take<float>((int64_t)g->V_src * 2 * dB);
-  if (!drop_mask) dS = G;
-  rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat, Cf, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy Cf");
-  if (!rc) rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat + (size_t)R * B, Cb, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy Cb");
+  rc = concat_coefficients(Cf, Cb, (int64_t)R * B, Ccat, st);
   if (rc) return rc;
 
   MARK("start");
-  rc = launch_grad_prologue(dOut, out, drop_mask, 1.0f / keep, relu, (int64_t)g->V_dst * d, G, dS, st);
+  rc = grad_prologue(dOut, out, drop_mask, keep, relu, (int64_t)g->V_dst * d, G, dS, st);
+  if (!rc) rc = self_loop_backward(g, d, H, dS, Wself, dWself, dH, split_ws, nullptr, st);
   if (rc) return rc;
-  rc = gemm_any(st, split_ws, true, false, d, d, g->V_dst, H, d, dS, d, 0.f, dWself, d);
-  if (rc) return rc;
-  rc = gemm_any(st, split_ws, false, true, g->V_dst, d, d, dS, d, Wself, d, 0.f, dH, d);
-  if (rc) return rc;
-  if (g->V_src > g->V_dst) {
-    rc = rgcn_check_cuda(cudaMemsetAsync(dH + (size_t)g->V_dst * d, 0,
-                                         (size_t)(g->V_src - g->V_dst) * d * sizeof(float), st),
-                         "memset(dH halo)");
-    if (rc) return rc;
-  }
   MARK("basis_self_loop_bwd");
   // dV_dir.reshape(d*B, d) = Agg_dir^T G
   rc = gemm_any(st, split_ws, true, false, dB, d, g->V_dst, saved, 2 * dB, G, d, 0.f, dVf, d);
@@ -752,8 +738,7 @@ extern "C" int rgcn_basis_backward(const rgcn_graph_t* g, int32_t d, int32_t B, 
   rc = launch_basis_dc(a, dAgg, B, g->n_relw, dCcat, st);
   if (rc) return rc;
   MARK("basis_dC");
-  rc = rgcn_check_cuda(cudaMemcpyAsync(dCf, dCcat, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy dCf");
-  if (!rc) rc = rgcn_check_cuda(cudaMemcpyAsync(dCb, dCcat + (size_t)R * B, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy dCb");
+  rc = split_coefficients(dCcat, (int64_t)R * B, dCf, dCb, st);
   if (rc) return rc;
   // P[u][dir][b*d+n] = sum_{m: src_m=u} norm_m C[relw_m,b] G[dst_m,n];  dH += P_dir V_dir.reshape(d, B*d)^T
   rc = launch_zero_rows(P, 2 * dB, g->by_src.d_split_rows, (int)g->by_src.n_split, st);
@@ -785,43 +770,15 @@ extern "C" int64_t rgcn_basis_onehot_workspace_bytes(const rgcn_graph_t* g, int3
   return bytes + 256;
 }
 
-// argument validation runs before anything touches the device: bad shapes, null pointers and short workspaces are
-// RGCN_ERR_INVALID / RGCN_ERR_WORKSPACE even for a host-only graph
-static int onehot_shape_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
-  if (!g || d <= 0 || d % 4 != 0 || B <= 0) {
-    rgcn_set_error(std::string(who) + ": need a graph, d > 0, d % 4 == 0, B > 0");
-    return RGCN_ERR_INVALID;
-  }
-  return RGCN_OK;
-}
-
-static int onehot_graph_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
-  int rc = layer_checks(g, d, B, who);
-  if (rc) return rc;
-  return need_views(g, true, false, who);
-}
-
-static int concat_coefficients(const float* Cf, const float* Cb, int R, int B, float* Ccat, cudaStream_t st) {
-  int rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat, Cf, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy Cf");
-  if (!rc) rc = rgcn_check_cuda(cudaMemcpyAsync(Ccat + (size_t)R * B, Cb, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy Cb");
-  return rc;
-}
-
 extern "C" int rgcn_basis_onehot_forward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* Wf,
                                          const float* Wb, const float* Cf, const float* Cb, const float* Wself,
                                          const uint8_t* drop_mask, float keep, int relu, float* out, void* workspace,
                                          int64_t workspace_bytes, void* stream) {
-  int rc = onehot_shape_checks(g, d, B, "rgcn_basis_onehot_forward");
-  if (rc) return rc;
-  if (!Wf || !Wb || !Cf || !Cb || !Wself || !out || !workspace || keep <= 0.f) {
-    rgcn_set_error("rgcn_basis_onehot_forward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_basis_onehot_workspace_bytes(g, d, B, 0)) {
-    rgcn_set_error("rgcn_basis_onehot_forward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
-  rc = onehot_graph_checks(g, d, B, "rgcn_basis_onehot_forward");
+  const char* who = "rgcn_basis_onehot_forward";
+  int rc = shape_checks(g, d, B, who);
+  if (!rc) rc = pointer_checks(Wf && Wb && Cf && Cb && Wself && out && workspace, keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_basis_onehot_workspace_bytes(g, d, B, 0), who);
+  if (!rc) rc = graph_checks(g, d, B, who, true, true, false);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
@@ -830,7 +787,7 @@ extern "C" int rgcn_basis_onehot_forward(const rgcn_graph_t* g, int32_t d, int32
   const int64_t n = (int64_t)g->V_dst * d;
   Carver ws(workspace, workspace_bytes);
   float* Ccat = ws.take<float>((int64_t)g->n_relw * B);
-  rc = concat_coefficients(Cf, Cb, R, B, Ccat, st);
+  rc = concat_coefficients(Cf, Cb, (int64_t)R * B, Ccat, st);
   if (rc) return rc;
   MARK("start");
   // out = dropout(W_self)  (the self loop looks up W_self with tf.range(V): message_gcn.py:56, gcn_basis.py:70-71)
@@ -853,18 +810,13 @@ extern "C" int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int3
                                           const uint8_t* drop_mask, float keep, int relu, const float* out,
                                           const float* dOut, float* dWf, float* dWb, float* dCf, float* dCb,
                                           float* dWself, void* workspace, int64_t workspace_bytes, void* stream) {
-  int rc = onehot_shape_checks(g, d, B, "rgcn_basis_onehot_backward");
-  if (rc) return rc;
-  if (!Wf || !Wb || !Cf || !Cb || !dOut || !dWf || !dWb || !dCf || !dCb || !dWself || !workspace ||
-      (relu && !out) || keep <= 0.f) {
-    rgcn_set_error("rgcn_basis_onehot_backward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_basis_onehot_workspace_bytes(g, d, B, 1)) {
-    rgcn_set_error("rgcn_basis_onehot_backward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
-  rc = onehot_graph_checks(g, d, B, "rgcn_basis_onehot_backward");
+  const char* who = "rgcn_basis_onehot_backward";
+  int rc = shape_checks(g, d, B, who);
+  if (!rc)
+    rc = pointer_checks(
+        Wf && Wb && Cf && Cb && dOut && dWf && dWb && dCf && dCb && dWself && workspace && (!relu || out), keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_basis_onehot_workspace_bytes(g, d, B, 1), who);
+  if (!rc) rc = graph_checks(g, d, B, who, true, true, false);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
@@ -875,7 +827,7 @@ extern "C" int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int3
   float* Ccat = ws.take<float>((int64_t)g->n_relw * B);
   float* dCcat = ws.take<float>((int64_t)g->n_relw * B);
   float* G = ws.take<float>((int64_t)g->V_dst * d);
-  rc = concat_coefficients(Cf, Cb, R, B, Ccat, st);
+  rc = concat_coefficients(Cf, Cb, (int64_t)R * B, Ccat, st);
   if (rc) return rc;
   MARK("start");
   // G = dOut * relu'(out);  dW_self = G * mask / keep (without a mask dW_self IS G: written once, read in place)
@@ -892,9 +844,7 @@ extern "C" int rgcn_basis_onehot_backward(const rgcn_graph_t* g, int32_t d, int3
   rc = launch_basis_agg_dc(a, Ccat, B, g->n_relw, Wf, Wb, dWf, dWb, dCcat, st);
   if (rc) return rc;
   MARK("onehot_agg_dW_dC");
-  rc = rgcn_check_cuda(cudaMemcpyAsync(dCf, dCcat, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy dCf");
-  if (!rc) rc = rgcn_check_cuda(cudaMemcpyAsync(dCb, dCcat + (size_t)R * B, (size_t)R * B * 4, cudaMemcpyDeviceToDevice, st), "copy dCb");
-  return rc;
+  return split_coefficients(dCcat, (int64_t)R * B, dCf, dCb, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -915,29 +865,16 @@ extern "C" int64_t rgcn_basis_diagcoef_workspace_bytes(const rgcn_graph_t* g, in
   return bytes + 256;
 }
 
-// shape, pointer and workspace checks first, then the graph (device, views) -- nothing touches the device before
-static int diagcoef_graph_checks(const rgcn_graph_t* g, int32_t d, int32_t B, const char* who) {
-  int rc = layer_checks(g, d, B, who);
-  if (rc) return rc;
-  return need_views(g, true, true, who);
-}
-
 extern "C" int rgcn_basis_diagcoef_forward(const rgcn_graph_t* g, int32_t d, int32_t B, const float* H,
                                            const float* Vf, const float* Vb, const float* Cf, const float* Cb,
                                            const float* Wself, const float* b, const uint8_t* drop_mask, float keep,
                                            int relu, float* out, float* saved, void* workspace,
                                            int64_t workspace_bytes, void* stream) {
-  int rc = onehot_shape_checks(g, d, B, "rgcn_basis_diagcoef_forward");
-  if (rc) return rc;
-  if (!H || !Vf || !Vb || !Cf || !Cb || !Wself || !b || !out || !saved || !workspace || keep <= 0.f) {
-    rgcn_set_error("rgcn_basis_diagcoef_forward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_basis_diagcoef_workspace_bytes(g, d, B, 0)) {
-    rgcn_set_error("rgcn_basis_diagcoef_forward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
-  rc = diagcoef_graph_checks(g, d, B, "rgcn_basis_diagcoef_forward");
+  const char* who = "rgcn_basis_diagcoef_forward";
+  int rc = shape_checks(g, d, B, who);
+  if (!rc) rc = pointer_checks(H && Vf && Vb && Cf && Cb && Wself && b && out && saved && workspace, keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_basis_diagcoef_workspace_bytes(g, d, B, 0), who);
+  if (!rc) rc = graph_checks(g, d, B, who, true, true, true);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
@@ -955,8 +892,7 @@ extern "C" int rgcn_basis_diagcoef_forward(const rgcn_graph_t* g, int32_t d, int
   if (!rc) rc = gemm_any(st, split_ws, false, false, g->V_src, dB, d, H, d, Vb, dB, 0.f, saved + dB, 2 * dB);
   if (rc) return rc;
   MARK("diagcoef_gemms_P");
-  rc = gemm_any(st, split_ws, false, false, g->V_dst, d, d, H, d, Wself, d, 0.f, out, d);
-  if (!rc) rc = launch_mask_relu(out, drop_mask, 1.0f / keep, 0, (int64_t)g->V_dst * d, st);
+  rc = self_loop_forward(g, d, H, Wself, drop_mask, keep, out, split_ws, st);
   if (rc) return rc;
   MARK("gemm_self_loop");
   rc = launch_diagcoef_fwd(g->by_dst.d_items, (int)g->by_dst.n_items, g->by_dst.d_nbr, g->by_dst.d_relw,
@@ -974,18 +910,14 @@ extern "C" int rgcn_basis_diagcoef_backward(const rgcn_graph_t* g, int32_t d, in
                                             const float* out, const float* saved, const float* dOut, float* dH,
                                             float* dVf, float* dVb, float* dCf, float* dCb, float* dWself, float* db,
                                             void* workspace, int64_t workspace_bytes, void* stream) {
-  int rc = onehot_shape_checks(g, d, B, "rgcn_basis_diagcoef_backward");
-  if (rc) return rc;
-  if (!H || !Vf || !Vb || !Cf || !Cb || !Wself || !saved || !dOut || !dH || !dVf || !dVb || !dCf || !dCb ||
-      !dWself || !db || !workspace || (relu && !out) || keep <= 0.f) {
-    rgcn_set_error("rgcn_basis_diagcoef_backward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_basis_diagcoef_workspace_bytes(g, d, B, 1)) {
-    rgcn_set_error("rgcn_basis_diagcoef_backward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
-  rc = diagcoef_graph_checks(g, d, B, "rgcn_basis_diagcoef_backward");
+  const char* who = "rgcn_basis_diagcoef_backward";
+  int rc = shape_checks(g, d, B, who);
+  if (!rc)
+    rc = pointer_checks(H && Vf && Vb && Cf && Cb && Wself && saved && dOut && dH && dVf && dVb && dCf && dCb &&
+                            dWself && db && workspace && (!relu || out),
+                        keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_basis_diagcoef_workspace_bytes(g, d, B, 1), who);
+  if (!rc) rc = graph_checks(g, d, B, who, true, true, true);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
@@ -998,31 +930,15 @@ extern "C" int rgcn_basis_diagcoef_backward(const rgcn_graph_t* g, int32_t d, in
   float* G = ws.take<float>((int64_t)g->V_dst * d);
   float* dS = ws.take<float>((int64_t)g->V_dst * d);
   float* dP = ws.take<float>((int64_t)g->V_src * 2 * dB);
-  if (!drop_mask) dS = G;
 
   MARK("start");
   rc = launch_diagcoef_sigmoid(Cf, Cb, (int64_t)R * dB, sig, st);
-  if (rc) return rc;
-  // G = dOut * relu'(out);  dS = G * mask / keep   (dropout is on the self loop only)
-  if (!relu && !drop_mask) {
-    G = dS = const_cast<float*>(dOut);
-  } else {
-    rc = launch_grad_prologue(dOut, out, drop_mask, 1.0f / keep, relu, (int64_t)g->V_dst * d, G, dS, st);
-    if (rc) return rc;
-  }
-  rc = launch_diagcoef_colsum(G, g->V_dst, d, db, st);
+  if (!rc) rc = grad_prologue(dOut, out, drop_mask, keep, relu, (int64_t)g->V_dst * d, G, dS, st);
+  if (!rc) rc = launch_diagcoef_colsum(G, g->V_dst, d, db, st);
   if (rc) return rc;
   MARK("grad_prologue_db");
-  rc = gemm_any(st, split_ws, true, false, d, d, g->V_dst, H, d, dS, d, 0.f, dWself, d);
+  rc = self_loop_backward(g, d, H, dS, Wself, dWself, dH, split_ws, nullptr, st);
   if (rc) return rc;
-  rc = gemm_any(st, split_ws, false, true, g->V_dst, d, d, dS, d, Wself, d, 0.f, dH, d);
-  if (rc) return rc;
-  if (g->V_src > g->V_dst) {
-    rc = rgcn_check_cuda(cudaMemsetAsync(dH + (size_t)g->V_dst * d, 0,
-                                         (size_t)(g->V_src - g->V_dst) * d * sizeof(float), st),
-                         "memset(dH halo)");
-    if (rc) return rc;
-  }
   MARK("diagcoef_self_loop_bwd");
   // dP[u][dir][b][:] = sum_{m from u} norm_m sig[relw_m,b,:] G[dst_m,:]
   rc = launch_zero_rows(dP, 2 * dB, g->by_src.d_split_rows, (int)g->by_src.n_split, st);
@@ -1066,45 +982,27 @@ extern "C" int64_t rgcn_diag_workspace_bytes(const rgcn_graph_t* g, int32_t d, i
   return bytes + 256;
 }
 
-// shape, pointer and workspace checks come first (they need no device), then the graph: device, V_src >= V_dst, CSR
-static int diag_graph_checks(const rgcn_graph_t* g, int32_t d, const char* who) {
-  int rc = layer_checks(g, d, 1, who);
-  if (rc) return rc;
-  return need_views(g, true, false, who);
-}
-
 extern "C" int rgcn_diag_forward(const rgcn_graph_t* g, int32_t d, const float* H, const float* Df, const float* Db,
                                  const float* Wself, const float* b, const uint8_t* drop_mask, float keep, int relu,
                                  float* out, void* workspace, int64_t workspace_bytes, void* stream) {
-  int rc = onehot_shape_checks(g, d, 1, "rgcn_diag_forward");
-  if (rc) return rc;
-  if (!H || !Df || !Db || !Wself || !b || !out || !workspace || keep <= 0.f) {
-    rgcn_set_error("rgcn_diag_forward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_diag_workspace_bytes(g, d, 0)) {
-    rgcn_set_error("rgcn_diag_forward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
-  rc = diag_graph_checks(g, d, "rgcn_diag_forward");
+  const char* who = "rgcn_diag_forward";
+  int rc = shape_checks(g, d, 1, who);
+  if (!rc) rc = pointer_checks(H && Df && Db && Wself && b && out && workspace, keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_diag_workspace_bytes(g, d, 0), who);
+  if (!rc) rc = graph_checks(g, d, 1, who, true, true, false);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
   if (rc) return rc;
-  const int64_t n_split = g->by_dst.n_split;
-  const int slabs = slabs_for(d);
   Carver ws(workspace, workspace_bytes);
   float* split_ws = ws.take<float>((int64_t)2 * d * d);
-  float* scratch = ws.take<float>(n_split * d);
-  int* counters = ws.take<int>(n_split * slabs);
+  float* scratch;
+  int* counters;
   MARK("start");
-  if (n_split > 0) {
-    rc = rgcn_check_cuda(cudaMemsetAsync(scratch, 0, (char*)(counters + n_split * slabs) - (char*)scratch, st),
-                         "memset(scratch)");
-    if (rc) return rc;
-  }
+  rc = split_scratch(ws, g->by_dst.n_split, d, scratch, counters, st);
+  if (rc) return rc;
   // self-loop term H[0:V_dst] W_self written straight into `out`; the walk applies the dropout mask (gcn_diag.py:39-40)
-  rc = gemm_any(st, split_ws, false, false, g->V_dst, d, d, H, d, Wself, d, 0.f, out, d);
+  rc = self_loop_forward(g, d, H, Wself, nullptr, keep, out, split_ws, st);
   if (rc) return rc;
   MARK("gemm_self_loop");
   // out[v] = act(dropout(out[v]) + sum_{m into v} norm_m D[relw_m] (.) H[src_m] + b)   (gcn_diag.py:29-58)
@@ -1119,18 +1017,13 @@ extern "C" int rgcn_diag_backward(const rgcn_graph_t* g, int32_t d, const float*
                                   const float* Wself, const uint8_t* drop_mask, float keep, int relu, const float* out,
                                   const float* dOut, float* dH, float* dDf, float* dDb, float* dWself, float* db,
                                   float* slice_sumsq2, void* workspace, int64_t workspace_bytes, void* stream) {
-  int rc = onehot_shape_checks(g, d, 1, "rgcn_diag_backward");
-  if (rc) return rc;
-  if (!H || !Df || !Db || !Wself || !dOut || !dH || !dDf || !dDb || !dWself || !db || !workspace ||
-      (relu && !out) || keep <= 0.f) {
-    rgcn_set_error("rgcn_diag_backward: null pointer or keep <= 0");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_diag_workspace_bytes(g, d, 1)) {
-    rgcn_set_error("rgcn_diag_backward: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
-  rc = diag_graph_checks(g, d, "rgcn_diag_backward");
+  const char* who = "rgcn_diag_backward";
+  int rc = shape_checks(g, d, 1, who);
+  if (!rc)
+    rc = pointer_checks(
+        H && Df && Db && Wself && dOut && dH && dDf && dDb && dWself && db && workspace && (!relu || out), keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_diag_workspace_bytes(g, d, 1), who);
+  if (!rc) rc = graph_checks(g, d, 1, who, true, true, false);
   if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
@@ -1140,29 +1033,14 @@ extern "C" int rgcn_diag_backward(const rgcn_graph_t* g, int32_t d, const float*
   float* split_ws = ws.take<float>((int64_t)2 * d * d);
   float* G = ws.take<float>((int64_t)g->V_dst * d);
   float* dS = ws.take<float>((int64_t)g->V_dst * d);
-  if (!drop_mask) dS = G;
 
   MARK("start");
-  // G = dOut * relu'(out);  dS = G * mask / keep   (dropout is on the self loop only)
-  if (!relu && !drop_mask) {
-    G = dS = const_cast<float*>(dOut);
-  } else {
-    rc = launch_grad_prologue(dOut, out, drop_mask, 1.0f / keep, relu, (int64_t)g->V_dst * d, G, dS, st);
-    if (rc) return rc;
-  }
-  rc = launch_diagcoef_colsum(G, g->V_dst, d, db, st);
+  rc = grad_prologue(dOut, out, drop_mask, keep, relu, (int64_t)g->V_dst * d, G, dS, st);
+  if (!rc) rc = launch_diagcoef_colsum(G, g->V_dst, d, db, st);
   if (rc) return rc;
   MARK("grad_prologue_db");
-  rc = gemm_any(st, split_ws, true, false, d, d, g->V_dst, H, d, dS, d, 0.f, dWself, d);
+  rc = self_loop_backward(g, d, H, dS, Wself, dWself, dH, split_ws, nullptr, st);
   if (rc) return rc;
-  rc = gemm_any(st, split_ws, false, true, g->V_dst, d, d, dS, d, Wself, d, 0.f, dH, d);
-  if (rc) return rc;
-  if (g->V_src > g->V_dst) {
-    rc = rgcn_check_cuda(cudaMemsetAsync(dH + (size_t)g->V_dst * d, 0,
-                                         (size_t)(g->V_src - g->V_dst) * d * sizeof(float), st),
-                         "memset(dH halo)");
-    if (rc) return rc;
-  }
   MARK("diag_self_loop_bwd");
   // dH[u] += sum_{m from u} norm_m D[relw_m] (.) G[dst_m];  dD[w] = sum_{m: relw_m = w} norm_m H[src_m] (.) G[dst_m]
   rc = rgcn_check_cuda(cudaMemsetAsync(dDf, 0, (size_t)R * d * 4, st), "memset(dDf)");
@@ -1429,18 +1307,13 @@ extern "C" int64_t rgcn_block_slice_sumsq_workspace_bytes(const rgcn_graph_t* g,
 
 extern "C" int rgcn_block_slice_sumsq(const rgcn_graph_t* g, int32_t d, int32_t B, const float* H, const float* G,
                                       float* sumsq2, void* workspace, int64_t workspace_bytes, void* stream) {
-  int rc = common_checks(g, d, B, "rgcn_block_slice_sumsq");
+  const char* who = "rgcn_block_slice_sumsq";
+  int rc = graph_checks(g, d, B, who, false, false, false);
+  if (!rc) rc = block_size_checks(d, B, who);
+  if (!rc) rc = pointer_checks(H && G && sumsq2 && workspace, 1.f, who);
+  if (!rc) rc = need_views(g, false, true, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_block_slice_sumsq_workspace_bytes(g, d, B), who);
   if (rc) return rc;
-  if (d % B != 0 || !H || !G || !sumsq2 || !workspace) {
-    rgcn_set_error("rgcn_block_slice_sumsq: bad arguments");
-    return RGCN_ERR_INVALID;
-  }
-  rc = need_views(g, false, true, "rgcn_block_slice_sumsq");
-  if (rc) return rc;
-  if (workspace_bytes < rgcn_block_slice_sumsq_workspace_bytes(g, d, B)) {
-    rgcn_set_error("rgcn_block_slice_sumsq: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
   cudaStream_t st = (cudaStream_t)stream;
   rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
   if (rc) return rc;
@@ -1460,32 +1333,51 @@ extern "C" int rgcn_block_slice_sumsq(const rgcn_graph_t* g, int32_t d, int32_t 
 // ------------------------------------------------------------------------------------------------
 // DistMult all-entity scoring + ranking, fused (next row N3)
 // ------------------------------------------------------------------------------------------------
-// The decoder-independent body of distmult_rank / rgcn_complex_rank: hi/lo split of `codes` (unless reused), the
-// decoder's query rows + gold scores, the scoring GEMM with its rank-counting epilogue, raw/filtered ranks.
-// Workspace layout: [hi V*d | lo V*d | Q n*d | gold_sig n | gold_col n | raw_cnt n | known_cnt n].
+// The decoder-independent body of the rank entry points (entity and relation queries, DistMult and ComplEx): the
+// argument checks, the hi/lo split of the candidate rows (unless reused), the decoder's query rows + gold scores, the
+// scoring GEMM with its rank-counting epilogue, raw/filtered ranks.  The candidates are the first N rows of `table`:
+// the codes (N = V) for entity queries, the relation table (N = R) for relation queries.
+// Workspace layout: [hi N*d | lo N*d | Q n*d | gold_sig n | gold_col n | raw_cnt n | known_cnt n].
 typedef int (*RankPrepareFn)(const float*, const float*, int, const int32_t*, int64_t, int, float*, float*, int32_t*,
                              cudaStream_t);
+typedef int64_t (*RankWorkspaceFn)(int32_t, int32_t, int64_t);
 
-static int rank_with_queries(RankPrepareFn prepare, const float* codes, const float* rel, int32_t V, int32_t d,
-                             const int32_t* X, int64_t n, int side, const uint32_t* known_mask, int reuse_split,
-                             int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
-                             cudaStream_t st) {
+static int rank_with_queries(const char* who, RankPrepareFn prepare, const float* table, int32_t N,
+                             RankWorkspaceFn workspace_fn, const float* codes, const float* rel, int32_t V,
+                             int32_t Vrel, int32_t d, const int32_t* X, int64_t n, int side,
+                             const uint32_t* known_mask, int reuse_split, int32_t* raw_rank, int32_t* filtered_rank,
+                             void* workspace, int64_t workspace_bytes, cudaStream_t st) {
+  if (!codes || !rel || (n > 0 && (!X || !raw_rank)) || !workspace || V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 ||
+      n < 0 || n > 0x7fffffffLL || (side != 0 && side != 1)) {
+    rgcn_set_error(std::string(who) + ": bad arguments (need non-null pointers, d % 4 == 0, side in {0,1})");
+    return RGCN_ERR_INVALID;
+  }
+  if (filtered_rank && !known_mask) {
+    rgcn_set_error(std::string(who) + ": bad arguments (filtered ranks need a known mask)");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t need = workspace_fn(N, d, n);
+  if (need < 0) return (int)need;
+  if (workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
   Carver ws(workspace, workspace_bytes);
-  float* hi = ws.take<float>((int64_t)V * d);
-  float* lo = ws.take<float>((int64_t)V * d);
+  float* hi = ws.take<float>((int64_t)N * d);
+  float* lo = ws.take<float>((int64_t)N * d);
   float* Q = ws.take<float>(n * d);
   float* gold_sig = ws.take<float>(n);
   int32_t* gold_col = ws.take<int32_t>(n);
   int32_t* raw_cnt = ws.take<int32_t>(n);
   int32_t* known_cnt = ws.take<int32_t>(n);
   int rc = RGCN_OK;
-  if (!reuse_split) rc = launch_gemm_split_b(codes, d, V, d, /*transposed=*/0, hi, lo, st);
+  if (!reuse_split) rc = launch_gemm_split_b(table, d, N, d, /*transposed=*/0, hi, lo, st);
   if (rc || n == 0) return rc;
   rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
   if (rc) return rc;
   rc = prepare(codes, rel, d, X, n, side, Q, gold_sig, gold_col, st);
   if (rc) return rc;
-  rc = launch_gemm_rank_tf32x3(Q, d, hi, lo, d, (int)n, V, d, gold_sig, gold_col, known_mask, (V + 31) / 32, raw_cnt,
+  rc = launch_gemm_rank_tf32x3(Q, d, hi, lo, d, (int)n, N, d, gold_sig, gold_col, known_mask, (N + 31) / 32, raw_cnt,
                                known_cnt, st);
   if (rc) return rc;
   return launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
@@ -1503,17 +1395,9 @@ extern "C" int distmult_rank(const float* codes, const float* rel, int32_t V, in
                              const int32_t* X, int64_t n, int side, const uint32_t* known_mask, int reuse_split,
                              int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
                              void* stream) {
-  if (!codes || !rel || (n > 0 && (!X || !raw_rank)) || !workspace || V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 ||
-      n < 0 || n > 0x7fffffffLL || (side != 0 && side != 1) || (filtered_rank && !known_mask)) {
-    rgcn_set_error("distmult_rank: bad arguments (need d % 4 == 0, side in {0,1}, a known mask when filtered ranks are requested)");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < distmult_rank_workspace_bytes(V, d, n)) {
-    rgcn_set_error("distmult_rank: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
-  return rank_with_queries(launch_distmult_rank_prepare, codes, rel, V, d, X, n, side, known_mask, reuse_split,
-                           raw_rank, filtered_rank, workspace, workspace_bytes, (cudaStream_t)stream);
+  return rank_with_queries("distmult_rank", launch_distmult_rank_prepare, codes, V, distmult_rank_workspace_bytes, codes,
+                           rel, V, Vrel, d, X, n, side, known_mask, reuse_split, raw_rank, filtered_rank, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1555,18 +1439,9 @@ extern "C" int rgcn_complex_rank(const float* codes, const float* rel, int32_t V
                                  const int32_t* X, int64_t n, int side, const uint32_t* known_mask, int reuse_split,
                                  int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
                                  void* stream) {
-  if (!codes || !rel || (n > 0 && (!X || !raw_rank)) || !workspace || V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 ||
-      n < 0 || n > 0x7fffffffLL || (side != 0 && side != 1) || (filtered_rank && !known_mask)) {
-    rgcn_set_error("rgcn_complex_rank: bad arguments (need d % 4 == 0, side in {0,1}, a known mask when filtered "
-                   "ranks are requested)");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_complex_rank_workspace_bytes(V, d, n)) {
-    rgcn_set_error("rgcn_complex_rank: workspace too small");
-    return RGCN_ERR_WORKSPACE;
-  }
-  return rank_with_queries(launch_complex_rank_prepare, codes, rel, V, d, X, n, side, known_mask, reuse_split,
-                           raw_rank, filtered_rank, workspace, workspace_bytes, (cudaStream_t)stream);
+  return rank_with_queries("rgcn_complex_rank", launch_complex_rank_prepare, codes, V, rgcn_complex_rank_workspace_bytes,
+                           codes, rel, V, Vrel, d, X, n, side, known_mask, reuse_split, raw_rank, filtered_rank,
+                           workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1681,7 +1556,11 @@ extern "C" int64_t rgcn_topk_workspace_bytes(int32_t V, int32_t d, int64_t n, in
   return 2 * align_up((int64_t)V * d * 4) + align_up(n * d * 4) + align_up(n * tn * k * 8) + 256;
 }
 
-static int topk_with_queries(RankPrepareFn prepare, const char* who, const float* codes, const float* rel, int32_t V,
+// The candidates are the first N rows of `table`, as in rank_with_queries.
+typedef int64_t (*TopkWorkspaceFn)(int32_t, int32_t, int64_t, int32_t);
+
+static int topk_with_queries(const char* who, RankPrepareFn prepare, const float* table, int32_t N,
+                             TopkWorkspaceFn workspace_fn, const float* codes, const float* rel, int32_t V,
                              int32_t Vrel, int32_t d, const int32_t* X, int64_t n, int side, int32_t k,
                              const uint32_t* exclude_mask, int reuse_split, int32_t* ids, float* energies,
                              void* workspace, int64_t workspace_bytes, cudaStream_t st) {
@@ -1694,24 +1573,24 @@ static int topk_with_queries(RankPrepareFn prepare, const char* who, const float
     rgcn_set_error(std::string(who) + ": k = " + std::to_string(k) + " is out of range (1 <= k <= 128)");
     return RGCN_ERR_INVALID;
   }
-  const int64_t need = rgcn_topk_workspace_bytes(V, d, n, k);
+  const int64_t need = workspace_fn(N, d, n, k);
   if (need < 0) return (int)need;
   if (workspace_bytes < need) {
-    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_topk_workspace_bytes)");
+    rgcn_set_error(std::string(who) + ": workspace too small");
     return RGCN_ERR_WORKSPACE;
   }
-  const int tn = (V + 127) / 128;
+  const int tn = (N + 127) / 128;
   Carver ws(workspace, workspace_bytes);
-  float* hi = ws.take<float>((int64_t)V * d);
-  float* lo = ws.take<float>((int64_t)V * d);
+  float* hi = ws.take<float>((int64_t)N * d);
+  float* lo = ws.take<float>((int64_t)N * d);
   float* Q = ws.take<float>(n * d);
   uint2* cand = ws.take<uint2>(n * tn * k);
   int rc = RGCN_OK;
-  if (!reuse_split) rc = launch_gemm_split_b(codes, d, V, d, /*transposed=*/0, hi, lo, st);
+  if (!reuse_split) rc = launch_gemm_split_b(table, d, N, d, /*transposed=*/0, hi, lo, st);
   if (rc || n == 0) return rc;
   rc = prepare(codes, rel, d, X, n, side, Q, nullptr, nullptr, st);
   if (rc) return rc;
-  rc = launch_gemm_topk_tf32x3(Q, d, hi, lo, d, (int)n, V, d, exclude_mask, (V + 31) / 32, k, cand, st);
+  rc = launch_gemm_topk_tf32x3(Q, d, hi, lo, d, (int)n, N, d, exclude_mask, (N + 31) / 32, k, cand, st);
   if (rc) return rc;
   return launch_topk_merge(cand, n, tn * k, k, ids, energies, st);
 }
@@ -1720,16 +1599,18 @@ extern "C" int distmult_topk(const float* codes, const float* rel, int32_t V, in
                              const int32_t* X, int64_t n, int side, int32_t k, const uint32_t* exclude_mask,
                              int reuse_split, int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes,
                              void* stream) {
-  return topk_with_queries(launch_distmult_rank_prepare, "distmult_topk", codes, rel, V, Vrel, d, X, n, side, k,
-                           exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+  return topk_with_queries("distmult_topk", launch_distmult_rank_prepare, codes, V, rgcn_topk_workspace_bytes, codes,
+                           rel, V, Vrel, d, X, n, side, k, exclude_mask, reuse_split, ids, energies, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int rgcn_complex_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
                                  const int32_t* X, int64_t n, int side, int32_t k, const uint32_t* exclude_mask,
                                  int reuse_split, int32_t* ids, float* energies, void* workspace,
                                  int64_t workspace_bytes, void* stream) {
-  return topk_with_queries(launch_complex_rank_prepare, "rgcn_complex_topk", codes, rel, V, Vrel, d, X, n, side, k,
-                           exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+  return topk_with_queries("rgcn_complex_topk", launch_complex_rank_prepare, codes, V, rgcn_topk_workspace_bytes, codes,
+                           rel, V, Vrel, d, X, n, side, k, exclude_mask, reuse_split, ids, energies, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1739,11 +1620,19 @@ extern "C" int rgcn_complex_topk(const float* codes, const float* rel, int32_t V
 // prepare kernel) and the energies of all relations are Q @ rel[0:R]^T: the entity-side scoring GEMM with its rank or
 // top-k epilogue, run with Bt = the hi/lo split of the first R relation rows and N = R.  Rows R..Vrel-1 of `rel` (the
 // R-GCN encoders keep a [V, d] relation table) are never split, scored, counted or returned.
-// Workspace layouts: rank [hi R*d | lo R*d | Q n*d | gold_sig n | gold_col n | raw_cnt n | known_cnt n] (that of
-// rank_with_queries with V = R), top-k [hi R*d | lo R*d | Q n*d | cand n*ceil(R/128)*k] (that of topk_with_queries);
-// one relation workspace with its split serves both, never the entity split.
-typedef int (*RelationPrepareFn)(const float*, const float*, int, const int32_t*, int64_t, float*, float*, int32_t*,
-                                 cudaStream_t);
+// The entry points are rank_with_queries / topk_with_queries with the candidates rel[0:R] (N = R); one relation
+// workspace with its split serves both, never the entity split.
+
+// The relation prepare kernels in the RankPrepareFn shape: a pair query has no corruption side.
+static int distmult_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int,
+                                     float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st) {
+  return launch_distmult_relation_prepare(codes, rel, d, X, n, Q, gold_sig, gold_col, st);
+}
+
+static int complex_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int,
+                                    float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st) {
+  return launch_complex_relation_prepare(codes, rel, d, X, n, Q, gold_sig, gold_col, st);
+}
 
 static bool relation_sizes_ok(int32_t R, int32_t d, int64_t n, int64_t per_row) {
   return R > 0 && d > 0 && d % 4 == 0 && n >= 0 && (n == 0 || per_row <= ((int64_t)1 << 60) / n);
@@ -1767,15 +1656,8 @@ extern "C" int64_t rgcn_relation_topk_workspace_bytes(int32_t R, int32_t d, int6
   return rgcn_topk_workspace_bytes(R, d, n, k);
 }
 
-// the argument checks shared by the four relation entry points (before any device work)
-static bool relation_args_ok(const char* who, const float* codes, const float* rel, int32_t V, int32_t Vrel,
-                             int32_t R, int32_t d, const int32_t* X, int64_t n, const void* out1, const void* out2,
-                             const void* workspace) {
-  if (!codes || !rel || (n > 0 && (!X || !out1 || !out2)) || !workspace || V <= 0 || d <= 0 || d % 4 != 0 || n < 0 ||
-      n > 0x7fffffffLL) {
-    rgcn_set_error(std::string(who) + ": bad arguments (need non-null pointers, V > 0, d % 4 == 0)");
-    return false;
-  }
+// the candidates are rel[0:R], which must be rows of the table
+static bool relation_count_ok(const char* who, int32_t R, int32_t Vrel) {
   if (R < 1 || R > Vrel) {
     rgcn_set_error(std::string(who) + ": R = " + std::to_string(R) + " relations, need 1 <= R <= Vrel = " +
                    std::to_string(Vrel));
@@ -1784,103 +1666,46 @@ static bool relation_args_ok(const char* who, const float* codes, const float* r
   return true;
 }
 
-static int relation_rank(RelationPrepareFn prepare, const char* who, const float* codes, const float* rel, int32_t V,
-                         int32_t Vrel, int32_t R, int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
-                         int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
-                         int64_t workspace_bytes, cudaStream_t st) {
-  if (!relation_args_ok(who, codes, rel, V, Vrel, R, d, X, n, raw_rank, raw_rank, workspace)) return RGCN_ERR_INVALID;
-  if (filtered_rank && !known_mask) {
-    rgcn_set_error(std::string(who) + ": bad arguments (filtered ranks need a known mask)");
-    return RGCN_ERR_INVALID;
-  }
-  const int64_t need = rgcn_relation_rank_workspace_bytes(R, d, n);
-  if (need < 0) return (int)need;
-  if (workspace_bytes < need) {
-    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_relation_rank_workspace_bytes)");
-    return RGCN_ERR_WORKSPACE;
-  }
-  Carver ws(workspace, workspace_bytes);
-  float* hi = ws.take<float>((int64_t)R * d);
-  float* lo = ws.take<float>((int64_t)R * d);
-  float* Q = ws.take<float>(n * d);
-  float* gold_sig = ws.take<float>(n);
-  int32_t* gold_col = ws.take<int32_t>(n);
-  int32_t* raw_cnt = ws.take<int32_t>(n);
-  int32_t* known_cnt = ws.take<int32_t>(n);
-  int rc = RGCN_OK;
-  if (!reuse_split) rc = launch_gemm_split_b(rel, d, R, d, /*transposed=*/0, hi, lo, st);
-  if (rc || n == 0) return rc;
-  rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
-  if (rc) return rc;
-  rc = prepare(codes, rel, d, X, n, Q, gold_sig, gold_col, st);
-  if (rc) return rc;
-  rc = launch_gemm_rank_tf32x3(Q, d, hi, lo, d, (int)n, R, d, gold_sig, gold_col, known_mask, (R + 31) / 32, raw_cnt,
-                               known_cnt, st);
-  if (rc) return rc;
-  return launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
-}
-
-static int relation_topk(RelationPrepareFn prepare, const char* who, const float* codes, const float* rel, int32_t V,
-                         int32_t Vrel, int32_t R, int32_t d, const int32_t* X, int64_t n, int32_t k,
-                         const uint32_t* exclude_mask, int reuse_split, int32_t* ids, float* energies, void* workspace,
-                         int64_t workspace_bytes, cudaStream_t st) {
-  if (!relation_args_ok(who, codes, rel, V, Vrel, R, d, X, n, ids, energies, workspace)) return RGCN_ERR_INVALID;
-  if (k < 1 || k > 128) {
-    rgcn_set_error(std::string(who) + ": k = " + std::to_string(k) + " is out of range (1 <= k <= 128)");
-    return RGCN_ERR_INVALID;
-  }
-  const int64_t need = rgcn_relation_topk_workspace_bytes(R, d, n, k);
-  if (need < 0) return (int)need;
-  if (workspace_bytes < need) {
-    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_relation_topk_workspace_bytes)");
-    return RGCN_ERR_WORKSPACE;
-  }
-  const int tn = (R + 127) / 128;
-  Carver ws(workspace, workspace_bytes);
-  float* hi = ws.take<float>((int64_t)R * d);
-  float* lo = ws.take<float>((int64_t)R * d);
-  float* Q = ws.take<float>(n * d);
-  uint2* cand = ws.take<uint2>(n * tn * k);
-  int rc = RGCN_OK;
-  if (!reuse_split) rc = launch_gemm_split_b(rel, d, R, d, /*transposed=*/0, hi, lo, st);
-  if (rc || n == 0) return rc;
-  rc = prepare(codes, rel, d, X, n, Q, nullptr, nullptr, st);
-  if (rc) return rc;
-  rc = launch_gemm_topk_tf32x3(Q, d, hi, lo, d, (int)n, R, d, exclude_mask, (R + 31) / 32, k, cand, st);
-  if (rc) return rc;
-  return launch_topk_merge(cand, n, tn * k, k, ids, energies, st);
-}
-
 extern "C" int distmult_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
                                       int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
                                       int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
                                       int64_t workspace_bytes, void* stream) {
-  return relation_rank(launch_distmult_relation_prepare, "distmult_relation_rank", codes, rel, V, Vrel, R, d, X, n,
-                       known_mask, reuse_split, raw_rank, filtered_rank, workspace, workspace_bytes,
-                       (cudaStream_t)stream);
+  const char* who = "distmult_relation_rank";
+  if (!relation_count_ok(who, R, Vrel)) return RGCN_ERR_INVALID;
+  return rank_with_queries(who, distmult_relation_prepare, rel, R, rgcn_relation_rank_workspace_bytes, codes, rel, V,
+                           Vrel, d, X, n, 0, known_mask, reuse_split, raw_rank, filtered_rank, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int rgcn_complex_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
                                           int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
                                           int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
                                           int64_t workspace_bytes, void* stream) {
-  return relation_rank(launch_complex_relation_prepare, "rgcn_complex_relation_rank", codes, rel, V, Vrel, R, d, X, n,
-                       known_mask, reuse_split, raw_rank, filtered_rank, workspace, workspace_bytes,
-                       (cudaStream_t)stream);
+  const char* who = "rgcn_complex_relation_rank";
+  if (!relation_count_ok(who, R, Vrel)) return RGCN_ERR_INVALID;
+  return rank_with_queries(who, complex_relation_prepare, rel, R, rgcn_relation_rank_workspace_bytes, codes, rel, V,
+                           Vrel, d, X, n, 0, known_mask, reuse_split, raw_rank, filtered_rank, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int distmult_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
                                       int32_t d, const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask,
                                       int reuse_split, int32_t* ids, float* energies, void* workspace,
                                       int64_t workspace_bytes, void* stream) {
-  return relation_topk(launch_distmult_relation_prepare, "distmult_relation_topk", codes, rel, V, Vrel, R, d, X, n, k,
-                       exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+  const char* who = "distmult_relation_topk";
+  if (!relation_count_ok(who, R, Vrel)) return RGCN_ERR_INVALID;
+  return topk_with_queries(who, distmult_relation_prepare, rel, R, rgcn_relation_topk_workspace_bytes, codes, rel, V,
+                           Vrel, d, X, n, 0, k, exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes,
+                           (cudaStream_t)stream);
 }
 
 extern "C" int rgcn_complex_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
                                           int32_t d, const int32_t* X, int64_t n, int32_t k,
                                           const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
                                           float* energies, void* workspace, int64_t workspace_bytes, void* stream) {
-  return relation_topk(launch_complex_relation_prepare, "rgcn_complex_relation_topk", codes, rel, V, Vrel, R, d, X, n,
-                       k, exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+  const char* who = "rgcn_complex_relation_topk";
+  if (!relation_count_ok(who, R, Vrel)) return RGCN_ERR_INVALID;
+  return topk_with_queries(who, complex_relation_prepare, rel, R, rgcn_relation_topk_workspace_bytes, codes, rel, V,
+                           Vrel, d, X, n, 0, k, exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes,
+                           (cudaStream_t)stream);
 }

@@ -182,6 +182,17 @@ def _workspace(nbytes, device):
     return torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=device)
 
 
+def _call(entry, workspace_fn, workspace_args, args, device):
+    """lib.entry(*args, workspace, workspace_bytes, stream) with a workspace of lib.workspace_fn(*workspace_args) bytes
+    on `device` and its current stream; a negative size or a non-zero return code raises RgcnError."""
+    lib = _lib.load()
+    nb = getattr(lib, workspace_fn)(*workspace_args)
+    if nb < 0:
+        _lib.check(int(nb), workspace_fn)
+    ws = _workspace(nb, device)
+    _lib.check(getattr(lib, entry)(*args, _ptr(ws), ws.numel(), _stream(device)), entry)
+
+
 def _mask_arg(mask, V, d):
     if mask is None:
         return None
@@ -194,7 +205,6 @@ def _mask_arg(mask, V, d):
 class _BlockLayerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, H, Wf, Wb, Wself, graph, n_blocks, drop_mask, keep, relu):
-        lib = _lib.load()
         d = H.shape[1]
         R = graph.n_relw // 2
         s = d // n_blocks
@@ -205,14 +215,9 @@ class _BlockLayerFn(torch.autograd.Function):
         mask = _mask_arg(drop_mask, graph.V_dst, d)
         dev = H.device
         out = torch.empty(graph.V_dst, d, dtype=torch.float32, device=dev)
-        nb = lib.rgcn_block_workspace_bytes(graph.handle, d, n_blocks, 0)
-        if nb < 0:
-            _lib.check(int(nb), "rgcn_block_workspace_bytes")
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_block_forward(graph.handle, d, n_blocks, _ptr(H), _ptr(Wf), _ptr(Wb),
-                                    _ptr(Wself), _ptr(mask), float(keep), int(bool(relu)), _ptr(out),
-                                    _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_block_forward")
+        _call("rgcn_block_forward", "rgcn_block_workspace_bytes", (graph.handle, d, n_blocks, 0),
+              (graph.handle, d, n_blocks, _ptr(H), _ptr(Wf), _ptr(Wb), _ptr(Wself), _ptr(mask), float(keep),
+               int(bool(relu)), _ptr(out)), dev)
         ctx.graph, ctx.n_blocks, ctx.keep, ctx.relu = graph, n_blocks, float(keep), bool(relu)
         ctx.mask = mask
         ctx.params = (Wf, Wb)   # the caller's tensor objects (slice norms are parked on them)
@@ -221,7 +226,6 @@ class _BlockLayerFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dOut):
-        lib = _lib.load()
         H, Wf, Wb, Wself, out = ctx.saved_tensors
         graph, B = ctx.graph, ctx.n_blocks
         d = H.shape[1]
@@ -230,21 +234,14 @@ class _BlockLayerFn(torch.autograd.Function):
         dev = H.device
         dH = torch.empty_like(H)
         dWf, dWb, dWself = torch.empty_like(Wf), torch.empty_like(Wb), torch.empty_like(Wself)
-        nb = lib.rgcn_block_workspace_bytes(graph.handle, d, B, 1)
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_block_backward(graph.handle, d, B, _ptr(H), _ptr(Wf), _ptr(Wb), _ptr(Wself),
-                                     _ptr(ctx.mask), ctx.keep, int(ctx.relu), _ptr(out), _ptr(dOut),
-                                     _ptr(dH), _ptr(dWf), _ptr(dWb), _ptr(dWself), _ptr(ws),
-                                     ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_block_backward")
+        _call("rgcn_block_backward", "rgcn_block_workspace_bytes", (graph.handle, d, B, 1),
+              (graph.handle, d, B, _ptr(H), _ptr(Wf), _ptr(Wb), _ptr(Wself), _ptr(ctx.mask), ctx.keep, int(ctx.relu),
+               _ptr(out), _ptr(dOut), _ptr(dH), _ptr(dWf), _ptr(dWb), _ptr(dWself)), dev)
         if _SLICE_NORMS:
-            G = (dOut * (out > 0)) if ctx.relu else dOut
-            nb2 = lib.rgcn_block_slice_sumsq_workspace_bytes(graph.handle, d, B)
-            ws2 = _workspace(nb2, dev)
+            G = ((dOut * (out > 0)) if ctx.relu else dOut).contiguous()
             ss = torch.empty(2, dtype=torch.float32, device=dev)
-            rc = lib.rgcn_block_slice_sumsq(graph.handle, d, B, _ptr(H), _ptr(G.contiguous()), _ptr(ss), _ptr(ws2),
-                                            ws2.numel(), _stream(dev))
-            _lib.check(rc, "rgcn_block_slice_sumsq")
+            _call("rgcn_block_slice_sumsq", "rgcn_block_slice_sumsq_workspace_bytes", (graph.handle, d, B),
+                  (graph.handle, d, B, _ptr(H), _ptr(G), _ptr(ss)), dev)
             _add_slice_sumsq(ctx.params[0], ss[0])
             _add_slice_sumsq(ctx.params[1], ss[1])
         return dH, dWf, dWb, dWself, None, None, None, None, None
@@ -260,7 +257,6 @@ def block_layer(H, W_forward, W_backward, W_self, graph, n_blocks, drop_mask=Non
 class _BasisLayerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, H, Vf, Vb, Cf, Cb, Wself, graph, drop_mask, keep, relu):
-        lib = _lib.load()
         d = H.shape[1]
         R = graph.n_relw // 2
         B = Cf.shape[1]
@@ -274,21 +270,15 @@ class _BasisLayerFn(torch.autograd.Function):
         dev = H.device
         out = torch.empty(graph.V_dst, d, dtype=torch.float32, device=dev)
         saved = torch.empty(graph.V_dst, 2 * d * B, dtype=torch.float32, device=dev)
-        nb = lib.rgcn_basis_workspace_bytes(graph.handle, d, B, 0)
-        if nb < 0:
-            _lib.check(int(nb), "rgcn_basis_workspace_bytes")
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_basis_forward(graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf),
-                                    _ptr(Cb), _ptr(Wself), _ptr(mask), float(keep), int(bool(relu)),
-                                    _ptr(out), _ptr(saved), _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_basis_forward")
+        _call("rgcn_basis_forward", "rgcn_basis_workspace_bytes", (graph.handle, d, B, 0),
+              (graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf), _ptr(Cb), _ptr(Wself), _ptr(mask),
+               float(keep), int(bool(relu)), _ptr(out), _ptr(saved)), dev)
         ctx.graph, ctx.keep, ctx.relu, ctx.mask = graph, float(keep), bool(relu), mask
         ctx.save_for_backward(H, Vf, Vb, Cf, Cb, Wself, out, saved)
         return out
 
     @staticmethod
     def backward(ctx, dOut):
-        lib = _lib.load()
         H, Vf, Vb, Cf, Cb, Wself, out, saved = ctx.saved_tensors
         graph = ctx.graph
         d, B = H.shape[1], Cf.shape[1]
@@ -297,14 +287,10 @@ class _BasisLayerFn(torch.autograd.Function):
         dH = torch.empty_like(H)
         dVf, dVb = torch.empty_like(Vf), torch.empty_like(Vb)
         dCf, dCb, dWself = torch.empty_like(Cf), torch.empty_like(Cb), torch.empty_like(Wself)
-        nb = lib.rgcn_basis_workspace_bytes(graph.handle, d, B, 1)
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_basis_backward(graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf),
-                                     _ptr(Cb), _ptr(Wself), _ptr(ctx.mask), ctx.keep, int(ctx.relu),
-                                     _ptr(out), _ptr(saved), _ptr(dOut), _ptr(dH), _ptr(dVf),
-                                     _ptr(dVb), _ptr(dCf), _ptr(dCb), _ptr(dWself), _ptr(ws),
-                                     ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_basis_backward")
+        _call("rgcn_basis_backward", "rgcn_basis_workspace_bytes", (graph.handle, d, B, 1),
+              (graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf), _ptr(Cb), _ptr(Wself), _ptr(ctx.mask),
+               ctx.keep, int(ctx.relu), _ptr(out), _ptr(saved), _ptr(dOut), _ptr(dH), _ptr(dVf), _ptr(dVb), _ptr(dCf),
+               _ptr(dCb), _ptr(dWself)), dev)
         return dH, dVf, dVb, dCf, dCb, dWself, None, None, None, None
 
 
@@ -318,7 +304,6 @@ def basis_layer(H, W_forward, W_backward, C_forward, C_backward, W_self, graph, 
 class _BasisOnehotLayerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, Wf, Wb, Cf, Cb, Wself, graph, drop_mask, keep, relu):
-        lib = _lib.load()
         if not (isinstance(Wf, torch.Tensor) and Wf.dim() == 3):
             raise _lib.RgcnError("W_forward must be a [V, B, d] tensor")
         _, B, d = Wf.shape
@@ -331,21 +316,15 @@ class _BasisOnehotLayerFn(torch.autograd.Function):
         mask = _mask_arg(drop_mask, graph.V_dst, d)
         dev = Wf.device
         out = torch.empty(graph.V_dst, d, dtype=torch.float32, device=dev)
-        nb = lib.rgcn_basis_onehot_workspace_bytes(graph.handle, d, B, 0)
-        if nb < 0:
-            _lib.check(int(nb), "rgcn_basis_onehot_workspace_bytes")
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_basis_onehot_forward(graph.handle, d, B, _ptr(Wf), _ptr(Wb), _ptr(Cf), _ptr(Cb), _ptr(Wself),
-                                           _ptr(mask), float(keep), int(bool(relu)), _ptr(out), _ptr(ws),
-                                           ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_basis_onehot_forward")
+        _call("rgcn_basis_onehot_forward", "rgcn_basis_onehot_workspace_bytes", (graph.handle, d, B, 0),
+              (graph.handle, d, B, _ptr(Wf), _ptr(Wb), _ptr(Cf), _ptr(Cb), _ptr(Wself), _ptr(mask), float(keep),
+               int(bool(relu)), _ptr(out)), dev)
         ctx.graph, ctx.keep, ctx.relu, ctx.mask = graph, float(keep), bool(relu), mask
         ctx.save_for_backward(Wf, Wb, Cf, Cb, Wself, out)
         return out
 
     @staticmethod
     def backward(ctx, dOut):
-        lib = _lib.load()
         Wf, Wb, Cf, Cb, Wself, out = ctx.saved_tensors
         graph = ctx.graph
         B, d = Wf.shape[1], Wf.shape[2]
@@ -354,13 +333,9 @@ class _BasisOnehotLayerFn(torch.autograd.Function):
         dev = Wf.device
         dWf, dWb = torch.empty_like(Wf), torch.empty_like(Wb)
         dCf, dCb, dWself = torch.empty_like(Cf), torch.empty_like(Cb), torch.empty_like(Wself)
-        nb = lib.rgcn_basis_onehot_workspace_bytes(graph.handle, d, B, 1)
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_basis_onehot_backward(graph.handle, d, B, _ptr(Wf), _ptr(Wb), _ptr(Cf), _ptr(Cb),
-                                            _ptr(ctx.mask), ctx.keep, int(ctx.relu), _ptr(out), _ptr(dOut),
-                                            _ptr(dWf), _ptr(dWb), _ptr(dCf), _ptr(dCb), _ptr(dWself), _ptr(ws),
-                                            ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_basis_onehot_backward")
+        _call("rgcn_basis_onehot_backward", "rgcn_basis_onehot_workspace_bytes", (graph.handle, d, B, 1),
+              (graph.handle, d, B, _ptr(Wf), _ptr(Wb), _ptr(Cf), _ptr(Cb), _ptr(ctx.mask), ctx.keep, int(ctx.relu),
+               _ptr(out), _ptr(dOut), _ptr(dWf), _ptr(dWb), _ptr(dCf), _ptr(dCb), _ptr(dWself)), dev)
         return dWf, dWb, dCf, dCb, dWself, None, None, None, None
 
 
@@ -376,7 +351,6 @@ def basis_onehot_layer(W_forward, W_backward, C_forward, C_backward, W_self, gra
 class _BasisDiagcoefLayerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, H, Vf, Vb, Cf, Cb, Wself, b, graph, drop_mask, keep, relu):
-        lib = _lib.load()
         if not (isinstance(Cf, torch.Tensor) and Cf.dim() == 3):
             raise _lib.RgcnError("C_forward must be a [R, B, d] tensor")
         d = H.shape[1]
@@ -393,21 +367,15 @@ class _BasisDiagcoefLayerFn(torch.autograd.Function):
         dev = H.device
         out = torch.empty(graph.V_dst, d, dtype=torch.float32, device=dev)
         saved = torch.empty(graph.V_src, 2 * B * d, dtype=torch.float32, device=dev)
-        nb = lib.rgcn_basis_diagcoef_workspace_bytes(graph.handle, d, B, 0)
-        if nb < 0:
-            _lib.check(int(nb), "rgcn_basis_diagcoef_workspace_bytes")
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_basis_diagcoef_forward(graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf), _ptr(Cb),
-                                             _ptr(Wself), _ptr(b), _ptr(mask), float(keep), int(bool(relu)), _ptr(out),
-                                             _ptr(saved), _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_basis_diagcoef_forward")
+        _call("rgcn_basis_diagcoef_forward", "rgcn_basis_diagcoef_workspace_bytes", (graph.handle, d, B, 0),
+              (graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf), _ptr(Cb), _ptr(Wself), _ptr(b), _ptr(mask),
+               float(keep), int(bool(relu)), _ptr(out), _ptr(saved)), dev)
         ctx.graph, ctx.keep, ctx.relu, ctx.mask = graph, float(keep), bool(relu), mask
         ctx.save_for_backward(H, Vf, Vb, Cf, Cb, Wself, out, saved)
         return out
 
     @staticmethod
     def backward(ctx, dOut):
-        lib = _lib.load()
         H, Vf, Vb, Cf, Cb, Wself, out, saved = ctx.saved_tensors
         graph = ctx.graph
         d, B = H.shape[1], Cf.shape[1]
@@ -418,13 +386,10 @@ class _BasisDiagcoefLayerFn(torch.autograd.Function):
         dVf, dVb = torch.empty_like(Vf), torch.empty_like(Vb)
         dCf, dCb, dWself = torch.empty_like(Cf), torch.empty_like(Cb), torch.empty_like(Wself)
         db = torch.empty(d, dtype=torch.float32, device=dev)
-        nb = lib.rgcn_basis_diagcoef_workspace_bytes(graph.handle, d, B, 1)
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_basis_diagcoef_backward(graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf), _ptr(Cb),
-                                              _ptr(Wself), _ptr(ctx.mask), ctx.keep, int(ctx.relu), _ptr(out),
-                                              _ptr(saved), _ptr(dOut), _ptr(dH), _ptr(dVf), _ptr(dVb), _ptr(dCf),
-                                              _ptr(dCb), _ptr(dWself), _ptr(db), _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_basis_diagcoef_backward")
+        _call("rgcn_basis_diagcoef_backward", "rgcn_basis_diagcoef_workspace_bytes", (graph.handle, d, B, 1),
+              (graph.handle, d, B, _ptr(H), _ptr(Vf), _ptr(Vb), _ptr(Cf), _ptr(Cb), _ptr(Wself), _ptr(ctx.mask),
+               ctx.keep, int(ctx.relu), _ptr(out), _ptr(saved), _ptr(dOut), _ptr(dH), _ptr(dVf), _ptr(dVb), _ptr(dCf),
+               _ptr(dCb), _ptr(dWself), _ptr(db)), dev)
         return dH, dVf, dVb, dCf, dCb, dWself, db, None, None, None, None
 
 
@@ -440,7 +405,6 @@ def basis_diagcoef_layer(H, W_forward, W_backward, C_forward, C_backward, W_self
 class _DiagLayerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, H, Df, Db, Wself, b, graph, drop_mask, keep, relu):
-        lib = _lib.load()
         if not (isinstance(H, torch.Tensor) and H.dim() == 2):
             raise _lib.RgcnError("H must be a [V_src, d] tensor")
         d = H.shape[1]
@@ -453,13 +417,9 @@ class _DiagLayerFn(torch.autograd.Function):
         mask = _mask_arg(drop_mask, graph.V_dst, d)
         dev = H.device
         out = torch.empty(graph.V_dst, d, dtype=torch.float32, device=dev)
-        nb = lib.rgcn_diag_workspace_bytes(graph.handle, d, 0)
-        if nb < 0:
-            _lib.check(int(nb), "rgcn_diag_workspace_bytes")
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_diag_forward(graph.handle, d, _ptr(H), _ptr(Df), _ptr(Db), _ptr(Wself), _ptr(b), _ptr(mask),
-                                   float(keep), int(bool(relu)), _ptr(out), _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_diag_forward")
+        _call("rgcn_diag_forward", "rgcn_diag_workspace_bytes", (graph.handle, d, 0),
+              (graph.handle, d, _ptr(H), _ptr(Df), _ptr(Db), _ptr(Wself), _ptr(b), _ptr(mask), float(keep),
+               int(bool(relu)), _ptr(out)), dev)
         ctx.graph, ctx.keep, ctx.relu, ctx.mask = graph, float(keep), bool(relu), mask
         ctx.params = (Df, Db)   # the caller's tensor objects (slice norms are parked on them)
         ctx.save_for_backward(H, Df, Db, Wself, out)
@@ -467,7 +427,6 @@ class _DiagLayerFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dOut):
-        lib = _lib.load()
         H, Df, Db, Wself, out = ctx.saved_tensors
         graph = ctx.graph
         d = H.shape[1]
@@ -478,12 +437,9 @@ class _DiagLayerFn(torch.autograd.Function):
         dDf, dDb, dWself = torch.empty_like(Df), torch.empty_like(Db), torch.empty_like(Wself)
         db = torch.empty(d, dtype=torch.float32, device=dev)
         ss = torch.empty(2, dtype=torch.float32, device=dev) if _SLICE_NORMS else None
-        nb = lib.rgcn_diag_workspace_bytes(graph.handle, d, 1)
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_diag_backward(graph.handle, d, _ptr(H), _ptr(Df), _ptr(Db), _ptr(Wself), _ptr(ctx.mask),
-                                    ctx.keep, int(ctx.relu), _ptr(out), _ptr(dOut), _ptr(dH), _ptr(dDf), _ptr(dDb),
-                                    _ptr(dWself), _ptr(db), _ptr(ss), _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_diag_backward")
+        _call("rgcn_diag_backward", "rgcn_diag_workspace_bytes", (graph.handle, d, 1),
+              (graph.handle, d, _ptr(H), _ptr(Df), _ptr(Db), _ptr(Wself), _ptr(ctx.mask), ctx.keep, int(ctx.relu),
+               _ptr(out), _ptr(dOut), _ptr(dH), _ptr(dDf), _ptr(dDb), _ptr(dWself), _ptr(db), _ptr(ss)), dev)
         if ss is not None:
             _add_slice_sumsq(ctx.params[0], ss[0])
             _add_slice_sumsq(ctx.params[1], ss[1])
@@ -501,7 +457,6 @@ def diag_layer(H, D_forward, D_backward, W_self, b, graph, drop_mask=None, keep=
 class _HighwayFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, c1, c2, W, b):
-        lib = _lib.load()
         if not (isinstance(c1, torch.Tensor) and c1.dim() == 2):
             raise _lib.RgcnError("c1 must be a [V, d] tensor")
         V, d = c1.shape
@@ -512,19 +467,13 @@ class _HighwayFn(torch.autograd.Function):
         dev = c1.device
         out = torch.empty(V, d, dtype=torch.float32, device=dev)
         gate = torch.empty(V, d, dtype=torch.float32, device=dev)
-        nb = lib.rgcn_highway_workspace_bytes(V, d, 0)
-        if nb < 0:
-            _lib.check(int(nb), "rgcn_highway_workspace_bytes")
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_highway_forward(_ptr(c1), _ptr(c2), _ptr(W), _ptr(b), V, d, _ptr(out), _ptr(gate), _ptr(ws),
-                                      ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_highway_forward")
+        _call("rgcn_highway_forward", "rgcn_highway_workspace_bytes", (V, d, 0),
+              (_ptr(c1), _ptr(c2), _ptr(W), _ptr(b), V, d, _ptr(out), _ptr(gate)), dev)
         ctx.save_for_backward(c1, c2, W, gate)
         return out
 
     @staticmethod
     def backward(ctx, dOut):
-        lib = _lib.load()
         c1, c2, W, gate = ctx.saved_tensors
         V, d = c1.shape
         dOut = dOut.contiguous()
@@ -532,11 +481,9 @@ class _HighwayFn(torch.autograd.Function):
         dev = c1.device
         dc1, dc2, dW = torch.empty_like(c1), torch.empty_like(c2), torch.empty_like(W)
         db = torch.empty(d, dtype=torch.float32, device=dev)
-        nb = lib.rgcn_highway_workspace_bytes(V, d, 1)
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_highway_backward(_ptr(c1), _ptr(c2), _ptr(W), _ptr(gate), _ptr(dOut), V, d, _ptr(dc1),
-                                       _ptr(dc2), _ptr(dW), _ptr(db), _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_highway_backward")
+        _call("rgcn_highway_backward", "rgcn_highway_workspace_bytes", (V, d, 1),
+              (_ptr(c1), _ptr(c2), _ptr(W), _ptr(gate), _ptr(dOut), V, d, _ptr(dc1), _ptr(dc2), _ptr(dW), _ptr(db)),
+              dev)
         return dc1, dc2, dW, db
 
 
@@ -549,7 +496,6 @@ def highway(c1, c2, W, b):
 class _VariationalFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, H, W_mu, b_mu, W_sigma, b_sigma, eps):
-        lib = _lib.load()
         if not (isinstance(W_mu, torch.Tensor) and W_mu.dim() == 2):
             raise _lib.RgcnError("W_mu must be a 2-D tensor")
         w = W_mu.shape[1]
@@ -571,21 +517,15 @@ class _VariationalFn(torch.autograd.Function):
         z = torch.empty(V, w, dtype=torch.float32, device=dev)
         kl = torch.empty((), dtype=torch.float32, device=dev)
         P = torch.empty(V, 2 * w, dtype=torch.float32, device=dev) if d else None
-        nb = lib.rgcn_variational_workspace_bytes(V, d, w, 0)
-        if nb < 0:
-            _lib.check(int(nb), "rgcn_variational_workspace_bytes")
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_variational_forward(_ptr(H), V, d, w, _ptr(W_mu), _ptr(b_mu if d else None), _ptr(W_sigma),
-                                          _ptr(b_sigma if d else None), _ptr(eps), _ptr(z), _ptr(P), _ptr(kl),
-                                          _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_variational_forward")
+        _call("rgcn_variational_forward", "rgcn_variational_workspace_bytes", (V, d, w, 0),
+              (_ptr(H), V, d, w, _ptr(W_mu), _ptr(b_mu if d else None), _ptr(W_sigma), _ptr(b_sigma if d else None),
+               _ptr(eps), _ptr(z), _ptr(P), _ptr(kl)), dev)
         ctx.d = d
         ctx.save_for_backward(H, W_mu, W_sigma, P, eps)
         return z, kl
 
     @staticmethod
     def backward(ctx, dz, g_kl):
-        lib = _lib.load()
         H, W_mu, W_sigma, P, eps = ctx.saved_tensors
         d = ctx.d
         V, w = eps.shape
@@ -597,12 +537,9 @@ class _VariationalFn(torch.autograd.Function):
         dH = torch.empty_like(H) if d else None
         db_mu = torch.empty(w, dtype=torch.float32, device=dev) if d else None
         db_sigma = torch.empty(w, dtype=torch.float32, device=dev) if d else None
-        nb = lib.rgcn_variational_workspace_bytes(V, d, w, 1)
-        ws = _workspace(nb, dev)
-        rc = lib.rgcn_variational_backward(_ptr(H), V, d, w, _ptr(W_mu), _ptr(W_sigma), _ptr(P), _ptr(eps), _ptr(dz),
-                                           _ptr(g_kl), _ptr(dH), _ptr(dW_mu), _ptr(db_mu), _ptr(dW_sigma),
-                                           _ptr(db_sigma), _ptr(ws), ws.numel(), _stream(dev))
-        _lib.check(rc, "rgcn_variational_backward")
+        _call("rgcn_variational_backward", "rgcn_variational_workspace_bytes", (V, d, w, 1),
+              (_ptr(H), V, d, w, _ptr(W_mu), _ptr(W_sigma), _ptr(P), _ptr(eps), _ptr(dz), _ptr(g_kl), _ptr(dH),
+               _ptr(dW_mu), _ptr(db_mu), _ptr(dW_sigma), _ptr(db_sigma)), dev)
         # the embedding variant's biases are never read: their gradient is None, as in the reference
         return dH, dW_mu, db_mu, dW_sigma, db_sigma, None
 
@@ -773,21 +710,16 @@ def rows_gather_to(dst_ptr, src, rows, max_ctas=0):
 
 def block_aggregate_(out, X, W_forward, W_backward, graph, n_blocks):
     """out[dst] += sum_m norm_m W[relw_m] . X[src_m] (messages only, in place; rgcn_block_aggregate)."""
-    lib = _lib.load()
     d = X.shape[1]
     _check_cuda_f32("X", X, (graph.V_src, d))
     _check_cuda_f32("out", out, (graph.V_dst, d))
-    nb = lib.rgcn_block_aggregate_workspace_bytes(graph.handle, d, n_blocks, 0)
-    ws = _workspace(nb, X.device)
-    rc = lib.rgcn_block_aggregate(graph.handle, d, n_blocks, _ptr(X), _ptr(W_forward), _ptr(W_backward),
-                                  _ptr(out), _ptr(ws), ws.numel(), _stream(X.device))
-    _lib.check(rc, "rgcn_block_aggregate")
+    _call("rgcn_block_aggregate", "rgcn_block_aggregate_workspace_bytes", (graph.handle, d, n_blocks, 0),
+          (graph.handle, d, n_blocks, _ptr(X), _ptr(W_forward), _ptr(W_backward), _ptr(out)), X.device)
     return out
 
 
 def block_aggregate_backward(X, W_forward, W_backward, G, graph, n_blocks, dWf=None, dWb=None):
     """Returns (dX, dWf, dWb) of block_aggregate_; when dWf/dWb are given they are accumulated into."""
-    lib = _lib.load()
     d = X.shape[1]
     _check_cuda_f32("X", X, (graph.V_src, d))
     _check_cuda_f32("G", G, (graph.V_dst, d))
@@ -795,12 +727,9 @@ def block_aggregate_backward(X, W_forward, W_backward, G, graph, n_blocks, dWf=N
     if not acc:
         dWf, dWb = torch.empty_like(W_forward), torch.empty_like(W_backward)
     dX = torch.empty_like(X)
-    nb = lib.rgcn_block_aggregate_workspace_bytes(graph.handle, d, n_blocks, 1)
-    ws = _workspace(nb, X.device)
-    rc = lib.rgcn_block_aggregate_backward(graph.handle, d, n_blocks, _ptr(X), _ptr(W_forward), _ptr(W_backward),
-                                           _ptr(G), _ptr(dX), _ptr(dWf), _ptr(dWb), int(acc), _ptr(ws),
-                                           ws.numel(), _stream(X.device))
-    _lib.check(rc, "rgcn_block_aggregate_backward")
+    _call("rgcn_block_aggregate_backward", "rgcn_block_aggregate_workspace_bytes", (graph.handle, d, n_blocks, 1),
+          (graph.handle, d, n_blocks, _ptr(X), _ptr(W_forward), _ptr(W_backward), _ptr(G), _ptr(dX), _ptr(dWf),
+           _ptr(dWb), int(acc)), X.device)
     return dX, dWf, dWb
 
 
@@ -826,13 +755,24 @@ class DistMultRanker(object):
         # the relation queries keep their own workspace: its head is the split of rel[0:R], not of `codes`
         self._rel_ws, self._rel_split_ready = None, False
 
-    def _check_rows(self, X, mask, name):
+    def _check_rows(self, X, mask, name, count=None, label="V"):
+        """X int32 [n,3] CUDA; mask None or int32 [n, ceil(count/32)] CUDA, count the candidates (default: V)."""
         if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
             raise _lib.RgcnError("X must be a contiguous CUDA int32 [n,3] tensor")
-        words = (self.codes.shape[0] + 31) // 32
+        words = ((self.codes.shape[0] if count is None else count) + 31) // 32
         if mask is not None and not (mask.is_cuda and mask.dtype == torch.int32
                                      and mask.is_contiguous() and tuple(mask.shape) == (X.shape[0], words)):
-            raise _lib.RgcnError("%s must be a contiguous CUDA int32 [n, ceil(V/32)] tensor (bit masks)" % name)
+            raise _lib.RgcnError("%s must be a contiguous CUDA int32 [n, ceil(%s/32)] tensor (bit masks)"
+                                 % (name, label))
+
+    def _chunk_rows(self, n, workspace_bytes, name):
+        """(queries per library call, workspace bytes of such a call) for n queries, so that a call's workspace beyond
+        the split of its table stays under TOPK_CHUNK_BYTES; workspace_bytes(m) sizes a call of m queries."""
+        split_bytes = workspace_bytes(0)
+        if split_bytes < 0:
+            _lib.check(int(split_bytes), name)
+        chunk = max(1, min(n, self.TOPK_CHUNK_BYTES // max(1, workspace_bytes(1) - split_bytes)))
+        return chunk, workspace_bytes(chunk)
 
     def top_k(self, X, side, k, exclude_mask=None):
         """The k entities of highest energy for every triple of X (int32 [n,3] CUDA; side 0 predicts subjects, 1
@@ -844,13 +784,9 @@ class DistMultRanker(object):
         V, d = self.codes.shape
         self._check_rows(X, exclude_mask, "exclude_mask")
         k, n = int(k), X.shape[0]
-        split_bytes = lib.rgcn_topk_workspace_bytes(V, d, 0, k)
-        if split_bytes < 0:
-            _lib.check(int(split_bytes), "rgcn_topk_workspace_bytes")
-        per_row = lib.rgcn_topk_workspace_bytes(V, d, 1, k) - split_bytes
-        chunk = max(1, min(n, self.TOPK_CHUNK_BYTES // per_row))
+        chunk, nb = self._chunk_rows(n, lambda m: lib.rgcn_topk_workspace_bytes(V, d, m, k),
+                                     "rgcn_topk_workspace_bytes")
         dev = self.codes.device
-        nb = lib.rgcn_topk_workspace_bytes(V, d, chunk, k)
         if self._ws is None or self._ws.numel() < nb:
             self._ws, self._ws_n, self._split_ready = _workspace(nb, dev), -1, False
         ids = torch.empty((n, k), dtype=torch.int32, device=dev)
@@ -871,13 +807,8 @@ class DistMultRanker(object):
         Returns (raw_rank, filtered_rank or None) int32 CUDA tensors."""
         lib = _lib.load()
         V, d = self.codes.shape
-        if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
-            raise _lib.RgcnError("X must be a contiguous CUDA int32 [n,3] tensor")
+        self._check_rows(X, known_mask, "known_mask")
         n = X.shape[0]
-        words = (V + 31) // 32
-        if known_mask is not None and not (known_mask.is_cuda and known_mask.dtype == torch.int32
-                                           and known_mask.is_contiguous() and tuple(known_mask.shape) == (n, words)):
-            raise _lib.RgcnError("known_mask must be a contiguous CUDA int32 [n, ceil(V/32)] tensor (bit masks)")
         dev = self.codes.device
         if self._ws is None or n > self._ws_n:
             nb = getattr(lib, self._WORKSPACE)(V, d, n)
@@ -897,19 +828,9 @@ class DistMultRanker(object):
     def _relation_calls(self, X, mask, name, workspace_bytes):
         """Checks X and the [n, ceil(R/32)] mask, sizes the relation workspace for chunks of at most
         TOPK_CHUNK_BYTES beyond the split, and yields (c0, c1) per chunk; the split is marked ready after each."""
-        lib = _lib.load()
-        R, d = self.relation_count, self.codes.shape[1]
-        if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
-            raise _lib.RgcnError("X must be a contiguous CUDA int32 [n,3] tensor")
-        n, words = X.shape[0], (R + 31) // 32
-        if mask is not None and not (mask.is_cuda and mask.dtype == torch.int32
-                                     and mask.is_contiguous() and tuple(mask.shape) == (n, words)):
-            raise _lib.RgcnError("%s must be a contiguous CUDA int32 [n, ceil(R/32)] tensor (bit masks)" % name)
-        split_bytes = workspace_bytes(0)
-        if split_bytes < 0:
-            _lib.check(int(split_bytes), "relation workspace bytes")
-        chunk = max(1, min(n, self.TOPK_CHUNK_BYTES // max(1, workspace_bytes(1) - split_bytes)))
-        nb = workspace_bytes(chunk)
+        self._check_rows(X, mask, name, self.relation_count, "R")
+        n = X.shape[0]
+        chunk, nb = self._chunk_rows(n, workspace_bytes, "relation workspace bytes")
         if self._rel_ws is None or self._rel_ws.numel() < nb:
             self._rel_ws, self._rel_split_ready = _workspace(nb, self.codes.device), False
         for c0 in range(0, max(n, 1), chunk):

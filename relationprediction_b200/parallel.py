@@ -347,17 +347,14 @@ class _OverlappedBlockLayer(torch.autograd.Function):
             back = torch.empty(int(p.send_counts.sum()), G.shape[1], dtype=G.dtype, device=G.device)
             work = dist.all_to_all_single(back, dHalo, output_split_sizes=p.send_counts.tolist(),
                                           input_split_sizes=p.recv_counts.tolist(), group=sg.group, async_op=True)
-        lib = ops._lib.load()
         d = H_local.shape[1]
         dH = torch.empty_like(H_local)
         dWf_l, dWb_l, dWs = torch.empty_like(Wf), torch.empty_like(Wb), torch.empty_like(Ws)
-        nb = lib.rgcn_block_workspace_bytes(sg.graph_local.handle, d, B, 1)
-        ws = ops._workspace(nb, G.device)
-        rc = lib.rgcn_block_backward(sg.graph_local.handle, d, B, ops._ptr(H_local), ops._ptr(Wf), ops._ptr(Wb),
-                                     ops._ptr(Ws), ops._ptr(ctx.mask), float(ctx.keep), 0, ops._ptr(out),
-                                     ops._ptr(G), ops._ptr(dH), ops._ptr(dWf_l), ops._ptr(dWb_l), ops._ptr(dWs),
-                                     ops._ptr(ws), ws.numel(), ops._stream(G.device))
-        ops._lib.check(rc, "rgcn_block_backward")
+        h = sg.graph_local.handle
+        ops._call("rgcn_block_backward", "rgcn_block_workspace_bytes", (h, d, B, 1),
+                  (h, d, B, ops._ptr(H_local), ops._ptr(Wf), ops._ptr(Wb), ops._ptr(Ws), ops._ptr(ctx.mask),
+                   float(ctx.keep), 0, ops._ptr(out), ops._ptr(G), ops._ptr(dH), ops._ptr(dWf_l), ops._ptr(dWb_l),
+                   ops._ptr(dWs)), G.device)
         dWf += dWf_l
         dWb += dWb_l
         if work is not None:
@@ -456,16 +453,13 @@ class _PipelinedBlockLayer(torch.autograd.Function):
                                                             sg.graph_halo_peer[rf], B, dWf, dWb)
                 alive.append(dX)
             works.append(ring_post_backward_step(sg, k, dX, back))
-        lib = ops._lib.load()
         dH = torch.empty_like(H_local)
         dWf_l, dWb_l, dWs = torch.empty_like(Wf), torch.empty_like(Wb), torch.empty_like(Ws)
-        nb = lib.rgcn_block_workspace_bytes(sg.graph_local.handle, d, B, 1)
-        ws = ops._workspace(nb, G.device)
-        rc = lib.rgcn_block_backward(sg.graph_local.handle, d, B, ops._ptr(H_local), ops._ptr(Wf), ops._ptr(Wb),
-                                     ops._ptr(Ws), ops._ptr(ctx.mask), float(ctx.keep), 0, ops._ptr(out),
-                                     ops._ptr(G), ops._ptr(dH), ops._ptr(dWf_l), ops._ptr(dWb_l), ops._ptr(dWs),
-                                     ops._ptr(ws), ws.numel(), ops._stream(G.device))
-        ops._lib.check(rc, "rgcn_block_backward")
+        h = sg.graph_local.handle
+        ops._call("rgcn_block_backward", "rgcn_block_workspace_bytes", (h, d, B, 1),
+                  (h, d, B, ops._ptr(H_local), ops._ptr(Wf), ops._ptr(Wb), ops._ptr(Ws), ops._ptr(ctx.mask),
+                   float(ctx.keep), 0, ops._ptr(out), ops._ptr(G), ops._ptr(dH), ops._ptr(dWf_l), ops._ptr(dWb_l),
+                   ops._ptr(dWs)), G.device)
         if dWf is not None:
             dWf_l += dWf
             dWb_l += dWb

@@ -1,7 +1,7 @@
 """The message-walk kernels of the block-diagonal layer -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
-One row per configuration the dispatch can reach: `use_rel_major` / `use_staged` and the dW-fusion decision in
-csrc/api.cu, `launch_block_stg` (csrc/block_staged.cu), `launch_block_rel`, `launch_block_agg` and
+One row per configuration the dispatch can reach: the walk choice of `choose_block_walk` (weight-id major, staged,
+fused dW) in csrc/api.cu, `launch_block_stg` (csrc/block_staged.cu), `launch_block_rel`, `launch_block_agg` and
 `launch_block_dw` (csrc/rgcn_kernels.cu).  A row names the block_algo option, the environment knobs, the block size
 s, a representative width d, and the walk kernels (with their template arguments) that one forward and one backward
 of the layer launch.  tests/test_block_walk_table_host.py checks that the table and UNREACHABLE together name every

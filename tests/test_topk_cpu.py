@@ -40,6 +40,29 @@ def test_entry_points_reject_bad_arguments(name):
     assert b"workspace too small" in lib.rgcn_last_error()
 
 
+@pytest.mark.parametrize("name", ("distmult_rank", "rgcn_complex_rank"))
+def test_rank_entry_points_reject_bad_arguments(name):
+    lib = _lib.load()
+    buf = np.zeros(1 << 16, np.float32)
+    p = ctypes.c_void_p(buf.ctypes.data)
+    need = lib.distmult_rank_workspace_bytes(300, 8, 4)
+
+    def call(V=300, Vrel=7, d=8, n=4, side=1, codes=p, rel=p, X=p, mask=None, raw=p, filt=None, ws=p, ws_bytes=need):
+        return getattr(lib, name)(codes, rel, V, Vrel, d, X, n, side, mask, 0, raw, filt, ws, ws_bytes, None)
+    for kw, needle in ((dict(codes=None), b"bad arguments"), (dict(rel=None), b"bad arguments"),
+                       (dict(X=None), b"bad arguments"), (dict(raw=None), b"bad arguments"),
+                       (dict(ws=None), b"bad arguments"), (dict(V=0), b"bad arguments"),
+                       (dict(Vrel=0), b"bad arguments"), (dict(d=0), b"bad arguments"), (dict(d=6), b"d % 4"),
+                       (dict(n=-1), b"bad arguments"), (dict(side=2), b"side"), (dict(side=-1), b"side"),
+                       (dict(filt=p), b"known mask")):
+        assert call(**kw) == -1, kw
+        msg = lib.rgcn_last_error()
+        assert name.encode() in msg and needle in msg, (kw, msg)
+    assert call(ws_bytes=need - 1) == -4
+    assert b"workspace too small" in lib.rgcn_last_error()
+    assert call(filt=p, mask=p, ws_bytes=need - 1) == -4   # a filtered call with its mask passes the checks
+
+
 def test_workspace_bytes_rejects_bad_input_and_grows_with_n_and_k():
     lib = _lib.load()
     for args in ((0, 8, 4, 10), (100, 0, 4, 10), (100, 6, 4, 10), (100, 8, -1, 10), (100, 8, 4, 0),
