@@ -621,6 +621,54 @@ int rgcn_complex_relation_topk(const float* codes, const float* rel, int32_t V, 
                                const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask, int reuse_split,
                                int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * 1-N training (also called KvsAll), fused: every query scored against every entity with a sigmoid cross-entropy
+ * over multi-hot targets.  queries : int32 [n, 3] HOST rows (anchor, relation, side), 0 <= anchor < V,
+ * 0 <= relation < R, side 1 = object query (anchor, r, ?), side 0 = subject query (?, r, anchor).  Query rows q are
+ * those of the rank entry points (DistMult: codes[anchor] * rel[r]; ComplEx: the rgcn_complex_rank row of the side).
+ *   z(t, v)  = sum_k q_t[k] codes[v, k]                     (3xTF32 GEMM)
+ *   y'(t, v) = (1 - eps) + eps / V if bit v of labels row t is set, else eps / V      (0 <= eps < 1)
+ *   loss[0]  = 1 / (n V) sum_{t, v} max(z, 0) - z y' + log1p(exp(-|z|))
+ *   loss[1]  = 1 / (n d) sum_t |codes[anchor_t]|^2 + |rel[r_t]|^2   (the decoders' L2 term, un-scaled)
+ * labels : uint32 [n, ceil(V/32)] device (rgcn_one_to_n_labels).  loss float32 [2] device; both parts are summed in a
+ * fixed order, so they are bitwise repeatable.  With dcodes / drel (both or neither; [V, d] / [Vrel, d] device,
+ * overwritten) the call also writes the gradient of g[0] loss[0] + g[1] loss[1], g = g_scale float32 [2] device (NULL:
+ * (1, 1)).  Queries sorted by side run as two launches of each per-query kernel; any order gives the same sums.
+ * chunk : queries per internal pass (>= 1); the workspace holds the [V, chunk] energy gradients of one pass (chunk
+ * rounded up to 8).
+ * workspace : rgcn_one_to_n_workspace_bytes(V, d, n, chunk).
+ * Errors, before any device work: RGCN_ERR_INVALID (null pointers, V <= 0, R outside [1, Vrel], d % 4 != 0, chunk < 1,
+ * eps outside [0, 1), a query id out of range or a side outside {0, 1}), RGCN_ERR_WORKSPACE, RGCN_ERR_NODEVICE.
+ *
+ * rgcn_one_to_n_finish: from dcodes_loss / drel_loss written by a call with g_scale = (1, 0) (the gradient of loss[0]
+ * alone) and the same queries, dcodes = g[0] dcodes_loss + g[1] d loss[1] / d codes, and drel likewise; g = g_scale
+ * float32 [2] device (required).  No GEMM: one scaling pass and the L2 term's scatter.  Outputs may not alias the
+ * inputs.  workspace : rgcn_one_to_n_finish_workspace_bytes(n).  Errors as above.
+ *
+ * rgcn_one_to_n_labels: the label rows of host queries (as above) from a CSR of the training triples: keys int64
+ * [n_keys] sorted ascending, key = (2 relation + side) V + anchor; the entities of key i are
+ * entities[offsets[i] .. offsets[i + 1]) (int64 offsets [n_keys + 1]), all device.  Bit v of bits row t is set iff v is
+ * listed under query t's key.  bits uint32 [n, ceil(V/32)] device; workspace rgcn_one_to_n_labels_workspace_bytes(n).
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_one_to_n_workspace_bytes(int32_t V, int32_t d, int64_t n, int64_t chunk);
+int distmult_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                      const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing, const float* g_scale,
+                      float* loss, float* dcodes, float* drel, int64_t chunk, void* workspace, int64_t workspace_bytes,
+                      void* stream);
+int rgcn_complex_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                          const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
+                          const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk,
+                          void* workspace, int64_t workspace_bytes, void* stream);
+int64_t rgcn_one_to_n_finish_workspace_bytes(int64_t n);
+int rgcn_one_to_n_finish(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                         const int32_t* queries, int64_t n, const float* g_scale, const float* dcodes_loss,
+                         const float* drel_loss, float* dcodes, float* drel, void* workspace, int64_t workspace_bytes,
+                         void* stream);
+int64_t rgcn_one_to_n_labels_workspace_bytes(int64_t n);
+int rgcn_one_to_n_labels(const int64_t* keys, const int64_t* offsets, const int32_t* entities, int64_t n_keys,
+                         int32_t V, int32_t R, const int32_t* queries, int64_t n, uint32_t* bits, void* workspace,
+                         int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

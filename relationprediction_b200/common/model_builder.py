@@ -6,7 +6,7 @@ BasisGcn; SkipConnections=Highway wraps every
 feature-input layer in a HighwayLayer), `embedding`, and the variational encoders `variational_embedding` and
 `variational_gcn_basis` (a VariationalEncoding over two linear AffineTransform heads); decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
-from ..decoders.bilinear_diag import BilinearDiag
+from ..decoders.bilinear_diag import BilinearDiag, parse_training_objective
 from ..decoders.complex import Complex
 from ..encoders.affine_transform import AffineTransform
 from ..encoders.message_gcns.gcn_basis import BasisGcn
@@ -163,6 +163,10 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
 
 
 def build_decoder(encoder, decoder_settings):
+    if decoder_settings['Name'] not in ("bilinear-diag", "complex") and \
+            parse_training_objective(decoder_settings)[0] == '1-N':
+        raise ValueError("TrainingObjective=1-N needs the bilinear-diag or complex decoder, not %r"
+                         % (decoder_settings['Name'],))
     if decoder_settings['Name'] == "bilinear-diag":
         return BilinearDiag(encoder, decoder_settings)
     if decoder_settings['Name'] == "complex":

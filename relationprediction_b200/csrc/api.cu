@@ -7,6 +7,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <vector>
 
 #include "kernels.cuh"
 
@@ -1708,4 +1709,279 @@ extern "C" int rgcn_complex_relation_topk(const float* codes, const float* rel, 
   return topk_with_queries(who, complex_relation_prepare, rel, R, rgcn_relation_topk_workspace_bytes, codes, rel, V,
                            Vrel, d, X, n, 0, k, exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes,
                            (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------------
+// 1-N training (DistMult and ComplEx): every query scored against every entity, BCE loss and gradients fused
+// ------------------------------------------------------------------------------------------------
+// The queries (anchor, r, side) come from the HOST, so every id is checked before any device work; they go to the
+// device as the triples (anchor, r, anchor) the rank prepare kernels read, and each maximal run of one side is one
+// launch of the prepare, label and query-backward kernels (callers that sort by side make two runs).
+// Per chunk of c queries (cp = c rounded up to 8, so that a warp's Gt stores are whole 32 B sectors):
+// Q = prepare(queries) [cp, d]; the BCE GEMM writes the loss parts and Gt [V, cp] (transposed energy gradients);
+// dQ = Gt^T codes (TN GEMM, contraction over V);
+// dcodes (+)= Gt Q (NT GEMM over the split of Q^T, contraction over the chunk); the query backward turns dQ and the
+// L2 term into the anchor and relation gradients.  Workspace layout: [hi V*d | lo V*d | X n*3 | reg parts |
+// loss parts | Q cp*d | dQ cp*d | Qt hi d*cp | Qt lo d*cp | Gt V*cp].
+struct OnenRun {
+  int64_t begin, end;
+  int side;
+};
+
+static int onen_query_checks(const char* who, const int32_t* queries, int64_t n, int32_t V, int32_t R,
+                             std::vector<OnenRun>* runs) {
+  for (int64_t t = 0; t < n; ++t) {
+    const int32_t a = queries[3 * t], r = queries[3 * t + 1], s = queries[3 * t + 2];
+    if (a < 0 || a >= V || r < 0 || r >= R || (s != 0 && s != 1)) {
+      rgcn_set_error(std::string(who) + ": query " + std::to_string(t) +
+                     " is invalid (need 0 <= anchor < V, 0 <= relation < R, side in {0,1})");
+      return RGCN_ERR_INVALID;
+    }
+    if (runs->empty() || runs->back().side != s) runs->push_back(OnenRun{t, t, s});
+    runs->back().end = t + 1;
+  }
+  return RGCN_OK;
+}
+
+static int onen_device_checks(const char* who) {
+  int n_dev = 0;
+  if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
+    cudaGetLastError();
+    rgcn_set_error(std::string(who) + ": no CUDA device");
+    return RGCN_ERR_NODEVICE;
+  }
+  return RGCN_OK;
+}
+
+// the queries as device triples (anchor, r, anchor)
+static int onen_upload(const int32_t* queries, int64_t n, int32_t* X, cudaStream_t st) {
+  std::vector<int32_t> tri((size_t)n * 3);
+  for (int64_t t = 0; t < n; ++t) {
+    tri[3 * t] = tri[3 * t + 2] = queries[3 * t];
+    tri[3 * t + 1] = queries[3 * t + 1];
+  }
+  // from pageable memory: the call returns once the host buffer has been read
+  return rgcn_check_cuda(cudaMemcpyAsync(X, tri.data(), tri.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st),
+                         "memcpy(queries)");
+}
+
+static int64_t onen_chunk(int64_t n, int64_t chunk) { return std::max<int64_t>(1, std::min(chunk, n)); }
+
+static int64_t onen_loss_parts(int64_t n, int64_t c, int32_t V) {
+  return n == 0 ? 0 : (n / c) * gemm_onen_loss_parts(c, V) + (n % c ? gemm_onen_loss_parts(n % c, V) : 0);
+}
+
+extern "C" int64_t rgcn_one_to_n_workspace_bytes(int32_t V, int32_t d, int64_t n, int64_t chunk) {
+  if (V <= 0 || d <= 0 || d % 4 != 0 || n < 0 || n > 0x7fffffffLL || chunk < 1) {
+    rgcn_set_error("rgcn_one_to_n_workspace_bytes: bad arguments (need V > 0, d > 0, d % 4 == 0, 0 <= n < 2^31, "
+                   "chunk >= 1)");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t c = onen_chunk(n, chunk), cp = (c + 7) / 8 * 8;
+  return 2 * align_up((int64_t)V * d * 4) + align_up(n * 12) + align_up(onen_reg_parts(n) * 4) +
+         align_up(onen_loss_parts(n, c, V) * 4) + 2 * align_up(cp * d * 4) + 2 * align_up((int64_t)d * cp * 4) +
+         align_up((int64_t)V * cp * 4) + 256;
+}
+
+static int one_to_n(const char* who, int complex, const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                    int32_t R, int32_t d, const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
+                    const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk, void* workspace,
+                    int64_t workspace_bytes, cudaStream_t st) {
+  if (!codes || !rel || !loss || !workspace || (n > 0 && (!queries || !labels)) || (!dcodes != !drel)) {
+    rgcn_set_error(std::string(who) + ": null pointer (dcodes and drel are both given or both NULL)");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || Vrel <= 0 || R < 1 || R > Vrel || d <= 0 || d % 4 != 0 || n < 0 || n > 0x7fffffffLL || chunk < 1) {
+    rgcn_set_error(std::string(who) + ": bad sizes (need V > 0, 1 <= R <= Vrel, d > 0, d % 4 == 0, 0 <= n < 2^31, "
+                   "chunk >= 1)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!(smoothing >= 0.f && smoothing < 1.f)) {   // also refuses NaN
+    rgcn_set_error(std::string(who) + ": label smoothing must be in [0, 1)");
+    return RGCN_ERR_INVALID;
+  }
+  std::vector<OnenRun> runs;
+  int rc = onen_query_checks(who, queries, n, V, R, &runs);
+  if (rc) return rc;
+  if (workspace_bytes < rgcn_one_to_n_workspace_bytes(V, d, n, chunk)) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_one_to_n_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who);
+  if (rc) return rc;
+
+  const bool grads = dcodes != nullptr;
+  if (n == 0) {   // no queries: zero loss and gradients
+    rc = rgcn_check_cuda(cudaMemsetAsync(loss, 0, 2 * sizeof(float), st), "memset(loss)");
+    if (!rc && grads) rc = rgcn_check_cuda(cudaMemsetAsync(dcodes, 0, (size_t)V * d * 4, st), "memset(dcodes)");
+    if (!rc && grads) rc = rgcn_check_cuda(cudaMemsetAsync(drel, 0, (size_t)Vrel * d * 4, st), "memset(drel)");
+    return rc;
+  }
+  const int64_t c = onen_chunk(n, chunk), cp = (c + 7) / 8 * 8;
+  const int words = (V + 31) / 32;
+  Carver ws(workspace, workspace_bytes);
+  float* hi = ws.take<float>((int64_t)V * d);
+  float* lo = ws.take<float>((int64_t)V * d);
+  int32_t* X = ws.take<int32_t>(n * 3);
+  float* reg_part = ws.take<float>(onen_reg_parts(n));
+  float* loss_part = ws.take<float>(onen_loss_parts(n, c, V));
+  float* Q = ws.take<float>(cp * d);
+  float* dQ = ws.take<float>(cp * d);
+  float* qt_hi = ws.take<float>((int64_t)d * cp);
+  float* qt_lo = ws.take<float>((int64_t)d * cp);
+  float* Gt = ws.take<float>((int64_t)V * cp);
+  const RankPrepareFn prepare = complex ? launch_complex_rank_prepare : launch_distmult_rank_prepare;
+  const float pos = (float)((1.0 - smoothing) + (double)smoothing / V), neg = (float)((double)smoothing / V);
+  const float scale = (float)(1.0 / ((double)n * V));
+  const float c_reg = (float)(2.0 / ((double)n * d));
+
+  MARK("start");
+  rc = onen_upload(queries, n, X, st);
+  if (!rc) rc = launch_gemm_split_b(codes, d, V, d, /*transposed=*/0, hi, lo, st);
+  if (!rc) rc = launch_onen_reg(codes, rel, d, X, n, reg_part, st);
+  if (!rc && grads) rc = rgcn_check_cuda(cudaMemsetAsync(drel, 0, (size_t)Vrel * d * 4, st), "memset(drel)");
+  if (rc) return rc;
+  MARK("onen_setup");
+  int64_t part = 0;
+  for (int64_t c0 = 0; c0 < n; c0 += c) {
+    const int64_t c1 = std::min(n, c0 + c), m = c1 - c0, mp = (m + 7) / 8 * 8;
+    for (const OnenRun& run : runs) {
+      const int64_t b = std::max(run.begin, c0), e = std::min(run.end, c1);
+      if (b < e) rc = prepare(codes, rel, d, X + 3 * b, e - b, run.side, Q + (b - c0) * d, nullptr, nullptr, st);
+      if (rc) return rc;
+    }
+    rc = launch_gemm_onen_tf32x3(Q, d, hi, lo, d, (int)m, V, d, labels + c0 * words, pos, neg, scale, g_scale,
+                                 grads ? Gt : nullptr, mp, loss_part + part, st);
+    if (rc) return rc;
+    part += gemm_onen_loss_parts(m, V);
+    MARK("onen_scoring_gemm");
+    if (!grads) continue;
+    if (mp > m) {   // the K padding of the dcodes GEMM: zero rows of Q, zero columns of Gt
+      rc = rgcn_check_cuda(cudaMemsetAsync(Q + m * d, 0, (size_t)(mp - m) * d * 4, st), "memset(Q pad)");
+      if (!rc)
+        rc = rgcn_check_cuda(cudaMemset2DAsync(Gt + m, (size_t)mp * 4, 0, (size_t)(mp - m) * 4, V, st),
+                             "memset(Gt pad)");
+      if (rc) return rc;
+    }
+    rc = launch_gemm_tn_tf32x3(Gt, mp, codes, d, dQ, d, (int)mp, d, V, /*accumulate=*/0, st);
+    MARK("onen_dQ_gemm");
+    if (!rc) rc = launch_gemm_split_b(Q, d, d, (int)mp, /*transposed=*/1, qt_hi, qt_lo, st);
+    if (!rc) rc = launch_gemm_tf32x3(Gt, mp, qt_hi, qt_lo, mp, dcodes, d, V, d, (int)mp, c0 > 0, st);
+    MARK("onen_dcodes_gemm");
+    for (const OnenRun& run : runs) {
+      const int64_t b = std::max(run.begin, c0), e = std::min(run.end, c1);
+      if (!rc && b < e)
+        rc = launch_onen_query_bwd(complex, codes, rel, d, X + 3 * b, e - b, run.side, dQ + (b - c0) * d, g_scale,
+                                   c_reg, dcodes, drel, st);
+    }
+    if (rc) return rc;
+    MARK("onen_query_bwd");
+  }
+  return launch_onen_loss_reduce(loss_part, part, reg_part, onen_reg_parts(n), 1.0 / ((double)n * V),
+                                 1.0 / ((double)n * d), loss, st);
+}
+
+extern "C" int distmult_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                                 const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
+                                 const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk,
+                                 void* workspace, int64_t workspace_bytes, void* stream) {
+  return one_to_n("distmult_one_to_n", 0, codes, rel, V, Vrel, R, d, queries, n, labels, smoothing, g_scale, loss,
+                  dcodes, drel, chunk, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_complex_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                     int32_t d, const int32_t* queries, int64_t n, const uint32_t* labels,
+                                     float smoothing, const float* g_scale, float* loss, float* dcodes, float* drel,
+                                     int64_t chunk, void* workspace, int64_t workspace_bytes, void* stream) {
+  return one_to_n("rgcn_complex_one_to_n", 1, codes, rel, V, Vrel, R, d, queries, n, labels, smoothing, g_scale, loss,
+                  dcodes, drel, chunk, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+// The backward of a call made with g_scale = (1, 0): its dcodes / drel are the loss's gradient alone, so the gradient
+// of g[0] loss[0] + g[1] loss[1] is g[0] times them plus g[1] times the L2 term's gradient, which needs no GEMM.
+extern "C" int64_t rgcn_one_to_n_finish_workspace_bytes(int64_t n) {
+  if (n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_one_to_n_finish_workspace_bytes: need 0 <= n < 2^31");
+    return RGCN_ERR_INVALID;
+  }
+  return align_up(n * 12) + 256;
+}
+
+extern "C" int rgcn_one_to_n_finish(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                                    const int32_t* queries, int64_t n, const float* g_scale, const float* dcodes_loss,
+                                    const float* drel_loss, float* dcodes, float* drel, void* workspace,
+                                    int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_one_to_n_finish";
+  if (!codes || !rel || !g_scale || !dcodes_loss || !drel_loss || !dcodes || !drel || !workspace ||
+      (n > 0 && !queries)) {
+    rgcn_set_error(std::string(who) + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || Vrel <= 0 || R < 1 || R > Vrel || d <= 0 || d % 4 != 0 || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error(std::string(who) + ": bad sizes (need V > 0, 1 <= R <= Vrel, d > 0, d % 4 == 0, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  std::vector<OnenRun> runs;
+  int rc = onen_query_checks(who, queries, n, V, R, &runs);
+  if (rc) return rc;
+  if (workspace_bytes < rgcn_one_to_n_finish_workspace_bytes(n)) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_one_to_n_finish_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = launch_onen_scale(dcodes_loss, g_scale, (int64_t)V * d, dcodes, st);
+  if (!rc) rc = launch_onen_scale(drel_loss, g_scale, (int64_t)Vrel * d, drel, st);
+  if (rc || n == 0) return rc;
+  int32_t* X = (int32_t*)workspace;
+  rc = onen_upload(queries, n, X, st);
+  const float c_reg = (float)(2.0 / ((double)n * d));
+  for (const OnenRun& run : runs) {   // the L2 term is the same for both decoders
+    if (!rc)
+      rc = launch_onen_query_bwd(0, codes, rel, d, X + 3 * run.begin, run.end - run.begin, run.side, nullptr, g_scale,
+                                 c_reg, dcodes, drel, st);
+  }
+  return rc;
+}
+
+extern "C" int64_t rgcn_one_to_n_labels_workspace_bytes(int64_t n) {
+  if (n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_one_to_n_labels_workspace_bytes: need 0 <= n < 2^31");
+    return RGCN_ERR_INVALID;
+  }
+  return align_up(n * 12) + 256;
+}
+
+extern "C" int rgcn_one_to_n_labels(const int64_t* keys, const int64_t* offsets, const int32_t* entities,
+                                    int64_t n_keys, int32_t V, int32_t R, const int32_t* queries, int64_t n,
+                                    uint32_t* bits, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_one_to_n_labels";
+  if (!offsets || !workspace || (n_keys > 0 && (!keys || !entities)) || (n > 0 && (!queries || !bits))) {
+    rgcn_set_error(std::string(who) + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || R <= 0 || n_keys < 0 || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error(std::string(who) + ": bad sizes (need V > 0, R > 0, n_keys >= 0, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  std::vector<OnenRun> runs;
+  int rc = onen_query_checks(who, queries, n, V, R, &runs);
+  if (rc) return rc;
+  if (workspace_bytes < rgcn_one_to_n_labels_workspace_bytes(n)) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_one_to_n_labels_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who);
+  if (rc || n == 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  int32_t* X = (int32_t*)workspace;
+  rc = onen_upload(queries, n, X, st);
+  const int words = (V + 31) / 32;
+  for (const OnenRun& run : runs) {
+    if (!rc)
+      rc = launch_onen_labels(keys, offsets, entities, n_keys, X + 3 * run.begin, run.end - run.begin, run.side, V,
+                              words, bits + run.begin * words, st);
+  }
+  return rc;
 }

@@ -218,9 +218,30 @@ struct TopKEpi {
   int tn;                      // N tiles
   uint2* cand;                 // [M, tn, k] (energy bits, column)
 };
+// EPI = 5: 1-N BCE epilogue (1-N training of DistMult / ComplEx): row m of A is a query, row n of Bt an entity code,
+// z the energy.  With y' = pos if bit n of labels row m is set, else neg (the smoothed targets),
+//   loss term  max(z, 0) - z y' + log1p(exp(-|z|)),   g = (sigmoid(z) - y') * scale * g_scale[0]
+// and g is written TRANSPOSED, Gt[n * ldgt + m] (a warp's store covers 4 columns x 8 consecutive rows: whole 32 B
+// sectors when ldgt % 8 == 0, as the caller pads it), so that the backward GEMMs read Gt with the contraction index contiguous.  Columns >= N and rows >= M
+// are never written.  Every consumer warp writes loss_part[tile * 8 + warp] = the sum of its loss terms (per thread in
+// a fixed order, then a shuffle tree), so the loss reduced from the parts is bitwise repeatable.
+struct BceEpi {
+  const uint32_t* labels;      // [M, words] bit n = entity n completes query m in the training split
+  int words;                   // ceil(N / 32)
+  float pos, neg;              // y' of a set and of a clear bit
+  float scale;                 // 1 / (n V) of the whole query set
+  const float* g_scale;        // [1] upstream gradient of the loss (device) or nullptr (1)
+  float* Gt;                   // [N, ldgt] or nullptr: loss only
+  int64_t ldgt;
+  float* loss_part;            // [tiles * 8]
+};
 template <int EPI>
 struct EpiArgs {
   using type = RankEpi;
+};
+template <>
+struct EpiArgs<5> {
+  using type = BceEpi;
 };
 template <>
 struct EpiArgs<2> {
@@ -463,6 +484,38 @@ __global__ void __launch_bounds__(N_THREADS, 1)
               if (r0 + 8 * h < M) *slot(h, p) = none;
           }
         }
+        continue;
+      }
+      if constexpr (EPI == 5) {
+        const float gs = re.scale * (re.g_scale ? __ldg(re.g_scale) : 1.f);
+        float ls = 0.f;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int row = r0 + 8 * h;
+          if (row >= M) continue;
+#pragma unroll
+          for (int cb = 0; cb < BN / 32; ++cb) {
+            const int chunk = n0 + 32 * cb;
+            const uint32_t lw = chunk < N ? __ldg(re.labels + (size_t)row * re.words + (chunk >> 5)) : 0u;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * cb + jj;
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int col = c0 + 8 * j + e;
+                if (col < N) {
+                  const float z = big[4 * j + 2 * h + e] + small[4 * j + 2 * h + e];
+                  const float y = ((lw >> (col & 31)) & 1u) ? re.pos : re.neg;
+                  ls += fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));
+                  if (re.Gt) re.Gt[(size_t)col * re.ldgt + row] = (1.0f / (1.0f + expf(-z)) - y) * gs;
+                }
+              }
+            }
+          }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) ls += __shfl_xor_sync(0xffffffffu, ls, o);
+        if (lane == 0) re.loss_part[(size_t)tile * 8 + (ctid >> 5)] = ls;
         continue;
       }
       if constexpr (EPI == 3) {
@@ -1128,6 +1181,41 @@ int launch_gemm_topk_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
                                                          (int)tiles, TopKEpi{excl, words, k, tn, cand});
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<topk>");
+}
+
+int64_t gemm_onen_loss_parts(int64_t M, int N) {
+  return ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * 8;
+}
+
+// 1-N scoring GEMM with the BCE epilogue (EPI = 5): queries Q [M,K] against the pre-split entity codes Bt [N,K];
+// gemm_onen_loss_parts(M, N) loss parts, and Gt [N, ldgt] (transposed gradients of the energies) unless Gt is null.
+int launch_gemm_onen_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, const float* Bt_lo, int64_t ldb, int M,
+                            int N, int K, const uint32_t* labels, float pos, float neg, float scale,
+                            const float* g_scale, float* Gt, int64_t ldgt, float* loss_part, cudaStream_t st) {
+  if (M == 0 || N == 0) return RGCN_OK;
+  if (K <= 0 || K % 4 != 0 || ldq % 4 != 0 || ldb % 4 != 0) {
+    rgcn_set_error("gemm_onen_tf32x3: K > 0; K and leading dimensions must be multiples of 4");
+    return RGCN_ERR_INVALID;
+  }
+  static bool attr_set = false;
+  if (!attr_set) {
+    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<5>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                  SMEM_BYTES),
+                             "cudaFuncSetAttribute(gemm onen smem)");
+    if (rc) return rc;
+    attr_set = true;
+  }
+  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+  if (tiles > 0x7fffffffLL / 8) {
+    rgcn_set_error("gemm_onen_tf32x3: too many tiles");
+    return RGCN_ERR_INVALID;
+  }
+  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
+  k_gemm_tf32x3<5><<<grid, N_THREADS, SMEM_BYTES, st>>>(
+      Q, ldq, Bt_hi, Bt_lo, ldb, nullptr, 0, M, N, K, 0, (int)tiles,
+      BceEpi{labels, (N + 31) / 32, pos, neg, scale, g_scale, Gt, ldgt, loss_part});
+  ++g_rgcn_launches;
+  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<onen>");
 }
 
 int launch_split_trunc(float* a, float* lo, int64_t count, cudaStream_t st) {

@@ -178,6 +178,34 @@ int launch_gemm_ensemble_rank_tf32x3(const float* qa_hi, const float* qa_lo, con
 int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
                           int M, int N, int K, int accumulate, cudaStream_t st);
 
+// 1-N training (onen.cu and the EPI = 5 scoring GEMM).  Loss parts the GEMM writes for M queries and N entities:
+int64_t gemm_onen_loss_parts(int64_t M, int N);
+// For query m and entity n, z = <Q[m], codes[n]>, y' = pos / neg as bit n of labels row m is set / clear:
+// loss_part gets the sums of max(z,0) - z y' + log1p(exp(-|z|)); Gt[n * ldgt + m] = (sigmoid(z) - y') scale g_scale[0]
+// (g_scale null: 1; Gt null: loss only)
+int launch_gemm_onen_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, const float* Bt_lo, int64_t ldb, int M,
+                            int N, int K, const uint32_t* labels, float pos, float neg, float scale,
+                            const float* g_scale, float* Gt, int64_t ldgt, float* loss_part, cudaStream_t st);
+// label rows: bits [n, words] of the queries X[t] = (anchor, r, anchor) of one side from the training CSR (keys sorted,
+// key = (2 r + side) V + anchor; entities of key i at offsets[i] .. offsets[i+1])
+int launch_onen_labels(const int64_t* keys, const int64_t* offsets, const int32_t* entities, int64_t n_keys,
+                       const int32_t* X, int64_t n, int side, int V, int words, uint32_t* bits, cudaStream_t st);
+// reg parts: onen_reg_parts(n) sums of |codes[anchor]|^2 + |rel[r]|^2 over the queries
+int64_t onen_reg_parts(int64_t n);
+int launch_onen_reg(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, float* reg_part,
+                    cudaStream_t st);
+// loss[0] = inv_nv * (sum of the loss parts), loss[1] = inv_nd * (sum of the reg parts), each summed in a fixed order
+int launch_onen_loss_reduce(const float* loss_part, int64_t n_loss, const float* reg_part, int64_t n_reg,
+                            double inv_nv, double inv_nd, float* loss, cudaStream_t st);
+// dst = g_scale[0] src, count % 4 == 0 floats
+int launch_onen_scale(const float* src, const float* g_scale, int64_t count, float* dst, cudaStream_t st);
+// anchor and relation gradients of the queries of one side: from dQ [n, d] and the L2 term c = g_scale[1] 2 / (n_all d)
+// (g_scale null: 1), red.global.add into dcodes[anchor] and drel[r]; complex = 0 DistMult, 1 ComplEx; dQ null (DistMult
+// kernel, either decoder): the L2 term only
+int launch_onen_query_bwd(int complex, const float* codes, const float* rel, int d, const int32_t* X, int64_t n,
+                          int side, const float* dQ, const float* g_scale, float c_reg, float* dcodes, float* drel,
+                          cudaStream_t st);
+
 // Highway gate GEMM with the blend epilogue: gate = sigmoid(c2 W + bias), out = c2 + gate (c1 - c2); W given
 // pre-split as Bt = W^T [d, d]; all [M, d] matrices contiguous
 int launch_gemm_highway_tf32x3(const float* c2, const float* Bt_hi, const float* Bt_lo, const float* bias,

@@ -5,15 +5,41 @@ import torch
 from ..model import Model, Placeholder
 from .. import ops
 
+TRAINING_OBJECTIVES = ('NegativeSampling', '1-N')
+
+
+def parse_training_objective(settings):
+    """(TrainingObjective, LabelSmoothing) of [General]: 'NegativeSampling' (the default: the reference's objective
+    over NegativeSampleRate corruptions per positive) or '1-N' (every query scored against every entity, ops.one_to_n_loss),
+    and the label smoothing eps in [0, 1) of the 1-N targets (default 0)."""
+    objective = str(settings['TrainingObjective']) if 'TrainingObjective' in settings else 'NegativeSampling'
+    if objective not in TRAINING_OBJECTIVES:
+        raise ValueError("TrainingObjective must be one of %s, got %r" % (", ".join(TRAINING_OBJECTIVES), objective))
+    eps = float(settings['LabelSmoothing']) if 'LabelSmoothing' in settings else 0.0
+    if not 0.0 <= eps < 1.0:
+        raise ValueError("LabelSmoothing must be in [0, 1), got %r" % (eps,))
+    return objective, eps
+
 
 class BilinearDiag(Model):
+    ONE_TO_N = "distmult"   # the decoder kind of ops.one_to_n_loss
+
     def __init__(self, next_component, settings):
         self.encoder_cache = {'train': None, 'test': None}
         self._scored = {'train': None, 'test': None}
+        self._one_to_n_loss = None
+        self._one_to_n_feed = None   # (fed X, its queries, their label rows)
+        self.one_to_n_labels = None
         Model.__init__(self, next_component, settings)
 
     def parse_settings(self):
         self.regularization_parameter = float(self.settings['RegularizationParameter'])
+        self.training_objective, self.label_smoothing = parse_training_objective(self.settings)
+
+    def set_one_to_n_labels(self, labels):
+        """The ops.OneToNLabels of the training split, which 1-N training reads its targets from."""
+        self.one_to_n_labels = labels
+        self._one_to_n_feed = None
 
     def local_initialize_train(self):
         self.Y = Placeholder('Y', 'float32', [None])
@@ -22,6 +48,7 @@ class BilinearDiag(Model):
     def local_clear_cache(self):
         self.encoder_cache = {'train': None, 'test': None}
         self._scored = {'train': None, 'test': None}
+        self._one_to_n_loss = None
 
     def local_get_train_input_variables(self):
         return [self.X, self.Y]
@@ -62,10 +89,32 @@ class BilinearDiag(Model):
             self.encoder_cache[mode] = (subject_codes[X[:, 0]], relation_codes[X[:, 1]], object_codes[X[:, 2]])
         return self.encoder_cache[mode]
 
+    def _one_to_n(self):
+        """(loss, reg) of 1-N training: the fed positives X become their de-duplicated object and subject queries,
+        scored against every entity with the training split's label rows (ops.one_to_n_loss)."""
+        if self._one_to_n_loss is None:
+            if self.one_to_n_labels is None:
+                raise RuntimeError("TrainingObjective=1-N needs the training labels: call set_one_to_n_labels first")
+            subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='train')
+            assert subject_codes is object_codes, "1-N training expects one shared entity code matrix"
+            # the queries and label rows of a fed array are kept while the same array is fed again: without a graph
+            # batch the driver feeds the whole training split every step
+            if self._one_to_n_feed is None or self._one_to_n_feed[0] is not self.X.value:
+                queries = ops.one_to_n_queries(np.asarray(self.X.value, dtype=np.int32).reshape(-1, 3))
+                self._one_to_n_feed = (self.X.value, queries, self.one_to_n_labels.rows(queries))
+            _, queries, labels = self._one_to_n_feed
+            self._one_to_n_loss = ops.one_to_n_loss(subject_codes.contiguous(), relation_codes.contiguous(), queries,
+                                                    labels, self.label_smoothing, self.ONE_TO_N, self.relation_count)
+        return self._one_to_n_loss
+
     def get_loss(self, mode='train'):
+        if mode == 'train' and self.training_objective == '1-N':
+            return self._one_to_n()[0]
         return self._fused(mode)[1]  # reduce_mean(weighted CE, pos_weight forced to 1) (:27-34)
 
     def local_get_regularization(self):
+        if self.training_objective == '1-N':
+            return self.regularization_parameter * self._one_to_n()[1]   # L2 of the two rows a query gathers
         return self.regularization_parameter * self._fused('train')[2]  # (:63-69)
 
     def predict(self):

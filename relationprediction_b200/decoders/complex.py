@@ -10,6 +10,8 @@ from .bilinear_diag import BilinearDiag
 
 
 class Complex(BilinearDiag):
+    ONE_TO_N = "complex"
+
     def __init__(self, dimension, settings, next_component=None):
         BilinearDiag.__init__(self, next_component, settings)
         self.dimension = dimension

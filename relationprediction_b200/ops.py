@@ -935,3 +935,136 @@ class EnsembleRanker(object):
         _lib.check(rc, "rgcn_ensemble_rank")
         self._split_ready = True
         return raw, filt
+
+
+# ---- 1-N training (distmult_one_to_n / rgcn_complex_one_to_n, include/rgcn_b200.h) ----
+ONE_TO_N_DECODERS = {"distmult": "distmult_one_to_n", "complex": "rgcn_complex_one_to_n"}
+# device bytes of the per-query buffers (energy gradients Gt [V, chunk], query rows and their gradients) of one
+# internal pass; more queries than fit run in several passes of one call
+ONE_TO_N_CHUNK_BYTES = 1 << 30
+
+
+def one_to_n_queries(triples):
+    """The de-duplicated 1-N queries of positive triples [m, 3]: (s, r, 1) asks for the objects of (s, r, ?) and
+    (o, r, 0) for the subjects of (?, r, o).  int32 [n, 3] rows (anchor, relation, side), sorted by (side, relation,
+    anchor): all subject queries first.  The rows are de-duplicated as the 1-D keys (side R' + r) V' + anchor
+    (V', R' one past the largest ids): one sort of int64 keys, far faster than a de-duplication of rows."""
+    tri = np.asarray(triples, dtype=np.int64).reshape(-1, 3)
+    if len(tri) == 0:
+        return np.zeros((0, 3), np.int32)
+    V, R = int(max(tri[:, 0].max(), tri[:, 2].max())) + 1, int(tri[:, 1].max()) + 1
+    keys = np.sort(np.concatenate([tri[:, 1] * V + tri[:, 2], (R + tri[:, 1]) * V + tri[:, 0]]))
+    keys = keys[np.concatenate([[True], keys[1:] != keys[:-1]])]
+    q = np.empty((len(keys), 3), np.int32)
+    q[:, 0] = keys % V
+    q[:, 1] = (keys // V) % R
+    q[:, 2] = keys // (V * R)
+    return q
+
+
+def _check_queries(queries, V, R):
+    q = np.ascontiguousarray(np.asarray(queries, dtype=np.int32).reshape(-1, 3))
+    if len(q) and (q[:, 0].min() < 0 or q[:, 0].max() >= V or q[:, 1].min() < 0 or q[:, 1].max() >= R
+                   or not np.isin(q[:, 2], (0, 1)).all()):
+        raise ValueError("1-N queries need 0 <= anchor < %d, 0 <= relation < %d and side in {0, 1}" % (V, R))
+    return q
+
+
+class OneToNLabels(object):
+    """The 1-N targets of a training split on the device: a CSR from the query key (2 relation + side) V + anchor to
+    the entities that complete a training triple, built once; rows(queries) writes the [n, ceil(V/32)] label bits of a
+    step with one library call (rgcn_one_to_n_labels)."""
+
+    def __init__(self, triples, n_entities, n_relations, device):
+        tri = np.asarray(triples, dtype=np.int64).reshape(-1, 3)
+        V = self.V = int(n_entities)
+        self.R = int(n_relations)
+        if len(tri) and (tri[:, [0, 2]].min() < 0 or tri[:, [0, 2]].max() >= V or tri[:, 1].min() < 0
+                         or tri[:, 1].max() >= self.R):
+            raise ValueError("OneToNLabels: training triples need entity ids in [0, %d) and relation ids in [0, %d)"
+                             % (V, self.R))
+        s, r, o = tri[:, 0], tri[:, 1], tri[:, 2]
+        # (query key, entity) pairs as one sorted, de-duplicated int64 key V + entity
+        pairs = np.sort(np.concatenate([((2 * r + 1) * V + s) * V + o, ((2 * r) * V + o) * V + s]))
+        pairs = pairs[np.concatenate([[True], pairs[1:] != pairs[:-1]])]
+        qkey, ent = pairs // V, pairs % V
+        starts = np.flatnonzero(np.concatenate([[True], qkey[1:] != qkey[:-1]]))
+        dev = torch.device(device)
+        self.keys = torch.as_tensor(qkey[starts].astype(np.int64), device=dev)
+        self.offsets = torch.as_tensor(np.append(starts, len(pairs)).astype(np.int64), device=dev)
+        self.entities = torch.as_tensor(ent.astype(np.int32), device=dev)
+        self.device = dev
+
+    def rows(self, queries):
+        """uint32 label bits [n, ceil(V/32)] (as int32) of host queries (anchor, relation, side): bit e of an object
+        query (s, r, 1) is set iff (s, r, e) is a training triple, of a subject query (o, r, 0) iff (e, r, o) is."""
+        q = _check_queries(queries, self.V, self.R)
+        bits = torch.empty(len(q), (self.V + 31) // 32, dtype=torch.int32, device=self.device)
+        _call("rgcn_one_to_n_labels", "rgcn_one_to_n_labels_workspace_bytes", (len(q),),
+              (_ptr(self.keys), _ptr(self.offsets), _ptr(self.entities), self.keys.numel(), self.V, self.R,
+               _np_ptr(q), len(q), _ptr(bits)), self.device)
+        return bits
+
+
+class _OneToNFn(torch.autograd.Function):
+    """Returns (loss, reg) of distmult_one_to_n / rgcn_complex_one_to_n.  When codes or rel need a gradient, the forward
+    also writes the gradient of the loss alone (g_scale = (1, 0)); the gradient is linear in the two upstream scalars,
+    so the backward is rgcn_one_to_n_finish: one scaling pass and the L2 term, no GEMM."""
+
+    @staticmethod
+    def forward(ctx, codes, rel, labels, queries, smoothing, entry, R, chunk, grads):
+        V, d = codes.shape
+        dev = codes.device
+        loss = torch.empty(2, dtype=torch.float32, device=dev)
+        dcodes = torch.empty_like(codes) if grads else None
+        drel = torch.empty_like(rel) if grads else None
+        g_loss_only = torch.tensor([1.0, 0.0], dtype=torch.float32, device=dev) if grads else None
+        _call(entry, "rgcn_one_to_n_workspace_bytes", (V, d, len(queries), chunk),
+              (_ptr(codes), _ptr(rel), V, rel.shape[0], R, d, _np_ptr(queries), len(queries), _ptr(labels),
+               smoothing, _ptr(g_loss_only), _ptr(loss), _ptr(dcodes), _ptr(drel), chunk), dev)
+        ctx.args = (queries, R)
+        if grads:
+            ctx.save_for_backward(codes, rel, dcodes, drel)
+        return loss[0], loss[1]
+
+    @staticmethod
+    def backward(ctx, g_loss, g_reg):
+        codes, rel, dcodes_loss, drel_loss = ctx.saved_tensors
+        queries, R = ctx.args
+        V, d = codes.shape
+        dev = codes.device
+        gs = torch.zeros(2, dtype=torch.float32, device=dev)
+        if g_loss is not None:
+            gs[0] = g_loss
+        if g_reg is not None:
+            gs[1] = g_reg
+        dcodes, drel = torch.empty_like(codes), torch.empty_like(rel)
+        _call("rgcn_one_to_n_finish", "rgcn_one_to_n_finish_workspace_bytes", (len(queries),),
+              (_ptr(codes), _ptr(rel), V, rel.shape[0], R, d, _np_ptr(queries), len(queries), _ptr(gs),
+               _ptr(dcodes_loss), _ptr(drel_loss), _ptr(dcodes), _ptr(drel)), dev)
+        return dcodes, drel, None, None, None, None, None, None, None
+
+
+def one_to_n_loss(codes, rel, queries, labels, smoothing, decoder, relation_count=None):
+    """1-N loss of host queries (anchor, relation, side) int32 [n, 3] against every entity, with the label bits of
+    OneToNLabels.rows and label smoothing eps in [0, 1): returns (loss, reg), loss = the mean over the n V scores of the
+    sigmoid cross-entropy against y' = (1 - eps) y + eps / V, reg = (|codes[anchor]|^2 + |rel[r]|^2) / (n d) summed
+    over the queries (the decoders' un-scaled L2 term).  decoder is "distmult" or "complex"; the relation ids must be
+    below relation_count (default: all rows of rel).  Differentiable in codes and rel."""
+    if decoder not in ONE_TO_N_DECODERS:
+        raise ValueError("one_to_n_loss: decoder must be one of %s, got %r" % (sorted(ONE_TO_N_DECODERS), decoder))
+    _check_cuda_f32("codes", codes)
+    _check_cuda_f32("relation table", rel)
+    V, d = codes.shape
+    R = rel.shape[0] if relation_count is None else int(relation_count)
+    q = _check_queries(queries, V, R)
+    words = (V + 31) // 32
+    if not (labels.is_cuda and labels.dtype == torch.int32 and labels.is_contiguous()
+            and tuple(labels.shape) == (len(q), words)):
+        raise _lib.RgcnError("labels must be a contiguous CUDA int32 [n, ceil(V/32)] tensor (bit rows)")
+    if not 0.0 <= float(smoothing) < 1.0:
+        raise ValueError("one_to_n_loss: label smoothing must be in [0, 1), got %r" % (smoothing,))
+    chunk = max(1, min(len(q), ONE_TO_N_CHUNK_BYTES // ((V + 4 * d) * 4)))
+    # inside Function.forward the grad mode is off and needs_input_grad ignores torch.no_grad(): decide here
+    grads = torch.is_grad_enabled() and (codes.requires_grad or rel.requires_grad)
+    return _OneToNFn.apply(codes, rel, labels, q, float(smoothing), ONE_TO_N_DECODERS[decoder], R, chunk, grads)

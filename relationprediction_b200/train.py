@@ -297,13 +297,28 @@ def main(argv=None):
     if encoder.needs_graph() and 'GraphBatchSize' in general and int(general['GraphBatchSize']) < len(train):
         edge_sampler = EdgeNeighborhoodSampler(train, len(entities))
 
+    # 1-N training: the step's positives are fed as X (an empty Y) and become their object and subject queries;
+    # the targets come from the training split's label CSR, built here once.  No negative is drawn.
+    one_to_n = model.training_objective == '1-N'
+    if one_to_n:
+        from . import ops
+        model.set_one_to_n_labels(ops.OneToNLabels(train, len(entities), len(relations), args.device))
+        print("Training objective: 1-N, label smoothing %g" % model.label_smoothing)
+    no_y = np.zeros(0, dtype=np.float32)
+
     def sample():
         if not encoder.needs_graph():
+            if one_to_n:
+                return (train, no_y)
             X, Y = ns.transform(train)
             return (X, Y)
         if edge_sampler is not None and not args.numpy_sampling:
             gbs = int(general['GraphBatchSize'])   # the whole sample in one library call (no interpreter lock held)
-            return edge_sampler.draw_batch(gbs, int(float(general['GraphSplitSize']) * gbs), ns.negative_sample_rate)
+            split = int(float(general['GraphSplitSize']) * gbs)
+            if one_to_n:   # rate 0: X is the batch itself
+                graph_split, X, _ = edge_sampler.draw_batch(gbs, split, 0)
+                return (graph_split, X, no_y)
+            return edge_sampler.draw_batch(gbs, split, ns.negative_sample_rate)
         if 'GraphBatchSize' in general and int(general['GraphBatchSize']) < len(train):
             ids = edge_sampler.draw(int(general['GraphBatchSize']))
         else:
@@ -311,6 +326,8 @@ def main(argv=None):
         graph_batch = train[ids]
         split = int(float(general['GraphSplitSize']) * len(graph_batch))
         graph_split = train[np.random.choice(ids, size=split, replace=False)]
+        if one_to_n:
+            return (graph_split, graph_batch, no_y)
         X, Y = ns.transform(graph_batch)
         return (graph_split, X, Y)
 
