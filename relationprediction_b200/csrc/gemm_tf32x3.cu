@@ -9,22 +9,31 @@
 // cvt.rna.tf32.f32) and three MMAs are issued per K-step:  a_hi*b_hi + a_hi*b_lo + a_lo*b_hi
 // (the a_lo*b_lo term is below fp32 rounding).
 //
-// Both kernels: 384 threads = three warpgroups, 1 CTA/SM, 128x128 tiles, 32-wide K blocks.
+// Three kernels (k_gemm_tf32x3<EPI>, k_gemm_tn_tf32x3, k_gemm_ensemble_rank): 384 threads = three warpgroups,
+// 1 CTA/SM, 128-row tiles, 32-wide K blocks.
 //   warpgroup 0     producer: global fp32 -> registers -> (hi, lo) -> st.shared in the K-major SWIZZLE_128B layout
 //                   that wgmma reads (TF32 wgmma takes K-major operands only, so the TN kernel transposes here);
-//                   cp.async of the pre-split Bt_hi / Bt_lo tiles (NT kernel); fence.proxy.async + mbarrier arrive.
-//   warpgroups 1-2  consumers: rows 0-63 / 64-127 of the tile.  Per K block 4 K-steps x 3 wgmma.m64n128k8.tf32
-//                   into two register accumulators (hi*hi; the two cross terms), then the stage is released.  The
-//                   epilogue works straight from the accumulator registers.
-//   3-stage smem ring (64 KB per stage: A_hi, A_lo, B_hi, B_lo); the TN kernel has 2 stages plus a ring of raw fp32
-//   blocks that its producer fills with cp.async and transposes from (see k_gemm_tn_tf32x3).
-// The NT kernel is persistent (min(tiles, SMs) CTAs walk the tiles; the producer runs on into the next tile while
-// the consumers finish the last one); the TN kernel keeps one tile (x split-K) per CTA.
+//                   cp.async of the pre-split Bt_hi / Bt_lo tiles (NT kernel; the ensemble kernel gets both
+//                   operands pre-split and only copies); fence.proxy.async + mbarrier arrive.
+//   warpgroups 1-2  consumers: rows 0-63 / 64-127 of the tile.  Per K block 4 K-steps x 3 wgmma.m64nNk8.tf32
+//                   into two register accumulators (hi*hi; the two cross terms), then the stage is released
+//                   (consume_tile, the one K loop of all three kernels).  The epilogue works straight from the
+//                   accumulator registers.
+//   NT: 128x128 tiles, 3-stage smem ring (64 KB per stage: A_hi, A_lo, B_hi, B_lo); TN: 2 such stages plus a ring of
+//   raw fp32 blocks that its producer fills with cp.async and transposes from (see k_gemm_tn_tf32x3); ensemble:
+//   128x64 tiles, 4 stages of 48 KB (see k_gemm_ensemble_rank).
+// The NT and ensemble kernels are persistent (min(tiles, SMs) CTAs walk the tiles; the producer runs on into the next
+// tile while the consumers finish the last one); the TN kernel keeps one tile (x split-K) per CTA.
+//
+// The epilogues of the NT kernel are functors (StoreEpi, RankEpi, HighwayEpi, VarEpi, TopKEpi, BceEpi): a struct with
+// the epilogue's data and one operator()(tile, big, small) over the accumulator fragment.  Epilogue<EPI> maps the
+// integer of k_gemm_tf32x3<EPI> to its functor (EPI_STORE = 0 .. EPI_BCE = 5).  A new epilogue is one such struct, one
+// Epilogue<n> line and one launcher that ends in launch_persistent.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
-#include <cstdlib>
+#include <string>
 
 #include "kernels.cuh"
 
@@ -32,8 +41,18 @@ namespace {
 
 constexpr int BM = 128, BN = 128, BK = 32;  // BK floats = 128 bytes = one swizzle row
 constexpr int STAGES = 3;
-constexpr int TILE_BYTES = BM * BK * 4;     // 16 KB (A_hi, A_lo, B_hi, B_lo each)
-constexpr int STAGE_BYTES = 4 * TILE_BYTES; // 64 KB
+// One stage of a shared-memory ring of NST stages: the hi and lo planes of 128 A rows, then those of TBN B rows
+template <int NST, int TBN>
+struct StageShape {
+  static constexpr int STAGE_COUNT = NST;
+  static constexpr int A_PLANE = BM * BK * 4;              // bytes of A_hi (= A_lo)
+  static constexpr int B_PLANE = TBN * BK * 4;             // bytes of B_hi (= B_lo)
+  static constexpr int BYTES = 2 * A_PLANE + 2 * B_PLANE;
+  static constexpr int FRAG = TBN / 2;                     // accumulator registers per thread and array
+};
+using NtStage = StageShape<STAGES, BN>;
+constexpr int TILE_BYTES = NtStage::A_PLANE;   // 16 KB (A_hi, A_lo, B_hi, B_lo each)
+constexpr int STAGE_BYTES = NtStage::BYTES;    // 64 KB
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024;  // + alignment slack
 constexpr int N_PRODUCERS = 128;            // one producer warpgroup
 constexpr int N_CONSUMERS = 256;            // two consumer warpgroups, 64 tile rows each
@@ -77,7 +96,7 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
 }
 
 // d[64 rows of this warpgroup x 128] (+)= A(desc) * B(desc)^T, TF32 inputs, fp32 accumulators
-__device__ __forceinline__ void wgmma_tf32(float (&d)[N_FRAG], uint64_t da, uint64_t db, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t"
       ".reg .pred p;\n\t"
@@ -99,10 +118,29 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[N_FRAG], uint64_t da, uint
       : "l"(da), "l"(db), "r"(accumulate)
       : "memory");
 }
+// the same for a 64-column tile: d[64 rows of this warpgroup x 64]
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+      "%23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(accumulate)
+      : "memory");
+}
 // keeps the compiler from touching the accumulators while wgmma owns them
-__device__ __forceinline__ void fence_acc(float (&d)[N_FRAG]) {
+template <int NF>
+__device__ __forceinline__ void fence_acc(float (&d)[NF]) {
 #pragma unroll
-  for (int i = 0; i < N_FRAG; ++i) asm volatile("" : "+f"(d[i])::"memory");
+  for (int i = 0; i < NF; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // Producer-side split by TRUNCATION: hi = a with the 13 low mantissa bits cleared, lo = (a - hi) (exact in fp32) with
@@ -138,17 +176,18 @@ __device__ __forceinline__ void init_barriers(uint64_t* full_bar, uint64_t* empt
 // The K loop of one tile for one consumer warpgroup: k-blocks g0 .. g0 + num_kb - 1 of the CTA's stage sequence.
 // The hi*hi products and the cross terms go to separate accumulators (the tensor core adds into its accumulator
 // with truncation; same-magnitude additions per accumulator keep the result at SGEMM-level accuracy) and are summed
-// in fp32 in the epilogue.  NST: stages in the ring.
-template <int NST = STAGES>
+// in fp32 in the epilogue.  S: the StageShape of the kernel's ring.  Every output element of every kernel sees its
+// K steps in this order, which is what makes the ensemble kernel reproduce the single-model ranks at w = 0 and 1.
+template <class S>
 __device__ __forceinline__ void consume_tile(uint32_t smem_base, uint64_t* full_bar, uint64_t* empty_bar, int g0,
-                                             int num_kb, uint32_t a_rows, float (&big)[N_FRAG],
-                                             float (&small)[N_FRAG]) {
+                                             int num_kb, uint32_t a_rows, float (&big)[S::FRAG],
+                                             float (&small)[S::FRAG]) {
   for (int kb = 0; kb < num_kb; ++kb) {
     const int g = g0 + kb;
-    const int s = g % NST;
-    mbar_wait(&full_bar[s], (uint32_t)(g / NST) & 1u);
-    const uint32_t a_hi = smem_base + s * STAGE_BYTES + a_rows, a_lo = a_hi + TILE_BYTES;
-    const uint32_t b_hi = smem_base + s * STAGE_BYTES + 2 * TILE_BYTES, b_lo = b_hi + TILE_BYTES;
+    const int s = g % S::STAGE_COUNT;
+    mbar_wait(&full_bar[s], (uint32_t)(g / S::STAGE_COUNT) & 1u);
+    const uint32_t a_hi = smem_base + s * S::BYTES + a_rows, a_lo = a_hi + S::A_PLANE;
+    const uint32_t b_hi = smem_base + s * S::BYTES + 2 * S::A_PLANE, b_lo = b_hi + S::B_PLANE;
     asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
     for (int kk = 0; kk < BK / 8; ++kk) {
@@ -167,6 +206,101 @@ __device__ __forceinline__ void consume_tile(uint32_t smem_base, uint64_t* full_
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// The accumulator fragment of wgmma m64nN, as every epilogue sees it: register 4j + 2h + e of a consumer thread holds
+// row 16 * (warp % 4) + lane / 4 + 8 h and column 8 j + 2 (lane % 4) + e of the warpgroup's 64 x N block.  TileCtx
+// gives the thread's place in the output: its rows are r0 and r0 + 8, its columns c0 + 8 j + e.
+// ------------------------------------------------------------------------------------------------
+struct TileCtx {
+  int tile;        // index in the kernel's tile order (N tiles fastest)
+  int m0, n0;      // first row and column of the tile
+  int r0, c0;      // this thread's row (h = 0) and its first column
+  int M, N;
+  int lane, warp;  // warp: 0..7 over the two consumer warpgroups
+};
+
+// Element walk of row r0 + 8 h over a fragment of NF registers: fn(reg, i, col, word) for the thread's i-th column
+// (i = 2 j + e, columns increasing with i) held in register reg; col_bit(word, col) is bit `col` of row r0 + 8 h of
+// the bitmap `bits` ([M, words], one 32-bit word loaded per 32 columns; 0 when bits is null).  Rows >= M and columns
+// >= N are visited too (with word 0): the caller decides what they mean.  The callers take the bit where they use it:
+// handing it over as a value costs the top-k epilogue 250 instructions per tile.
+__device__ __forceinline__ uint32_t col_bit(uint32_t word, int col) { return (word >> (col & 31)) & 1u; }
+template <int NF, class Fn>
+__device__ __forceinline__ void for_each_col(const TileCtx& t, int h, const uint32_t* bits, int words, Fn fn) {
+  const int row = t.r0 + 8 * h;
+#pragma unroll
+  for (int cb = 0; cb < NF / 16; ++cb) {
+    const int chunk = t.n0 + 32 * cb;
+    const uint32_t w =
+        (bits && row < t.M && chunk < t.N) ? __ldg(bits + (size_t)row * words + (chunk >> 5)) : 0u;
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int j = 4 * cb + jj, col = t.c0 + 8 * j + e;
+        fn(4 * j + 2 * h + e, 2 * j + e, col, w);
+      }
+    }
+  }
+}
+// Pair walk of row r0 + 8 h for the float2 epilogues: fn(reg, col) for every pair of columns (col, col + 1) < N held
+// in registers (reg, reg + 1); col is even.  N % 2 == 0, so both columns of a pair exist or neither does.
+template <class Fn>
+__device__ __forceinline__ void for_each_pair(const TileCtx& t, int h, Fn fn) {
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = t.c0 + 8 * j;
+    if (col < t.N) fn(4 * j + 2 * h, col);
+  }
+}
+// The rank counts of one row: the four lanes of a quad hold the row's columns; their counts are summed by two
+// shuffles and added to the row's totals (integer atomics: the totals do not depend on the order of the tiles).
+__device__ __forceinline__ void rank_counts_flush(int raw, int kn, int row, int M, int32_t* raw_cnt,
+                                                  int32_t* known_cnt, int lane) {
+  raw += __shfl_xor_sync(0xffffffffu, raw, 1);
+  raw += __shfl_xor_sync(0xffffffffu, raw, 2);
+  kn += __shfl_xor_sync(0xffffffffu, kn, 1);
+  kn += __shfl_xor_sync(0xffffffffu, kn, 2);
+  if ((lane & 3) == 0 && row < M) {
+    if (raw) atomicAdd(raw_cnt + row, raw);
+    if (kn) atomicAdd(known_cnt + row, kn);
+  }
+}
+// part[tile * 8 + warp] = the sum of x over the warp, by a shuffle tree in a fixed order: a sum reduced from the
+// parts is bitwise repeatable
+__device__ __forceinline__ void warp_part_store(float x, float* part, const TileCtx& t) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  if (t.lane == 0) part[(size_t)t.tile * 8 + t.warp] = x;
+}
+__device__ __forceinline__ float sigmoid_ref(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+// EPI = 0: STORE epilogue: C[M, N] = or += the tile.
+struct StoreEpi {
+  float* C;                    // [M, ldc]
+  int64_t ldc;
+  int accumulate;              // C += instead of C =
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const float (&big)[N_FRAG],
+                                             const float (&small)[N_FRAG]) const {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = t.r0 + 8 * h;
+      if (row >= t.M) continue;
+      float* crow = C + (size_t)row * ldc;
+      for_each_pair(t, h, [&](int r, int col) {
+        float2 o = make_float2(big[r] + small[r], big[r + 1] + small[r + 1]);
+        if (accumulate) {
+          const float2 old = *reinterpret_cast<const float2*>(crow + col);
+          o.x += old.x;
+          o.y += old.y;
+        }
+        *reinterpret_cast<float2*>(crow + col) = o;
+      });
+    }
+  }
+};
+
 // EPI = 1: RANKING epilogue (all-entity scoring of the DistMult decoder, decoders/bilinear_diag.py:51-61, fused with
 // the rank counts of common/evaluation.py:148-159): the C tile is never written.  Row m of A is a query (e1*r or r*e2),
 // row n of Bt an entity code; each energy goes through the reference's float32 sigmoid and is compared with the gold
@@ -179,22 +313,69 @@ struct RankEpi {
   int words;                   // ceil(N / 32)
   int32_t* raw_cnt;            // [M] += #{v : score_v >= gold}
   int32_t* known_cnt;          // [M] += #{known v : score_v >= gold}
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const float (&big)[N_FRAG],
+                                             const float (&small)[N_FRAG]) const {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = t.r0 + 8 * h;
+      int raw = 0, kn = 0;
+      if (row < t.M) {
+        const float gold_s = __ldg(gold_sig + row);
+        const int gold_c = __ldg(gold_col + row);
+        for_each_col<N_FRAG>(t, h, known, words, [&](int r, int, int col, uint32_t word) {
+          // the gold entity always scores >= itself
+          if (col < t.N && (sigmoid_ref(big[r] + small[r]) >= gold_s || col == gold_c)) {
+            ++raw;
+            kn += (int)col_bit(word, col);
+          }
+        });
+      }
+      rank_counts_flush(raw, kn, row, t.M, raw_cnt, known_cnt, t.lane);
+    }
+  }
 };
-__device__ __forceinline__ float sigmoid_ref(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // EPI = 2: HIGHWAY epilogue (the gate of extras/highway_layer.py:19-38): A = c2 [M, K = N] is the layer input, Bt the
 // gate weight W^T, and each accumulator pair becomes  z = acc + bias[col],  g = sigmoid(z),
-// out = c2 + g (c1 - c2)  (= g c1 + (1 - g) c2), written to C together with g (kept for the backward pass).  z itself
-// is never stored.  c1, C and gate share the leading dimension ldc; c2 is read through A with lda.
+// out = c2 + g (c1 - c2)  (= g c1 + (1 - g) c2), written to `out` together with g (kept for the backward pass).  z
+// itself is never stored.  c1, c2, out and gate share the leading dimension ld.
 struct HighwayEpi {
   const float* bias;           // [N]
-  const float* c1;             // [M, ldc] the wrapped layer's output
-  float* gate;                 // [M, ldc] g
+  const float* c1;             // [M, ld] the wrapped layer's output
+  const float* c2;             // [M, ld] the layer input (the GEMM's A)
+  float* out;                  // [M, ld]
+  float* gate;                 // [M, ld] g
+  int64_t ld;
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const float (&big)[N_FRAG],
+                                             const float (&small)[N_FRAG]) const {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = t.r0 + 8 * h;
+      if (row >= t.M) continue;
+      const float* c2row = c2 + (size_t)row * ld;
+      const float* c1row = c1 + (size_t)row * ld;
+      float* orow = out + (size_t)row * ld;
+      float* grow = gate + (size_t)row * ld;
+      asm volatile("" : "+l"(c2row), "+l"(c1row));   // no hoisting of the 16 pairs' loads ahead of use (spills)
+      for_each_pair(t, h, [&](int r, int col) {
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
+        const float2 x1 = __ldg(reinterpret_cast<const float2*>(c1row + col));
+        const float2 x2 = __ldg(reinterpret_cast<const float2*>(c2row + col));
+        const float g0 = sigmoid_ref(big[r] + small[r] + bb.x);
+        const float g1 = sigmoid_ref(big[r + 1] + small[r + 1] + bb.y);
+        *reinterpret_cast<float2*>(orow + col) = make_float2(x2.x + g0 * (x1.x - x2.x), x2.y + g1 * (x1.y - x2.y));
+        *reinterpret_cast<float2*>(grow + col) = make_float2(g0, g1);
+      });
+    }
+  }
 };
+
 // EPI = 3: VARIATIONAL epilogue (extras/variational_encoding.py:14-31): A = H [M, K], Bt the pre-split W_int^T whose
 // rows interleave the columns of W_mu and W_sigma (row 2j = W_mu[:, j], row 2j + 1 = W_sigma[:, j]), so each
 // accumulator pair (col, col + 1) = (2j, 2j + 1) is the (mu, log sigma) of element (row, j):
-//   mu = acc + b_mu[j],  l = acc' + b_sigma[j],  P[row, 2j .. 2j+1] = (mu, l)  (C, kept for the backward pass),
+//   mu = acc + b_mu[j],  l = acc' + b_sigma[j],  P[row, 2j .. 2j+1] = (mu, l)  (kept for the backward pass),
 //   z[row, j] = mu + exp(l) eps[row, j],
 // and every consumer warp writes kl_part[tile * 8 + warp] = sum of (1 + 2 l - mu^2 - exp(2 l)) over its elements,
 // summed in a fixed order (per thread, then a shuffle tree), so the KL reduced from the parts is bitwise repeatable.
@@ -202,10 +383,36 @@ struct VarEpi {
   const float* b_mu;           // [w]
   const float* b_sigma;        // [w]
   const float* eps;            // [M, w]
+  float* P;                    // [M, ldp] (mu, log sigma) interleaved, N = 2 w columns
+  int64_t ldp;
   float* z;                    // [M, w]
   float* kl_part;              // [tiles * 8]
   int w;
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const float (&big)[N_FRAG],
+                                             const float (&small)[N_FRAG]) const {
+    float kl = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = t.r0 + 8 * h;
+      if (row >= t.M) continue;
+      float* prow = P + (size_t)row * ldp;
+      const float* erow = eps + (size_t)row * w;
+      float* zrow = z + (size_t)row * w;
+      asm volatile("" : "+l"(erow), "+l"(zrow));   // no hoisting of the 16 pairs' loads ahead of use (spills)
+      for_each_pair(t, h, [&](int r, int col) {   // the pair is (mu, log sigma) of element col / 2
+        const int e = col >> 1;
+        const float mu = big[r] + small[r] + __ldg(b_mu + e);
+        const float ls = big[r + 1] + small[r + 1] + __ldg(b_sigma + e);
+        *reinterpret_cast<float2*>(prow + col) = make_float2(mu, ls);
+        zrow[e] = mu + expf(ls) * __ldg(erow + e);
+        kl += 1.f + 2.f * ls - mu * mu - expf(2.f * ls);
+      });
+    }
+    warp_part_store(kl, kl_part, t);
+  }
 };
+
 // EPI = 4: TOP-K epilogue (filtered top-k prediction over all entities, decoders/bilinear_diag.py:51-61 and
 // complex.py:77-106 without the [M, N] score matrix): row m of A is a query, row n of Bt an entity code.  For each
 // row the tile's best k eligible (energy, column) pairs -- energy descending, smaller column first on ties; columns
@@ -217,14 +424,81 @@ struct TopKEpi {
   int k;                       // candidates per row and tile, 1 <= k <= BN
   int tn;                      // N tiles
   uint2* cand;                 // [M, tn, k] (energy bits, column)
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const float (&big)[N_FRAG],
+                                             const float (&small)[N_FRAG]) const {
+    // The quad of lanes lane & ~3 holds rows r0 and r0 + 8 of the tile: 32 columns each per lane, value i
+    // (= 2 j + e) at column c0 + 8 j + e, so a lane's columns increase with i.  k rounds per row: every lane
+    // takes its best value not yet taken (strict > in i order: the smaller column wins a tie), the quad keeps
+    // the best of the four by two shuffles on (energy, column), and the lane that owned it marks it taken.
+    const int r0 = t.r0, c0 = t.c0, M = t.M;
+    float v[2][32];
+    uint32_t left[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      left[h] = 0u;
+      for_each_col<N_FRAG>(t, h, excl, words, [&](int r, int i, int col, uint32_t word) {
+        v[h][i] = big[r] + small[r];
+        if (r0 + 8 * h < M && col < t.N && !col_bit(word, col)) left[h] |= 1u << i;
+      });
+    }
+    // candidate p of row r0 + 8 h (formed at the store: a live pointer pair would spill)
+    auto slot = [&](int h, int p) { return cand + ((size_t)(r0 + 8 * h) * tn + (size_t)(t.n0 / BN)) * k + p; };
+    const bool writer = (t.lane & 3) == 0;
+    const uint2 none = make_uint2(__float_as_uint(-INFINITY), 0xffffffffu);
+    int p = 0;
+    for (; p < k; ++p) {
+      float be[2];
+      int bc[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        int bi = -1;
+        be[h] = -INFINITY;
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if (((left[h] >> i) & 1u) && (bi < 0 || v[h][i] > be[h])) {
+            be[h] = v[h][i];
+            bi = i;
+          }
+        const int mine = bi < 0 ? 0x7fffffff : c0 + 8 * (bi >> 1) + (bi & 1);
+        bc[h] = mine;
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          const float oe = __shfl_xor_sync(0xffffffffu, be[h], o);
+          const int oc = __shfl_xor_sync(0xffffffffu, bc[h], o);
+          if (oc != 0x7fffffff && (bc[h] == 0x7fffffff || oe > be[h] || (oe == be[h] && oc < bc[h]))) {
+            be[h] = oe;
+            bc[h] = oc;
+          }
+        }
+        if (bi >= 0 && bc[h] == mine) left[h] &= ~(1u << bi);
+      }
+      if (!__any_sync(0xffffffffu, bc[0] != 0x7fffffff || bc[1] != 0x7fffffff)) break;   // the warp's rows ran dry
+      if (writer) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (r0 + 8 * h < M)
+            *slot(h, p) = bc[h] == 0x7fffffff ? none : make_uint2(__float_as_uint(be[h]), (uint32_t)bc[h]);
+      }
+    }
+    if (writer) {
+      for (; p < k; ++p) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          if (r0 + 8 * h < M) *slot(h, p) = none;
+      }
+    }
+  }
 };
+
 // EPI = 5: 1-N BCE epilogue (1-N training of DistMult / ComplEx): row m of A is a query, row n of Bt an entity code,
 // z the energy.  With y' = pos if bit n of labels row m is set, else neg (the smoothed targets),
 //   loss term  max(z, 0) - z y' + log1p(exp(-|z|)),   g = (sigmoid(z) - y') * scale * g_scale[0]
 // and g is written TRANSPOSED, Gt[n * ldgt + m] (a warp's store covers 4 columns x 8 consecutive rows: whole 32 B
-// sectors when ldgt % 8 == 0, as the caller pads it), so that the backward GEMMs read Gt with the contraction index contiguous.  Columns >= N and rows >= M
-// are never written.  Every consumer warp writes loss_part[tile * 8 + warp] = the sum of its loss terms (per thread in
-// a fixed order, then a shuffle tree), so the loss reduced from the parts is bitwise repeatable.
+// sectors when ldgt % 8 == 0, as the caller pads it), so that the backward GEMMs read Gt with the contraction index
+// contiguous.  Columns >= N and rows >= M are never written.  Every consumer warp writes loss_part[tile * 8 + warp] =
+// the sum of its loss terms (per thread in a fixed order, then a shuffle tree), so the loss reduced from the parts is
+// bitwise repeatable.
 struct BceEpi {
   const uint32_t* labels;      // [M, words] bit n = entity n completes query m in the training split
   int words;                   // ceil(N / 32)
@@ -234,27 +508,39 @@ struct BceEpi {
   float* Gt;                   // [N, ldgt] or nullptr: loss only
   int64_t ldgt;
   float* loss_part;            // [tiles * 8]
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const float (&big)[N_FRAG],
+                                             const float (&small)[N_FRAG]) const {
+    const float gs = scale * (g_scale ? __ldg(g_scale) : 1.f);
+    float ls = 0.f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = t.r0 + 8 * h;
+      if (row >= t.M) continue;
+      for_each_col<N_FRAG>(t, h, labels, words, [&](int r, int, int col, uint32_t word) {
+        if (col < t.N) {
+          const float z = big[r] + small[r];
+          const float y = col_bit(word, col) ? pos : neg;
+          ls += fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));
+          if (Gt) Gt[(size_t)col * ldgt + row] = (1.0f / (1.0f + expf(-z)) - y) * gs;
+        }
+      });
+    }
+    warp_part_store(ls, loss_part, t);
+  }
 };
+
+// k_gemm_tf32x3<EPI> runs the epilogue Epilogue<EPI>::type.  There is no primary definition: an integer without a
+// line here does not compile.
+enum : int { EPI_STORE = 0, EPI_RANK = 1, EPI_HIGHWAY = 2, EPI_VAR = 3, EPI_TOPK = 4, EPI_BCE = 5 };
 template <int EPI>
-struct EpiArgs {
-  using type = RankEpi;
-};
-template <>
-struct EpiArgs<5> {
-  using type = BceEpi;
-};
-template <>
-struct EpiArgs<2> {
-  using type = HighwayEpi;
-};
-template <>
-struct EpiArgs<3> {
-  using type = VarEpi;
-};
-template <>
-struct EpiArgs<4> {
-  using type = TopKEpi;
-};
+struct Epilogue;
+template <> struct Epilogue<EPI_STORE> { using type = StoreEpi; };
+template <> struct Epilogue<EPI_RANK> { using type = RankEpi; };
+template <> struct Epilogue<EPI_HIGHWAY> { using type = HighwayEpi; };
+template <> struct Epilogue<EPI_VAR> { using type = VarEpi; };
+template <> struct Epilogue<EPI_TOPK> { using type = TopKEpi; };
+template <> struct Epilogue<EPI_BCE> { using type = BceEpi; };
 
 // PERSISTENT: a CTA walks the tiles blockIdx.x, blockIdx.x + gridDim.x, ... (N tiles fastest, see below); the
 // shared-memory stages and their barrier phases run on across tile boundaries, so the producer fills the pipeline of
@@ -262,8 +548,8 @@ struct EpiArgs<4> {
 template <int EPI>
 __global__ void __launch_bounds__(N_THREADS, 1)
     k_gemm_tf32x3(const float* __restrict__ A, int64_t lda, const float* __restrict__ Bhi,
-                  const float* __restrict__ Blo, int64_t ldb, float* __restrict__ C, int64_t ldc,
-                  int M, int N, int K, int accumulate, int n_tiles, typename EpiArgs<EPI>::type re) {
+                  const float* __restrict__ Blo, int64_t ldb, int M, int N, int K, int n_tiles,
+                  const typename Epilogue<EPI>::type epi) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
 
@@ -397,233 +683,17 @@ __global__ void __launch_bounds__(N_THREADS, 1)
     }
   } else {
     // ================= consumer warpgroups =================
-    // accumulator fragment of wgmma m64nN: register 4j + 2h + e holds row 16 * (warp % 4) + lane / 4 + 8 h and
-    // column 8 j + 2 (lane % 4) + e of the warpgroup's 64 x 128 block
     const int ctid = tid - N_PRODUCERS;
-    const int wg = ctid >> 7;
+    const int wg = ctid >> 7, warp = ctid >> 5;
     const uint32_t a_rows = (uint32_t)(wg * 64 * 128);   // the warpgroup's 64 A rows of 128 B
     float big[N_FRAG], small[N_FRAG];
     for (int ti = 0; ti < n_mine; ++ti) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int m0 = (tile / tn) * BM, n0 = (tile % tn) * BN;
-      consume_tile(smem_base, full_bar, empty_bar, ti * num_kb, num_kb, a_rows, big, small);
-      const int r0 = m0 + wg * 64 + ((ctid >> 5) & 3) * 16 + (lane >> 2);
-      const int c0 = n0 + 2 * (lane & 3);
-      if constexpr (EPI == 4) {
-        // The quad of lanes lane & ~3 holds rows r0 and r0 + 8 of the tile: 32 columns each per lane, value i
-        // (= 2 j + e) at column c0 + 8 j + e, so a lane's columns increase with i.  k rounds per row: every lane
-        // takes its best value not yet taken (strict > in i order: the smaller column wins a tie), the quad keeps
-        // the best of the four by two shuffles on (energy, column), and the lane that owned it marks it taken.
-        float v[2][32];
-        uint32_t left[2];
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
-          left[h] = 0u;
-#pragma unroll
-          for (int cb = 0; cb < BN / 32; ++cb) {
-            const int chunk = n0 + 32 * cb;
-            const uint32_t xw =
-                (re.excl && row < M && chunk < N) ? __ldg(re.excl + (size_t)row * re.words + (chunk >> 5)) : 0u;
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int j = 4 * cb + jj, i = 2 * j + e, col = c0 + 8 * j + e;
-                v[h][i] = big[4 * j + 2 * h + e] + small[4 * j + 2 * h + e];
-                if (row < M && col < N && !((xw >> (col & 31)) & 1u)) left[h] |= 1u << i;
-              }
-            }
-          }
-        }
-        // candidate p of row r0 + 8 h (formed at the store: a live pointer pair would spill)
-        auto slot = [&](int h, int p) {
-          return re.cand + ((size_t)(r0 + 8 * h) * re.tn + (size_t)(n0 / BN)) * re.k + p;
-        };
-        const bool writer = (lane & 3) == 0;
-        const uint2 none = make_uint2(__float_as_uint(-INFINITY), 0xffffffffu);
-        int p = 0;
-        for (; p < re.k; ++p) {
-          float be[2];
-          int bc[2];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            int bi = -1;
-            be[h] = -INFINITY;
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (((left[h] >> i) & 1u) && (bi < 0 || v[h][i] > be[h])) {
-                be[h] = v[h][i];
-                bi = i;
-              }
-            const int mine = bi < 0 ? 0x7fffffff : c0 + 8 * (bi >> 1) + (bi & 1);
-            bc[h] = mine;
-#pragma unroll
-            for (int o = 1; o <= 2; o <<= 1) {
-              const float oe = __shfl_xor_sync(0xffffffffu, be[h], o);
-              const int oc = __shfl_xor_sync(0xffffffffu, bc[h], o);
-              if (oc != 0x7fffffff && (bc[h] == 0x7fffffff || oe > be[h] || (oe == be[h] && oc < bc[h]))) {
-                be[h] = oe;
-                bc[h] = oc;
-              }
-            }
-            if (bi >= 0 && bc[h] == mine) left[h] &= ~(1u << bi);
-          }
-          if (!__any_sync(0xffffffffu, bc[0] != 0x7fffffff || bc[1] != 0x7fffffff)) break;   // the warp's rows ran dry
-          if (writer) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              if (r0 + 8 * h < M)
-                *slot(h, p) = bc[h] == 0x7fffffff ? none : make_uint2(__float_as_uint(be[h]), (uint32_t)bc[h]);
-          }
-        }
-        if (writer) {
-          for (; p < re.k; ++p) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              if (r0 + 8 * h < M) *slot(h, p) = none;
-          }
-        }
-        continue;
-      }
-      if constexpr (EPI == 5) {
-        const float gs = re.scale * (re.g_scale ? __ldg(re.g_scale) : 1.f);
-        float ls = 0.f;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
-          if (row >= M) continue;
-#pragma unroll
-          for (int cb = 0; cb < BN / 32; ++cb) {
-            const int chunk = n0 + 32 * cb;
-            const uint32_t lw = chunk < N ? __ldg(re.labels + (size_t)row * re.words + (chunk >> 5)) : 0u;
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              const int j = 4 * cb + jj;
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int col = c0 + 8 * j + e;
-                if (col < N) {
-                  const float z = big[4 * j + 2 * h + e] + small[4 * j + 2 * h + e];
-                  const float y = ((lw >> (col & 31)) & 1u) ? re.pos : re.neg;
-                  ls += fmaxf(z, 0.f) - z * y + log1pf(expf(-fabsf(z)));
-                  if (re.Gt) re.Gt[(size_t)col * re.ldgt + row] = (1.0f / (1.0f + expf(-z)) - y) * gs;
-                }
-              }
-            }
-          }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) ls += __shfl_xor_sync(0xffffffffu, ls, o);
-        if (lane == 0) re.loss_part[(size_t)tile * 8 + (ctid >> 5)] = ls;
-        continue;
-      }
-      if constexpr (EPI == 3) {
-        float kl = 0.f;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int row = r0 + 8 * h;
-          if (row >= M) continue;
-          float* prow = C + (size_t)row * ldc;
-          const float* erow = re.eps + (size_t)row * re.w;
-          float* zrow = re.z + (size_t)row * re.w;
-          asm volatile("" : "+l"(erow), "+l"(zrow));   // no hoisting of the 16 pairs' loads ahead of use (spills)
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const int col = c0 + 8 * j;
-            if (col < N) {  // col is even: the pair is (mu, log sigma) of element col / 2
-              const int e = col >> 1;
-              const float mu = big[4 * j + 2 * h] + small[4 * j + 2 * h] + __ldg(re.b_mu + e);
-              const float ls = big[4 * j + 2 * h + 1] + small[4 * j + 2 * h + 1] + __ldg(re.b_sigma + e);
-              *reinterpret_cast<float2*>(prow + col) = make_float2(mu, ls);
-              zrow[e] = mu + expf(ls) * __ldg(erow + e);
-              kl += 1.f + 2.f * ls - mu * mu - expf(2.f * ls);
-            }
-          }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) kl += __shfl_xor_sync(0xffffffffu, kl, o);
-        if (lane == 0) re.kl_part[(size_t)tile * 8 + (ctid >> 5)] = kl;
-        continue;
-      }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
-        if constexpr (EPI == 2) {
-          if (row >= M) continue;
-          const float* c2row = A + (size_t)row * lda;
-          const float* c1row = re.c1 + (size_t)row * ldc;
-          float* orow = C + (size_t)row * ldc;
-          float* grow = re.gate + (size_t)row * ldc;
-          asm volatile("" : "+l"(c2row), "+l"(c1row));   // no hoisting of the 16 pairs' loads ahead of use (spills)
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const int col = c0 + 8 * j;
-            if (col < N) {  // N % 4 == 0: both columns of the pair exist
-              const float2 bb = __ldg(reinterpret_cast<const float2*>(re.bias + col));
-              const float2 x1 = __ldg(reinterpret_cast<const float2*>(c1row + col));
-              const float2 x2 = __ldg(reinterpret_cast<const float2*>(c2row + col));
-              const float g0 = sigmoid_ref(big[4 * j + 2 * h] + small[4 * j + 2 * h] + bb.x);
-              const float g1 = sigmoid_ref(big[4 * j + 2 * h + 1] + small[4 * j + 2 * h + 1] + bb.y);
-              *reinterpret_cast<float2*>(orow + col) = make_float2(x2.x + g0 * (x1.x - x2.x), x2.y + g1 * (x1.y - x2.y));
-              *reinterpret_cast<float2*>(grow + col) = make_float2(g0, g1);
-            }
-          }
-          continue;
-        }
-        if constexpr (EPI == 1) {
-          int raw = 0, kn = 0;
-          if (row < M) {
-            const float gold_s = __ldg(re.gold_sig + row);
-            const int gold_c = __ldg(re.gold_col + row);
-#pragma unroll
-            for (int cb = 0; cb < BN / 32; ++cb) {
-              const int chunk = n0 + 32 * cb;
-              const uint32_t kw =
-                  (re.known && chunk < N) ? __ldg(re.known + (size_t)row * re.words + (chunk >> 5)) : 0u;
-#pragma unroll
-              for (int jj = 0; jj < 4; ++jj) {
-                const int j = 4 * cb + jj;
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  const int col = c0 + 8 * j + e;
-                  const float v = big[4 * j + 2 * h + e] + small[4 * j + 2 * h + e];
-                  // the gold entity always scores >= itself
-                  if (col < N && (sigmoid_ref(v) >= gold_s || col == gold_c)) {
-                    ++raw;
-                    kn += (int)((kw >> (col & 31)) & 1u);
-                  }
-                }
-              }
-            }
-          }
-          raw += __shfl_xor_sync(0xffffffffu, raw, 1);
-          raw += __shfl_xor_sync(0xffffffffu, raw, 2);
-          kn += __shfl_xor_sync(0xffffffffu, kn, 1);
-          kn += __shfl_xor_sync(0xffffffffu, kn, 2);
-          if ((lane & 3) == 0 && row < M) {
-            if (raw) atomicAdd(re.raw_cnt + row, raw);
-            if (kn) atomicAdd(re.known_cnt + row, kn);
-          }
-          continue;
-        }
-        if (row >= M) continue;
-        float* crow = C + (size_t)row * ldc;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int col = c0 + 8 * j;
-          if (col < N) {  // N % 4 == 0: both columns of the pair exist
-            float2 o = make_float2(big[4 * j + 2 * h] + small[4 * j + 2 * h],
-                                   big[4 * j + 2 * h + 1] + small[4 * j + 2 * h + 1]);
-            if (accumulate) {
-              const float2 old = *reinterpret_cast<const float2*>(crow + col);
-              o.x += old.x;
-              o.y += old.y;
-            }
-            *reinterpret_cast<float2*>(crow + col) = o;
-          }
-        }
-      }
+      consume_tile<NtStage>(smem_base, full_bar, empty_bar, ti * num_kb, num_kb, a_rows, big, small);
+      const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = n0 + 2 * (lane & 3);
+      const TileCtx t{tile, m0, n0, r0, c0, M, N, lane, warp};
+      epi(t, big, small);
     }
   }
 }
@@ -656,6 +726,7 @@ __global__ void __launch_bounds__(N_THREADS, 1)
 // ------------------------------------------------------------------------------------------------
 constexpr int TN_FLUSH_KB = 32;                         // k-blocks per accumulation chain
 constexpr int TN_STAGES = 2;                            // MMA stages (A_hi, A_lo, B_hi, B_lo)
+using TnStage = StageShape<TN_STAGES, BN>;
 constexpr int TN_RAW = 3;                               // fp32 staging blocks
 constexpr int RAW_TILE_BYTES = BK * BM * 4;             // 16 KB: 32 k-rows x 128 values of one operand
 constexpr int RAW_BYTES = 2 * RAW_TILE_BYTES;           // A and B
@@ -761,8 +832,8 @@ __global__ void __launch_bounds__(N_THREADS, 1)
     float* const cbase = C + (size_t)r0 * ldc + c0;
     float big[N_FRAG], small[N_FRAG];
     for (int kc = 0; kc < num_kb; kc += TN_FLUSH_KB) {
-      consume_tile<TN_STAGES>(smem_base, full_bar, empty_bar, kc, min(TN_FLUSH_KB, num_kb - kc),
-                              (uint32_t)(wg * 64 * 128), big, small);
+      consume_tile<TnStage>(smem_base, full_bar, empty_bar, kc, min(TN_FLUSH_KB, num_kb - kc),
+                            (uint32_t)(wg * 64 * 128), big, small);
       float* cp = cbase;
       asm volatile("" : "+l"(cp));   // keeps the 32 addresses below from being hoisted out of the loop (spills)
 #pragma unroll
@@ -835,11 +906,12 @@ __global__ void k_split_b_interleave(const float* __restrict__ Wmu, const float*
 constexpr int EN_BN = 64;
 constexpr int EN_STAGES = 4;
 constexpr int EN_LOOKAHEAD = 2;                                    // blocks in flight ahead of the one published
-constexpr int EN_Q_BYTES = BM * BK * 4;                            // 16 KB (Q_hi, Q_lo)
-constexpr int EN_C_BYTES = EN_BN * BK * 4;                         // 8 KB (code_hi, code_lo)
-constexpr int EN_STAGE_BYTES = 2 * EN_Q_BYTES + 2 * EN_C_BYTES;    // 48 KB
+using EnsStage = StageShape<EN_STAGES, EN_BN>;
+constexpr int EN_Q_BYTES = EnsStage::A_PLANE;                      // 16 KB (Q_hi, Q_lo)
+constexpr int EN_C_BYTES = EnsStage::B_PLANE;                      // 8 KB (code_hi, code_lo)
+constexpr int EN_STAGE_BYTES = EnsStage::BYTES;                    // 48 KB
 constexpr int EN_SMEM_BYTES = EN_STAGES * EN_STAGE_BYTES + 1024;
-constexpr int EN_FRAG = EN_BN / 2;                                 // accumulator registers per thread and array
+constexpr int EN_FRAG = EnsStage::FRAG;                            // accumulator registers per thread and array
 static_assert(EN_SMEM_BYTES <= 227 * 1024, "ensemble kernel exceeds the shared memory of a block");
 static_assert(EN_LOOKAHEAD < EN_STAGES, "the lookahead needs a free stage");
 
@@ -860,58 +932,6 @@ struct EnsEpi {
   int32_t* raw_cnt;            // [M] += #{v : c_v >= G}
   int32_t* known_cnt;          // [M] += #{known v : c_v >= G}
 };
-
-// d[64 rows of this warpgroup x 64] (+)= A(desc) * B(desc)^T, TF32 inputs, fp32 accumulators
-__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[EN_FRAG], uint64_t da, uint64_t db, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %34, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
-      "%23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "%32, %33, p, 1, 1;\n\t"
-      "}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void fence_acc64(float (&d)[EN_FRAG]) {
-#pragma unroll
-  for (int i = 0; i < EN_FRAG; ++i) asm volatile("" : "+f"(d[i])::"memory");
-}
-
-// consume_tile for the 128 x 64 stages of the ensemble kernel: k-blocks g0 .. g0 + num_kb - 1 of the CTA's stage
-// sequence into (big, small), the MMAs of a K step in the order of consume_tile
-__device__ __forceinline__ void ens_consume(uint32_t smem_base, uint64_t* full_bar, uint64_t* empty_bar, int g0,
-                                            int num_kb, uint32_t a_rows, float (&big)[EN_FRAG],
-                                            float (&small)[EN_FRAG]) {
-  for (int kb = 0; kb < num_kb; ++kb) {
-    const int g = g0 + kb;
-    const int s = g % EN_STAGES;
-    mbar_wait(&full_bar[s], (uint32_t)(g / EN_STAGES) & 1u);
-    const uint32_t a_hi = smem_base + s * EN_STAGE_BYTES + a_rows, a_lo = a_hi + EN_Q_BYTES;
-    const uint32_t b_hi = smem_base + s * EN_STAGE_BYTES + 2 * EN_Q_BYTES, b_lo = b_hi + EN_C_BYTES;
-    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int kk = 0; kk < BK / 8; ++kk) {
-      const uint64_t dah = make_desc(a_hi + kk * 32), dal = make_desc(a_lo + kk * 32);
-      const uint64_t dbh = make_desc(b_hi + kk * 32), dbl = make_desc(b_lo + kk * 32);
-      const uint32_t acc = (kb == 0 && kk == 0) ? 0u : 1u;
-      wgmma_tf32_n64(small, dal, dbh, acc);
-      wgmma_tf32_n64(small, dah, dbl, 1u);
-      wgmma_tf32_n64(big, dah, dbh, acc);
-    }
-    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-    fence_acc64(big);
-    fence_acc64(small);
-    mbar_arrive(&empty_bar[s]);
-  }
-}
 
 // Persistent like k_gemm_tf32x3 (N tiles fastest); a tile is num_kb_a + num_kb_b consecutive k-blocks of the CTA's
 // stage sequence.
@@ -993,57 +1013,36 @@ __global__ void __launch_bounds__(N_THREADS, 1)
     }
   } else {
     // ================= consumer warpgroups =================
-    // accumulator fragment of wgmma m64n64: register 4j + 2h + e holds row 16 * (warp % 4) + lane / 4 + 8 h and
-    // column 8 j + 2 (lane % 4) + e of the warpgroup's 64 x 64 block
     const int ctid = tid - N_PRODUCERS;
-    const int wg = ctid >> 7;
+    const int wg = ctid >> 7, warp = ctid >> 5;
     const uint32_t a_rows = (uint32_t)(wg * 64 * 128);
     float big_a[EN_FRAG], small_a[EN_FRAG], big_b[EN_FRAG], small_b[EN_FRAG];
     for (int ti = 0; ti < n_mine; ++ti) {
       const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
       const int m0 = (tile / tn) * BM, n0 = (tile % tn) * EN_BN;
-      ens_consume(smem_base, full_bar, empty_bar, ti * nkb, nkb_a, a_rows, big_a, small_a);
-      ens_consume(smem_base, full_bar, empty_bar, ti * nkb + nkb_a, nkb_b, a_rows, big_b, small_b);
-      const int r0 = m0 + wg * 64 + ((ctid >> 5) & 3) * 16 + (lane >> 2);
-      const int c0 = n0 + 2 * (lane & 3);
+      consume_tile<EnsStage>(smem_base, full_bar, empty_bar, ti * nkb, nkb_a, a_rows, big_a, small_a);
+      consume_tile<EnsStage>(smem_base, full_bar, empty_bar, ti * nkb + nkb_a, nkb_b, a_rows, big_b, small_b);
+      const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = n0 + 2 * (lane & 3);
+      const TileCtx t{tile, m0, n0, r0, c0, M, N, lane, warp};
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int row = r0 + 8 * h;
+        const int row = t.r0 + 8 * h;
         int raw = 0, kn = 0;
         if (row < M) {
           const double G = __dadd_rn(__dmul_rn(re.w, (double)__ldg(re.a.gold_sig + row)),
                                      __dmul_rn(re.omw, (double)__ldg(re.b.gold_sig + row)));
           const int gold_c = __ldg(re.gold_col + row);
-#pragma unroll
-          for (int cb = 0; cb < EN_BN / 32; ++cb) {
-            const int chunk = n0 + 32 * cb;
-            const uint32_t kw =
-                (re.known && chunk < N) ? __ldg(re.known + (size_t)row * re.words + (chunk >> 5)) : 0u;
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              const int j = 4 * cb + jj;
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int col = c0 + 8 * j + e, r = 4 * j + 2 * h + e;
-                const float sa = sigmoid_ref(big_a[r] + small_a[r]);
-                const float sb = sigmoid_ref(big_b[r] + small_b[r]);
-                const double cv = __dadd_rn(__dmul_rn(re.w, (double)sa), __dmul_rn(re.omw, (double)sb));
-                if (col < N && (cv >= G || col == gold_c)) {   // the gold entity always counts
-                  ++raw;
-                  kn += (int)((kw >> (col & 31)) & 1u);
-                }
-              }
+          for_each_col<EN_FRAG>(t, h, re.known, re.words, [&](int r, int, int col, uint32_t word) {
+            const float sa = sigmoid_ref(big_a[r] + small_a[r]);
+            const float sb = sigmoid_ref(big_b[r] + small_b[r]);
+            const double cv = __dadd_rn(__dmul_rn(re.w, (double)sa), __dmul_rn(re.omw, (double)sb));
+            if (col < N && (cv >= G || col == gold_c)) {   // the gold entity always counts
+              ++raw;
+              kn += (int)col_bit(word, col);
             }
-          }
+          });
         }
-        raw += __shfl_xor_sync(0xffffffffu, raw, 1);
-        raw += __shfl_xor_sync(0xffffffffu, raw, 2);
-        kn += __shfl_xor_sync(0xffffffffu, kn, 1);
-        kn += __shfl_xor_sync(0xffffffffu, kn, 2);
-        if ((lane & 3) == 0 && row < M) {
-          if (raw) atomicAdd(re.raw_cnt + row, raw);
-          if (kn) atomicAdd(re.known_cnt + row, kn);
-        }
+        rank_counts_flush(raw, kn, row, M, re.raw_cnt, re.known_cnt, lane);
       }
     }
   }
@@ -1073,22 +1072,55 @@ static int sm_count() {
   return sms;
 }
 
+// Tiles of an [M, N] output in 128 x bn tiles: the one count the launchers, the kernels' part arrays
+// (gemm_onen_loss_parts, gemm_variational_kl_parts) and the kernels' tile walk agree on
+static int64_t tiles_of(int64_t M, int64_t N, int bn) { return ((M + BM - 1) / BM) * ((N + bn - 1) / bn); }
+
+// The one launch path of the persistent kernels: the dynamic shared memory size is raised once per kernel, `tiles`
+// is checked against `tile_limit` (what the kernel's index arithmetic holds in an int), and min(tiles, SMs) CTAs walk
+// the tiles, at most one per SM.  `what` names the launcher in the error text, `label` the kernel.
+template <auto Kernel, class... Args>
+static int launch_persistent(const char* what, const char* label, int smem, int64_t tiles, int64_t tile_limit,
+                             cudaStream_t st, Args... args) {
+  static bool attr_set = false;   // one per kernel: Kernel is a template argument
+  if (!attr_set) {
+    int rc = rgcn_check_cuda(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem),
+                             (std::string("cudaFuncSetAttribute(") + label + " smem)").c_str());
+    if (rc) return rc;
+    attr_set = true;
+  }
+  if (tiles > tile_limit) {
+    rgcn_set_error(std::string(what) + ": too many tiles");
+    return RGCN_ERR_INVALID;
+  }
+  const unsigned grid = (unsigned)std::min<int64_t>(tiles, sm_count());
+  Kernel<<<grid, N_THREADS, smem, st>>>(args...);
+  ++g_rgcn_launches;
+  return rgcn_check_cuda(cudaGetLastError(), label);
+}
+constexpr int64_t TILE_LIMIT = 0x7fffffffLL;         // the tile index is an int
+constexpr int64_t PART_TILE_LIMIT = TILE_LIMIT / 8;  // ... and so is part[tile * 8 + warp]'s count (VarEpi, BceEpi)
+
+// The NT kernel with the epilogue `epi` of EPI over an [M, N] output
+template <int EPI>
+static int launch_nt(const char* what, const char* label, int64_t tile_limit, cudaStream_t st, const float* A,
+                     int64_t lda, const float* Bt_hi, const float* Bt_lo, int64_t ldb, int M, int N, int K,
+                     const typename Epilogue<EPI>::type& epi) {
+  const int64_t tiles = tiles_of(M, N, BN);
+  return launch_persistent<k_gemm_tf32x3<EPI>>(what, label, SMEM_BYTES, tiles, tile_limit, st, A, lda, Bt_hi, Bt_lo,
+                                               ldb, M, N, K, (int)tiles, epi);
+}
+
+// grid of the element-wise split kernels (256 threads, grid-stride)
+static int split_blocks(int64_t items) { return (int)std::min<int64_t>((items + 255) / 256, 132 * 8); }
+
 int launch_gemm_split_b(const float* B, int64_t ldb, int N, int K, int transposed, float* hi, float* lo,
                         cudaStream_t st) {
   const int64_t total = (int64_t)N * K;
   if (total == 0) return RGCN_OK;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  k_split_b<<<blocks, 256, 0, st>>>(B, ldb, N, K, transposed, hi, lo);
+  k_split_b<<<split_blocks(total), 256, 0, st>>>(B, ldb, N, K, transposed, hi, lo);
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_split_b");
-}
-
-// grid of the persistent NT kernel: the SM count of the current device ($RGCN_GEMM_CTAS overrides; a value >= the
-// tile count gives a one-tile-per-CTA schedule)
-static int64_t nt_grid_cap() {
-  if (const char* e = std::getenv("RGCN_GEMM_CTAS")) return std::max<int64_t>(1, std::atoll(e));
-  return sm_count();
 }
 
 int launch_gemm_tf32x3(const float* A, int64_t lda, const float* Bt_hi, const float* Bt_lo, int64_t ldb,
@@ -1102,24 +1134,8 @@ int launch_gemm_tf32x3(const float* A, int64_t lda, const float* Bt_hi, const fl
     if (accumulate) return RGCN_OK;
     return rgcn_check_cuda(cudaMemset2DAsync(C, ldc * sizeof(float), 0, (size_t)N * sizeof(float), M, st), "memset(C)");
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  SMEM_BYTES),
-                             "cudaFuncSetAttribute(gemm smem)");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((N + BN - 1) / BN);
-  if (tiles > 0x7fffffffLL) {
-    rgcn_set_error("gemm_tf32x3: too many tiles");
-    return RGCN_ERR_INVALID;
-  }
-  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));   // persistent: at most one CTA per SM
-  k_gemm_tf32x3<0><<<grid, N_THREADS, SMEM_BYTES, st>>>(A, lda, Bt_hi, Bt_lo, ldb, C, ldc, M, N, K, accumulate,
-                                                         (int)tiles, RankEpi{});
-  ++g_rgcn_launches;
-  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3");
+  return launch_nt<EPI_STORE>("gemm_tf32x3", "k_gemm_tf32x3", TILE_LIMIT, st, A, lda, Bt_hi, Bt_lo, ldb, M, N, K,
+                              StoreEpi{C, ldc, accumulate});
 }
 
 // Scoring GEMM with the ranking epilogue: queries Q [M,K] against the pre-split entity codes Bt [N,K]; the counts
@@ -1132,25 +1148,8 @@ int launch_gemm_rank_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
     rgcn_set_error("gemm_rank_tf32x3: K > 0; K and leading dimensions must be multiples of 4");
     return RGCN_ERR_INVALID;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<1>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  SMEM_BYTES),
-                             "cudaFuncSetAttribute(gemm rank smem)");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  RankEpi re{gold_sig, gold_col, known, words, raw_cnt, known_cnt};
-  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((N + BN - 1) / BN);
-  if (tiles > 0x7fffffffLL) {
-    rgcn_set_error("gemm_rank_tf32x3: too many tiles");
-    return RGCN_ERR_INVALID;
-  }
-  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
-  k_gemm_tf32x3<1><<<grid, N_THREADS, SMEM_BYTES, st>>>(Q, ldq, Bt_hi, Bt_lo, ldb, nullptr, 0, M, N, K, 0,
-                                                         (int)tiles, re);
-  ++g_rgcn_launches;
-  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<rank>");
+  return launch_nt<EPI_RANK>("gemm_rank_tf32x3", "k_gemm_tf32x3<rank>", TILE_LIMIT, st, Q, ldq, Bt_hi, Bt_lo, ldb, M,
+                             N, K, RankEpi{gold_sig, gold_col, known, words, raw_cnt, known_cnt});
 }
 
 // Scoring GEMM with the top-k epilogue (EPI = 4): queries Q [M,K] against the pre-split entity codes Bt [N,K]; each
@@ -1162,30 +1161,11 @@ int launch_gemm_topk_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
     rgcn_set_error("gemm_topk_tf32x3: K > 0; K and leading dimensions must be multiples of 4; 1 <= k <= 128");
     return RGCN_ERR_INVALID;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  SMEM_BYTES),
-                             "cudaFuncSetAttribute(gemm topk smem)");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  const int tn = (N + BN - 1) / BN;
-  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * tn;
-  if (tiles > 0x7fffffffLL) {
-    rgcn_set_error("gemm_topk_tf32x3: too many tiles");
-    return RGCN_ERR_INVALID;
-  }
-  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
-  k_gemm_tf32x3<4><<<grid, N_THREADS, SMEM_BYTES, st>>>(Q, ldq, Bt_hi, Bt_lo, ldb, nullptr, 0, M, N, K, 0,
-                                                         (int)tiles, TopKEpi{excl, words, k, tn, cand});
-  ++g_rgcn_launches;
-  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<topk>");
+  return launch_nt<EPI_TOPK>("gemm_topk_tf32x3", "k_gemm_tf32x3<topk>", TILE_LIMIT, st, Q, ldq, Bt_hi, Bt_lo, ldb, M,
+                             N, K, TopKEpi{excl, words, k, (N + BN - 1) / BN, cand});
 }
 
-int64_t gemm_onen_loss_parts(int64_t M, int N) {
-  return ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * 8;
-}
+int64_t gemm_onen_loss_parts(int64_t M, int N) { return tiles_of(M, N, BN) * 8; }
 
 // 1-N scoring GEMM with the BCE epilogue (EPI = 5): queries Q [M,K] against the pre-split entity codes Bt [N,K];
 // gemm_onen_loss_parts(M, N) loss parts, and Gt [N, ldgt] (transposed gradients of the energies) unless Gt is null.
@@ -1197,32 +1177,14 @@ int launch_gemm_onen_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, con
     rgcn_set_error("gemm_onen_tf32x3: K > 0; K and leading dimensions must be multiples of 4");
     return RGCN_ERR_INVALID;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<5>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  SMEM_BYTES),
-                             "cudaFuncSetAttribute(gemm onen smem)");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((N + BN - 1) / BN);
-  if (tiles > 0x7fffffffLL / 8) {
-    rgcn_set_error("gemm_onen_tf32x3: too many tiles");
-    return RGCN_ERR_INVALID;
-  }
-  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
-  k_gemm_tf32x3<5><<<grid, N_THREADS, SMEM_BYTES, st>>>(
-      Q, ldq, Bt_hi, Bt_lo, ldb, nullptr, 0, M, N, K, 0, (int)tiles,
-      BceEpi{labels, (N + 31) / 32, pos, neg, scale, g_scale, Gt, ldgt, loss_part});
-  ++g_rgcn_launches;
-  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<onen>");
+  return launch_nt<EPI_BCE>("gemm_onen_tf32x3", "k_gemm_tf32x3<onen>", PART_TILE_LIMIT, st, Q, ldq, Bt_hi, Bt_lo, ldb,
+                            M, N, K, BceEpi{labels, (N + 31) / 32, pos, neg, scale, g_scale, Gt, ldgt, loss_part});
 }
 
 int launch_split_trunc(float* a, float* lo, int64_t count, cudaStream_t st) {
   if (count == 0) return RGCN_OK;
   const int64_t count4 = count / 4;
-  int blocks = (int)std::min<int64_t>((count4 + 255) / 256, 132 * 8);
-  k_split_trunc<<<blocks, 256, 0, st>>>(a, lo, count4);
+  k_split_trunc<<<split_blocks(count4), 256, 0, st>>>(a, lo, count4);
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_split_trunc");
 }
@@ -1238,25 +1200,11 @@ int launch_gemm_ensemble_rank_tf32x3(const float* qa_hi, const float* qa_lo, con
     rgcn_set_error("gemm_ensemble_rank_tf32x3: K > 0 and K % 4 == 0 for both members");
     return RGCN_ERR_INVALID;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_ensemble_rank, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  EN_SMEM_BYTES),
-                             "cudaFuncSetAttribute(gemm ensemble smem)");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((N + EN_BN - 1) / EN_BN);
-  if (tiles > 0x7fffffffLL) {
-    rgcn_set_error("gemm_ensemble_rank_tf32x3: too many tiles");
-    return RGCN_ERR_INVALID;
-  }
+  const int64_t tiles = tiles_of(M, N, EN_BN);
   EnsEpi re{{qa_hi, qa_lo, ca_hi, ca_lo, gold_sig_a, Ka}, {qb_hi, qb_lo, cb_hi, cb_lo, gold_sig_b, Kb}, w, omw,
             gold_col, known, words, raw_cnt, known_cnt};
-  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
-  k_gemm_ensemble_rank<<<grid, N_THREADS, EN_SMEM_BYTES, st>>>(M, N, (int)tiles, re);
-  ++g_rgcn_launches;
-  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_ensemble_rank");
+  return launch_persistent<k_gemm_ensemble_rank>("gemm_ensemble_rank_tf32x3", "k_gemm_ensemble_rank", EN_SMEM_BYTES,
+                                                 tiles, TILE_LIMIT, st, M, N, (int)tiles, re);
 }
 
 // Highway gate GEMM with the blend epilogue (EPI = 2): z = c2 @ W + bias with W pre-split as Bt = W^T [d, d];
@@ -1268,40 +1216,20 @@ int launch_gemm_highway_tf32x3(const float* c2, const float* Bt_hi, const float*
     rgcn_set_error("gemm_highway_tf32x3: d > 0, d % 4 == 0");
     return RGCN_ERR_INVALID;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<2>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  SMEM_BYTES),
-                             "cudaFuncSetAttribute(gemm highway smem)");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((d + BN - 1) / BN);
-  if (tiles > 0x7fffffffLL) {
-    rgcn_set_error("gemm_highway_tf32x3: too many tiles");
-    return RGCN_ERR_INVALID;
-  }
-  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
-  k_gemm_tf32x3<2><<<grid, N_THREADS, SMEM_BYTES, st>>>(c2, d, Bt_hi, Bt_lo, d, out, d, M, d, d, 0, (int)tiles,
-                                                         HighwayEpi{bias, c1, gate});
-  ++g_rgcn_launches;
-  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<highway>");
+  return launch_nt<EPI_HIGHWAY>("gemm_highway_tf32x3", "k_gemm_tf32x3<highway>", TILE_LIMIT, st, c2, d, Bt_hi, Bt_lo,
+                                d, M, d, d, HighwayEpi{bias, c1, c2, out, gate, d});
 }
 
 int launch_gemm_split_b_interleave(const float* Wmu, const float* Wsig, int d, int w, int transposed, float* hi,
                                    float* lo, cudaStream_t st) {
   const int64_t total = (int64_t)2 * d * w;
   if (total == 0) return RGCN_OK;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  k_split_b_interleave<<<blocks, 256, 0, st>>>(Wmu, Wsig, d, w, transposed, hi, lo);
+  k_split_b_interleave<<<split_blocks(total), 256, 0, st>>>(Wmu, Wsig, d, w, transposed, hi, lo);
   ++g_rgcn_launches;
   return rgcn_check_cuda(cudaGetLastError(), "k_split_b_interleave");
 }
 
-int64_t gemm_variational_kl_parts(int64_t M, int w) {
-  return ((M + BM - 1) / BM) * ((2 * (int64_t)w + BN - 1) / BN) * 8;
-}
+int64_t gemm_variational_kl_parts(int64_t M, int w) { return tiles_of(M, 2 * (int64_t)w, BN) * 8; }
 
 // Variational head GEMM (EPI = 3): P = H W_int + [b_mu, b_sigma] interleaved, z = mu + exp(l) eps, one KL part per
 // consumer warp and tile (gemm_variational_kl_parts of them).  H [M, d], P [M, 2w], eps / z [M, w], contiguous.
@@ -1313,24 +1241,8 @@ int launch_gemm_variational_tf32x3(const float* H, const float* Bt_hi, const flo
     rgcn_set_error("gemm_variational_tf32x3: d > 0, d % 4 == 0, w > 0, w % 2 == 0");
     return RGCN_ERR_INVALID;
   }
-  static bool attr_set = false;
-  if (!attr_set) {
-    int rc = rgcn_check_cuda(cudaFuncSetAttribute(k_gemm_tf32x3<3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                  SMEM_BYTES),
-                             "cudaFuncSetAttribute(gemm variational smem)");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((2 * w + BN - 1) / BN);
-  if (tiles > 0x7fffffffLL / 8) {
-    rgcn_set_error("gemm_variational_tf32x3: too many tiles");
-    return RGCN_ERR_INVALID;
-  }
-  dim3 grid((unsigned)std::min<int64_t>(tiles, nt_grid_cap()));
-  k_gemm_tf32x3<3><<<grid, N_THREADS, SMEM_BYTES, st>>>(H, d, Bt_hi, Bt_lo, d, P, 2 * w, M, 2 * w, d, 0, (int)tiles,
-                                                         VarEpi{b_mu, b_sigma, eps, z, kl_part, w});
-  ++g_rgcn_launches;
-  return rgcn_check_cuda(cudaGetLastError(), "k_gemm_tf32x3<variational>");
+  return launch_nt<EPI_VAR>("gemm_variational_tf32x3", "k_gemm_tf32x3<variational>", PART_TILE_LIMIT, st, H, d, Bt_hi,
+                            Bt_lo, d, M, 2 * w, d, VarEpi{b_mu, b_sigma, eps, P, 2 * w, z, kl_part, w});
 }
 
 // C[M,N] (+)= A^T B, A [K,M] row-major, B [K,N] row-major (see k_gemm_tn_tf32x3)
@@ -1361,7 +1273,7 @@ int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t l
   // floor(sms / tiles) splits for long K (M = N = 512, K = 5 M on 132 SMs: 8 splits, 128 CTAs); with more tiles
   // than one wave holds, more (shorter) splits fill the last wave.
   constexpr int64_t TN_KB_FIXED = 4;
-  const int64_t tiles = (int64_t)((M + BM - 1) / BM) * ((N + BN - 1) / BN);
+  const int64_t tiles = tiles_of(M, N, BN);
   const int64_t kb_total = (K + BK - 1) / BK, sms = sm_count();
   int64_t splits = 1, kb_per_split = kb_total, best = -1;
   for (int64_t s = 1; s <= kb_total && (s == 1 || s * tiles <= 8 * sms); ++s) {
