@@ -550,6 +550,52 @@ int rgcn_ensemble_rank(int32_t decoder_a, const float* codes_a, const float* rel
                        int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * Ensemble top-k and relation prediction, fused (R-GCN+): the members, decoders, widths, weight w and V as in
+ * rgcn_ensemble_rank.
+ * rgcn_ensemble_topk: the k entities of best combined score for every triple of X (side 0 predicts subjects, 1
+ *   objects; the predicted column is not read), ordered by
+ *     u(t, v) = w sigma(-E_A(t, v)) + (1 - w) sigma(-E_B(t, v))      ascending, the smaller id first on ties,
+ *   with E_X member X's float32 energy (its rgcn_*_topk energy), sigma(-E) = 1 / (1 + exp(E)) in double, and the
+ *   products and sum separately rounded doubles.  u = 1 - c in exact arithmetic, so this is the c-descending order
+ *   without the float32 sigmoid's saturation at the top: sigma(-E) of a positive energy ties only once it underflows
+ *   (E > 745).  At the bottom it saturates earlier than the float32 sigmoid: sigma(-E) rounds to exactly 1 once E is
+ *   below about -37, so candidates that both members score below about -37 tie at u = 1 (id order, score 0).  A gold
+ *   entity's position here can therefore differ from its rank under c in saturated cases, as distmult_topk's energy
+ *   order does from distmult_rank's.  ids int32 [n, k], u double [n, k] and scores double [n, k] = 1 - u; a row with fewer than
+ *   k eligible entities ends in id -1, u +inf, score 0.  exclude_mask as in distmult_topk.  1 <= k <= 128.
+ *   workspace : rgcn_ensemble_topk_workspace_bytes(V, d_a, d_b, n, k), linear in n; its head holds the two members'
+ *   hi/lo code splits exactly as rgcn_ensemble_rank's workspace, so reuse_split != 0 serves both.
+ * rgcn_ensemble_relation_rank / rgcn_ensemble_relation_topk: (h, ?, t) queries over the first R relations, each
+ *   member's query row that of its *_relation_rank entry point (the relation column of X is the gold relation for the
+ *   ranks and is not read by top-k).  Ranks by rgcn_ensemble_rank's arithmetic and counting rules over relations
+ *   0..R-1 (known_mask [n, ceil(R/32)]); top-k by rgcn_ensemble_topk's order (exclude_mask [n, ceil(R/32)]).
+ *   1 <= R <= Vrel_a and R <= Vrel_b.  workspace : rgcn_ensemble_relation_rank_workspace_bytes(R, d_a, d_b, n) /
+ *   rgcn_ensemble_relation_topk_workspace_bytes(R, d_a, d_b, n, k); both start with the splits of rel_a[0:R] and
+ *   rel_b[0:R] in the same place (reuse_split != 0 skips them), never those of an entity workspace.
+ * Errors, before any device work: RGCN_ERR_INVALID (unknown decoder kind, d_x % 4 != 0, bad weight, k out of range,
+ * side, null pointers, R out of range, filtered ranks without a known mask), RGCN_ERR_WORKSPACE.  The
+ * *_workspace_bytes functions return RGCN_ERR_INVALID (-1) on bad arguments.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_ensemble_topk_workspace_bytes(int32_t V, int32_t d_a, int32_t d_b, int64_t n, int32_t k);
+int rgcn_ensemble_topk(int32_t decoder_a, const float* codes_a, const float* rel_a, int32_t Vrel_a, int32_t d_a,
+                       int32_t decoder_b, const float* codes_b, const float* rel_b, int32_t Vrel_b, int32_t d_b,
+                       int32_t V, double weight, const int32_t* X, int64_t n, int side, int32_t k,
+                       const uint32_t* exclude_mask, int reuse_split, int32_t* ids, double* u, double* scores,
+                       void* workspace, int64_t workspace_bytes, void* stream);
+int64_t rgcn_ensemble_relation_rank_workspace_bytes(int32_t R, int32_t d_a, int32_t d_b, int64_t n);
+int rgcn_ensemble_relation_rank(int32_t decoder_a, const float* codes_a, const float* rel_a, int32_t Vrel_a,
+                                int32_t d_a, int32_t decoder_b, const float* codes_b, const float* rel_b,
+                                int32_t Vrel_b, int32_t d_b, int32_t V, int32_t R, double weight, const int32_t* X,
+                                int64_t n, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
+                                int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream);
+int64_t rgcn_ensemble_relation_topk_workspace_bytes(int32_t R, int32_t d_a, int32_t d_b, int64_t n, int32_t k);
+int rgcn_ensemble_relation_topk(int32_t decoder_a, const float* codes_a, const float* rel_a, int32_t Vrel_a,
+                                int32_t d_a, int32_t decoder_b, const float* codes_b, const float* rel_b,
+                                int32_t Vrel_b, int32_t d_b, int32_t V, int32_t R, double weight, const int32_t* X,
+                                int64_t n, int32_t k, const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
+                                double* u, double* scores, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Top-k entity prediction, fused: the k entities each query believes in most, without the [n, V] score matrix
  * that predict_all_subject_scores / predict_all_object_scores (bilinear_diag.py:51-61, complex.py:77-106)
  * materialise and Scorer.dump_all_scores (common/evaluation.py:391-408) writes out.  For every triple t of X:

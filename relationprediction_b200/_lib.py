@@ -32,6 +32,9 @@ EXPORTED_SYMBOLS = [
     "rgcn_relation_rank_workspace_bytes", "distmult_relation_rank", "rgcn_complex_relation_rank",
     "rgcn_relation_topk_workspace_bytes", "distmult_relation_topk", "rgcn_complex_relation_topk",
     "rgcn_ensemble_rank_workspace_bytes", "rgcn_ensemble_rank",
+    "rgcn_ensemble_topk_workspace_bytes", "rgcn_ensemble_topk",
+    "rgcn_ensemble_relation_rank_workspace_bytes", "rgcn_ensemble_relation_rank",
+    "rgcn_ensemble_relation_topk_workspace_bytes", "rgcn_ensemble_relation_topk",
     "rgcn_one_to_n_workspace_bytes", "distmult_one_to_n", "rgcn_complex_one_to_n",
     "rgcn_one_to_n_labels_workspace_bytes", "rgcn_one_to_n_labels",
     "rgcn_one_to_n_finish_workspace_bytes", "rgcn_one_to_n_finish",
@@ -219,6 +222,23 @@ def _declare(lib):
     lib.rgcn_ensemble_rank.restype = c_int
     lib.rgcn_ensemble_rank.argtypes = [c_int32, vp, vp, c_int32, c_int32, c_int32, vp, vp, c_int32, c_int32, c_int32,
                                        c_double, vp, c_int64, c_int, vp, c_int, vp, vp, vp, c_int64, vp]
+    lib.rgcn_ensemble_topk_workspace_bytes.restype = c_int64
+    lib.rgcn_ensemble_topk_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int64, c_int32]
+    lib.rgcn_ensemble_topk.restype = c_int
+    lib.rgcn_ensemble_topk.argtypes = [c_int32, vp, vp, c_int32, c_int32, c_int32, vp, vp, c_int32, c_int32, c_int32,
+                                       c_double, vp, c_int64, c_int, c_int32, vp, c_int, vp, vp, vp, vp, c_int64, vp]
+    lib.rgcn_ensemble_relation_rank_workspace_bytes.restype = c_int64
+    lib.rgcn_ensemble_relation_rank_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int64]
+    lib.rgcn_ensemble_relation_rank.restype = c_int
+    lib.rgcn_ensemble_relation_rank.argtypes = [c_int32, vp, vp, c_int32, c_int32, c_int32, vp, vp, c_int32, c_int32,
+                                                c_int32, c_int32, c_double, vp, c_int64, vp, c_int, vp, vp, vp,
+                                                c_int64, vp]
+    lib.rgcn_ensemble_relation_topk_workspace_bytes.restype = c_int64
+    lib.rgcn_ensemble_relation_topk_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int64, c_int32]
+    lib.rgcn_ensemble_relation_topk.restype = c_int
+    lib.rgcn_ensemble_relation_topk.argtypes = [c_int32, vp, vp, c_int32, c_int32, c_int32, vp, vp, c_int32, c_int32,
+                                                c_int32, c_int32, c_double, vp, c_int64, c_int32, vp, c_int, vp, vp,
+                                                vp, vp, c_int64, vp]
     lib.rgcn_one_to_n_workspace_bytes.restype = c_int64
     lib.rgcn_one_to_n_workspace_bytes.argtypes = [c_int32, c_int32, c_int64, c_int64]
     for name in ("distmult_one_to_n", "rgcn_complex_one_to_n"):

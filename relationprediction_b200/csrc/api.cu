@@ -1457,56 +1457,19 @@ static RankPrepareFn ensemble_prepare(int32_t decoder) {
   return nullptr;
 }
 
-extern "C" int64_t rgcn_ensemble_rank_workspace_bytes(int32_t V, int32_t d_a, int32_t d_b, int64_t n) {
-  if (V <= 0 || d_a <= 0 || d_a % 4 != 0 || d_b <= 0 || d_b % 4 != 0 || n < 0 || n > 0x7fffffffLL) {
-    rgcn_set_error("rgcn_ensemble_rank_workspace_bytes: bad arguments (need V > 0, d > 0, d % 4 == 0, 0 <= n < 2^31)");
-    return RGCN_ERR_INVALID;
-  }
-  return 2 * align_up((int64_t)V * d_a * 4) + 2 * align_up((int64_t)V * d_b * 4) + 2 * align_up(n * d_a * 4) +
-         2 * align_up(n * d_b * 4) + 5 * align_up(n * 4) + 256;
-}
-
-extern "C" int rgcn_ensemble_rank(int32_t decoder_a, const float* codes_a, const float* rel_a, int32_t Vrel_a,
-                                  int32_t d_a, int32_t decoder_b, const float* codes_b, const float* rel_b,
-                                  int32_t Vrel_b, int32_t d_b, int32_t V, double weight, const int32_t* X, int64_t n,
-                                  int side, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
-                                  int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream) {
-  const RankPrepareFn prep_a = ensemble_prepare(decoder_a), prep_b = ensemble_prepare(decoder_b);
-  if (!prep_a || !prep_b) {
-    rgcn_set_error("rgcn_ensemble_rank: unknown decoder kind (RGCN_DECODER_DISTMULT or RGCN_DECODER_COMPLEX)");
-    return RGCN_ERR_INVALID;
-  }
-  if (d_a <= 0 || d_a % 4 != 0 || d_b <= 0 || d_b % 4 != 0) {
-    rgcn_set_error("rgcn_ensemble_rank: bad arguments (need d % 4 == 0 for both members)");
-    return RGCN_ERR_INVALID;
-  }
-  if (!(weight >= 0.0 && weight <= 1.0)) {   // also refuses NaN
-    rgcn_set_error("rgcn_ensemble_rank: bad arguments (the weight must be finite and in [0, 1])");
-    return RGCN_ERR_INVALID;
-  }
-  if (!codes_a || !rel_a || !codes_b || !rel_b || (n > 0 && (!X || !raw_rank)) || !workspace || V <= 0 ||
-      Vrel_a <= 0 || Vrel_b <= 0 || n < 0 || n > 0x7fffffffLL) {
-    rgcn_set_error("rgcn_ensemble_rank: bad arguments (null pointer or bad size)");
-    return RGCN_ERR_INVALID;
-  }
-  if (side != 0 && side != 1) {
-    rgcn_set_error("rgcn_ensemble_rank: bad arguments (side in {0,1})");
-    return RGCN_ERR_INVALID;
-  }
-  if (filtered_rank && !known_mask) {
-    rgcn_set_error("rgcn_ensemble_rank: bad arguments (filtered ranks need a known mask)");
-    return RGCN_ERR_INVALID;
-  }
-  if (workspace_bytes < rgcn_ensemble_rank_workspace_bytes(V, d_a, d_b, n)) {
-    rgcn_set_error("rgcn_ensemble_rank: workspace too small (rgcn_ensemble_rank_workspace_bytes)");
-    return RGCN_ERR_WORKSPACE;
-  }
-  cudaStream_t st = (cudaStream_t)stream;
+// The body of rgcn_ensemble_rank and rgcn_ensemble_relation_rank, after their argument checks: the candidates are the
+// first N rows of table_a / table_b (the codes, N = V, or the relation tables, N = R), the query rows come from
+// prep_a / prep_b (the members' entity or relation prepare kernels).
+static int ensemble_rank_body(RankPrepareFn prep_a, const float* table_a, RankPrepareFn prep_b, const float* table_b,
+                              int32_t N, const float* codes_a, const float* rel_a, int32_t d_a, const float* codes_b,
+                              const float* rel_b, int32_t d_b, double weight, const int32_t* X, int64_t n, int side,
+                              const uint32_t* known_mask, int reuse_split, int32_t* raw_rank, int32_t* filtered_rank,
+                              void* workspace, int64_t workspace_bytes, cudaStream_t st) {
   Carver ws(workspace, workspace_bytes);
-  float* hi_a = ws.take<float>((int64_t)V * d_a);
-  float* lo_a = ws.take<float>((int64_t)V * d_a);
-  float* hi_b = ws.take<float>((int64_t)V * d_b);
-  float* lo_b = ws.take<float>((int64_t)V * d_b);
+  float* hi_a = ws.take<float>((int64_t)N * d_a);
+  float* lo_a = ws.take<float>((int64_t)N * d_a);
+  float* hi_b = ws.take<float>((int64_t)N * d_b);
+  float* lo_b = ws.take<float>((int64_t)N * d_b);
   float* q_a = ws.take<float>(n * d_a);
   float* ql_a = ws.take<float>(n * d_a);
   float* q_b = ws.take<float>(n * d_b);
@@ -1518,8 +1481,8 @@ extern "C" int rgcn_ensemble_rank(int32_t decoder_a, const float* codes_a, const
   int32_t* known_cnt = ws.take<int32_t>(n);
   int rc = RGCN_OK;
   if (!reuse_split) {
-    rc = launch_gemm_split_b(codes_a, d_a, V, d_a, /*transposed=*/0, hi_a, lo_a, st);
-    if (!rc) rc = launch_gemm_split_b(codes_b, d_b, V, d_b, /*transposed=*/0, hi_b, lo_b, st);
+    rc = launch_gemm_split_b(table_a, d_a, N, d_a, /*transposed=*/0, hi_a, lo_a, st);
+    if (!rc) rc = launch_gemm_split_b(table_b, d_b, N, d_b, /*transposed=*/0, hi_b, lo_b, st);
   }
   if (rc || n == 0) return rc;
   rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
@@ -1528,11 +1491,92 @@ extern "C" int rgcn_ensemble_rank(int32_t decoder_a, const float* codes_a, const
   if (!rc) rc = launch_split_trunc(q_a, ql_a, n * d_a, st);
   if (!rc) rc = launch_split_trunc(q_b, ql_b, n * d_b, st);
   if (rc) return rc;
-  rc = launch_gemm_ensemble_rank_tf32x3(q_a, ql_a, hi_a, lo_a, gs_a, d_a, q_b, ql_b, hi_b, lo_b, gs_b, d_b, (int)n, V,
-                                        weight, 1.0 - weight, gold_col, known_mask, (V + 31) / 32, raw_cnt, known_cnt,
+  rc = launch_gemm_ensemble_rank_tf32x3(q_a, ql_a, hi_a, lo_a, gs_a, d_a, q_b, ql_b, hi_b, lo_b, gs_b, d_b, (int)n, N,
+                                        weight, 1.0 - weight, gold_col, known_mask, (N + 31) / 32, raw_cnt, known_cnt,
                                         st);
   if (rc) return rc;
   return launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
+}
+
+extern "C" int64_t rgcn_ensemble_rank_workspace_bytes(int32_t V, int32_t d_a, int32_t d_b, int64_t n) {
+  if (V <= 0 || d_a <= 0 || d_a % 4 != 0 || d_b <= 0 || d_b % 4 != 0 || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_ensemble_rank_workspace_bytes: bad arguments (need V > 0, d > 0, d % 4 == 0, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  return 2 * align_up((int64_t)V * d_a * 4) + 2 * align_up((int64_t)V * d_b * 4) + 2 * align_up(n * d_a * 4) +
+         2 * align_up(n * d_b * 4) + 5 * align_up(n * 4) + 256;
+}
+
+// The argument checks every ensemble entry point shares; relation queries (R > 0) also need R <= Vrel of both.
+static bool ensemble_args_ok(const char* who, RankPrepareFn prep_a, RankPrepareFn prep_b, const float* codes_a,
+                             const float* rel_a, int32_t Vrel_a, int32_t d_a, const float* codes_b, const float* rel_b,
+                             int32_t Vrel_b, int32_t d_b, int32_t V, int32_t R, double weight, const int32_t* X,
+                             int64_t n, int side, const void* out, const void* workspace) {
+  const std::string w(who);
+  if (!prep_a || !prep_b) {
+    rgcn_set_error(w + ": unknown decoder kind (RGCN_DECODER_DISTMULT or RGCN_DECODER_COMPLEX)");
+    return false;
+  }
+  if (d_a <= 0 || d_a % 4 != 0 || d_b <= 0 || d_b % 4 != 0) {
+    rgcn_set_error(w + ": bad arguments (need d % 4 == 0 for both members)");
+    return false;
+  }
+  if (!(weight >= 0.0 && weight <= 1.0)) {   // also refuses NaN
+    rgcn_set_error(w + ": bad arguments (the weight must be finite and in [0, 1])");
+    return false;
+  }
+  if (!codes_a || !rel_a || !codes_b || !rel_b || (n > 0 && (!X || !out)) || !workspace || V <= 0 || Vrel_a <= 0 ||
+      Vrel_b <= 0 || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error(w + ": bad arguments (null pointer or bad size)");
+    return false;
+  }
+  if (side != 0 && side != 1) {
+    rgcn_set_error(w + ": bad arguments (side in {0,1})");
+    return false;
+  }
+  if (R != 0 && (R < 1 || R > Vrel_a || R > Vrel_b)) {
+    rgcn_set_error(w + ": R = " + std::to_string(R) + " relations, need 1 <= R <= Vrel of both members (" +
+                   std::to_string(Vrel_a) + ", " + std::to_string(Vrel_b) + ")");
+    return false;
+  }
+  return true;
+}
+
+static bool ensemble_k_ok(const char* who, int32_t k) {
+  if (k < 1 || k > 128) {
+    rgcn_set_error(std::string(who) + ": k = " + std::to_string(k) + " is out of range (1 <= k <= 128)");
+    return false;
+  }
+  return true;
+}
+
+static bool ensemble_workspace_ok(const char* who, int64_t need, int64_t workspace_bytes) {
+  if (need < 0 || workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small");
+    return false;
+  }
+  return true;
+}
+
+extern "C" int rgcn_ensemble_rank(int32_t decoder_a, const float* codes_a, const float* rel_a, int32_t Vrel_a,
+                                  int32_t d_a, int32_t decoder_b, const float* codes_b, const float* rel_b,
+                                  int32_t Vrel_b, int32_t d_b, int32_t V, double weight, const int32_t* X, int64_t n,
+                                  int side, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
+                                  int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_ensemble_rank";
+  const RankPrepareFn prep_a = ensemble_prepare(decoder_a), prep_b = ensemble_prepare(decoder_b);
+  if (!ensemble_args_ok(who, prep_a, prep_b, codes_a, rel_a, Vrel_a, d_a, codes_b, rel_b, Vrel_b, d_b, V, 0, weight, X,
+                        n, side, raw_rank, workspace))
+    return RGCN_ERR_INVALID;
+  if (filtered_rank && !known_mask) {
+    rgcn_set_error(std::string(who) + ": bad arguments (filtered ranks need a known mask)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!ensemble_workspace_ok(who, rgcn_ensemble_rank_workspace_bytes(V, d_a, d_b, n), workspace_bytes))
+    return RGCN_ERR_WORKSPACE;
+  return ensemble_rank_body(prep_a, codes_a, prep_b, codes_b, V, codes_a, rel_a, d_a, codes_b, rel_b, d_b, weight, X,
+                            n, side, known_mask, reuse_split, raw_rank, filtered_rank, workspace, workspace_bytes,
+                            (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1709,6 +1753,161 @@ extern "C" int rgcn_complex_relation_topk(const float* codes, const float* rel, 
   return topk_with_queries(who, complex_relation_prepare, rel, R, rgcn_relation_topk_workspace_bytes, codes, rel, V,
                            Vrel, d, X, n, 0, k, exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes,
                            (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Ensemble (R-GCN+) top-k and relation prediction, fused: the two members' entity or relation candidates in one
+// two-member GEMM (k_gemm_ensemble) with the rank epilogue of rgcn_ensemble_rank or the (u, id) top-k epilogue
+// ------------------------------------------------------------------------------------------------
+// Entity top-k workspace: [hi_A V*d_A | lo_A | hi_B V*d_B | lo_B | Q_A n*d_A | Q_A lo | Q_B n*d_B | Q_B lo |
+// cand n*ceil(V/64)*min(k,64) (u, id)]: the head is rgcn_ensemble_rank's, so one workspace with its splits serves
+// both.  The relation workspaces have the same shape with the splits of rel_A[0:R] / rel_B[0:R] and N = R.
+static RankPrepareFn ensemble_relation_prepare(int32_t decoder) {
+  if (decoder == RGCN_DECODER_DISTMULT) return distmult_relation_prepare;
+  if (decoder == RGCN_DECODER_COMPLEX) return complex_relation_prepare;
+  return nullptr;
+}
+
+static int64_t ensemble_topk_bytes(int32_t N, int32_t d_a, int32_t d_b, int64_t n, int32_t k) {
+  if (N <= 0 || d_a <= 0 || d_a % 4 != 0 || d_b <= 0 || d_b % 4 != 0 || n < 0 || n > 0x7fffffffLL || k < 1 ||
+      k > 128)
+    return RGCN_ERR_INVALID;
+  const int64_t cand_per_row = (int64_t)((N + 63) / 64) * ensemble_topk_per_tile(k) * 16;
+  if (n > 0 && 8 * ((int64_t)d_a + d_b) + cand_per_row > ((int64_t)1 << 60) / n) return RGCN_ERR_INVALID;
+  return 2 * align_up((int64_t)N * d_a * 4) + 2 * align_up((int64_t)N * d_b * 4) + 2 * align_up(n * d_a * 4) +
+         2 * align_up(n * d_b * 4) + align_up(n * cand_per_row) + 256;
+}
+
+extern "C" int64_t rgcn_ensemble_topk_workspace_bytes(int32_t V, int32_t d_a, int32_t d_b, int64_t n, int32_t k) {
+  const int64_t b = ensemble_topk_bytes(V, d_a, d_b, n, k);
+  if (b < 0)
+    rgcn_set_error("rgcn_ensemble_topk_workspace_bytes: bad arguments (need V > 0, d > 0, d % 4 == 0, 0 <= n < 2^31, "
+                   "1 <= k <= 128)");
+  return b;
+}
+
+extern "C" int64_t rgcn_ensemble_relation_rank_workspace_bytes(int32_t R, int32_t d_a, int32_t d_b, int64_t n) {
+  if (R <= 0) {
+    rgcn_set_error("rgcn_ensemble_relation_rank_workspace_bytes: bad arguments (need R > 0)");
+    return RGCN_ERR_INVALID;
+  }
+  return rgcn_ensemble_rank_workspace_bytes(R, d_a, d_b, n);   // the same layout with N = R
+}
+
+extern "C" int64_t rgcn_ensemble_relation_topk_workspace_bytes(int32_t R, int32_t d_a, int32_t d_b, int64_t n,
+                                                               int32_t k) {
+  const int64_t b = ensemble_topk_bytes(R, d_a, d_b, n, k);
+  if (b < 0)
+    rgcn_set_error("rgcn_ensemble_relation_topk_workspace_bytes: bad arguments (need R > 0, d > 0, d % 4 == 0, "
+                   "0 <= n < 2^31, 1 <= k <= 128)");
+  return b;
+}
+
+// The body of the two top-k entry points after their checks (candidates: the first N rows of table_a / table_b)
+static int ensemble_topk_body(RankPrepareFn prep_a, const float* table_a, RankPrepareFn prep_b, const float* table_b,
+                              int32_t N, const float* codes_a, const float* rel_a, int32_t d_a, const float* codes_b,
+                              const float* rel_b, int32_t d_b, double weight, const int32_t* X, int64_t n, int side,
+                              int32_t k, const uint32_t* exclude_mask, int reuse_split, int32_t* ids, double* u,
+                              double* scores, void* workspace, int64_t workspace_bytes, cudaStream_t st) {
+  const int kt = ensemble_topk_per_tile(k), tn = (N + 63) / 64;
+  Carver ws(workspace, workspace_bytes);
+  float* hi_a = ws.take<float>((int64_t)N * d_a);
+  float* lo_a = ws.take<float>((int64_t)N * d_a);
+  float* hi_b = ws.take<float>((int64_t)N * d_b);
+  float* lo_b = ws.take<float>((int64_t)N * d_b);
+  float* q_a = ws.take<float>(n * d_a);
+  float* ql_a = ws.take<float>(n * d_a);
+  float* q_b = ws.take<float>(n * d_b);
+  float* ql_b = ws.take<float>(n * d_b);
+  EnsCand* cand = ws.take<EnsCand>(n * tn * kt);
+  int rc = RGCN_OK;
+  if (!reuse_split) {
+    rc = launch_gemm_split_b(table_a, d_a, N, d_a, /*transposed=*/0, hi_a, lo_a, st);
+    if (!rc) rc = launch_gemm_split_b(table_b, d_b, N, d_b, /*transposed=*/0, hi_b, lo_b, st);
+  }
+  if (rc || n == 0) return rc;
+  rc = prep_a(codes_a, rel_a, d_a, X, n, side, q_a, nullptr, nullptr, st);
+  if (!rc) rc = prep_b(codes_b, rel_b, d_b, X, n, side, q_b, nullptr, nullptr, st);
+  if (!rc) rc = launch_split_trunc(q_a, ql_a, n * d_a, st);
+  if (!rc) rc = launch_split_trunc(q_b, ql_b, n * d_b, st);
+  if (!rc)
+    rc = launch_gemm_ensemble_topk_tf32x3(q_a, ql_a, hi_a, lo_a, d_a, q_b, ql_b, hi_b, lo_b, d_b, (int)n, N, weight,
+                                          1.0 - weight, exclude_mask, (N + 31) / 32, k, cand, st);
+  if (rc) return rc;
+  return launch_ensemble_topk_merge(cand, n, tn * kt, k, ids, u, scores, st);
+}
+
+extern "C" int rgcn_ensemble_topk(int32_t decoder_a, const float* codes_a, const float* rel_a, int32_t Vrel_a,
+                                  int32_t d_a, int32_t decoder_b, const float* codes_b, const float* rel_b,
+                                  int32_t Vrel_b, int32_t d_b, int32_t V, double weight, const int32_t* X, int64_t n,
+                                  int side, int32_t k, const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
+                                  double* u, double* scores, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_ensemble_topk";
+  const RankPrepareFn prep_a = ensemble_prepare(decoder_a), prep_b = ensemble_prepare(decoder_b);
+  if (!ensemble_args_ok(who, prep_a, prep_b, codes_a, rel_a, Vrel_a, d_a, codes_b, rel_b, Vrel_b, d_b, V, 0, weight, X,
+                        n, side, ids, workspace) ||
+      !ensemble_k_ok(who, k))
+    return RGCN_ERR_INVALID;
+  if (n > 0 && (!u || !scores)) {
+    rgcn_set_error(std::string(who) + ": bad arguments (null pointer)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!ensemble_workspace_ok(who, ensemble_topk_bytes(V, d_a, d_b, n, k), workspace_bytes)) return RGCN_ERR_WORKSPACE;
+  return ensemble_topk_body(prep_a, codes_a, prep_b, codes_b, V, codes_a, rel_a, d_a, codes_b, rel_b, d_b, weight, X, n,
+                            side, k, exclude_mask, reuse_split, ids, u, scores, workspace, workspace_bytes,
+                            (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_ensemble_relation_rank(int32_t decoder_a, const float* codes_a, const float* rel_a,
+                                           int32_t Vrel_a, int32_t d_a, int32_t decoder_b, const float* codes_b,
+                                           const float* rel_b, int32_t Vrel_b, int32_t d_b, int32_t V, int32_t R,
+                                           double weight, const int32_t* X, int64_t n, const uint32_t* known_mask,
+                                           int reuse_split, int32_t* raw_rank, int32_t* filtered_rank,
+                                           void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_ensemble_relation_rank";
+  const RankPrepareFn prep_a = ensemble_relation_prepare(decoder_a), prep_b = ensemble_relation_prepare(decoder_b);
+  if (R <= 0) {
+    rgcn_set_error(std::string(who) + ": R = " + std::to_string(R) + " relations, need R >= 1");
+    return RGCN_ERR_INVALID;
+  }
+  if (!ensemble_args_ok(who, prep_a, prep_b, codes_a, rel_a, Vrel_a, d_a, codes_b, rel_b, Vrel_b, d_b, V, R, weight, X,
+                        n, 0, raw_rank, workspace))
+    return RGCN_ERR_INVALID;
+  if (filtered_rank && !known_mask) {
+    rgcn_set_error(std::string(who) + ": bad arguments (filtered ranks need a known mask)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!ensemble_workspace_ok(who, rgcn_ensemble_rank_workspace_bytes(R, d_a, d_b, n), workspace_bytes))
+    return RGCN_ERR_WORKSPACE;
+  return ensemble_rank_body(prep_a, rel_a, prep_b, rel_b, R, codes_a, rel_a, d_a, codes_b, rel_b, d_b, weight, X, n, 0,
+                            known_mask, reuse_split, raw_rank, filtered_rank, workspace, workspace_bytes,
+                            (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_ensemble_relation_topk(int32_t decoder_a, const float* codes_a, const float* rel_a,
+                                           int32_t Vrel_a, int32_t d_a, int32_t decoder_b, const float* codes_b,
+                                           const float* rel_b, int32_t Vrel_b, int32_t d_b, int32_t V, int32_t R,
+                                           double weight, const int32_t* X, int64_t n, int32_t k,
+                                           const uint32_t* exclude_mask, int reuse_split, int32_t* ids, double* u,
+                                           double* scores, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_ensemble_relation_topk";
+  const RankPrepareFn prep_a = ensemble_relation_prepare(decoder_a), prep_b = ensemble_relation_prepare(decoder_b);
+  if (R <= 0) {
+    rgcn_set_error(std::string(who) + ": R = " + std::to_string(R) + " relations, need R >= 1");
+    return RGCN_ERR_INVALID;
+  }
+  if (!ensemble_args_ok(who, prep_a, prep_b, codes_a, rel_a, Vrel_a, d_a, codes_b, rel_b, Vrel_b, d_b, V, R, weight, X,
+                        n, 0, ids, workspace) ||
+      !ensemble_k_ok(who, k))
+    return RGCN_ERR_INVALID;
+  if (n > 0 && (!u || !scores)) {
+    rgcn_set_error(std::string(who) + ": bad arguments (null pointer)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!ensemble_workspace_ok(who, ensemble_topk_bytes(R, d_a, d_b, n, k), workspace_bytes)) return RGCN_ERR_WORKSPACE;
+  return ensemble_topk_body(prep_a, rel_a, prep_b, rel_b, R, codes_a, rel_a, d_a, codes_b, rel_b, d_b, weight, X, n, 0,
+                            k, exclude_mask, reuse_split, ids, u, scores, workspace, workspace_bytes,
+                            (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -9,7 +9,7 @@
 // cvt.rna.tf32.f32) and three MMAs are issued per K-step:  a_hi*b_hi + a_hi*b_lo + a_lo*b_hi
 // (the a_lo*b_lo term is below fp32 rounding).
 //
-// Three kernels (k_gemm_tf32x3<EPI>, k_gemm_tn_tf32x3, k_gemm_ensemble_rank): 384 threads = three warpgroups,
+// Three kernels (k_gemm_tf32x3<EPI>, k_gemm_tn_tf32x3, k_gemm_ensemble<EPI>): 384 threads = three warpgroups,
 // 1 CTA/SM, 128-row tiles, 32-wide K blocks.
 //   warpgroup 0     producer: global fp32 -> registers -> (hi, lo) -> st.shared in the K-major SWIZZLE_128B layout
 //                   that wgmma reads (TF32 wgmma takes K-major operands only, so the TN kernel transposes here);
@@ -21,14 +21,15 @@
 //                   accumulator registers.
 //   NT: 128x128 tiles, 3-stage smem ring (64 KB per stage: A_hi, A_lo, B_hi, B_lo); TN: 2 such stages plus a ring of
 //   raw fp32 blocks that its producer fills with cp.async and transposes from (see k_gemm_tn_tf32x3); ensemble:
-//   128x64 tiles, 4 stages of 48 KB (see k_gemm_ensemble_rank).
+//   128x64 tiles, 4 stages of 48 KB (see k_gemm_ensemble).
 // The NT and ensemble kernels are persistent (min(tiles, SMs) CTAs walk the tiles; the producer runs on into the next
 // tile while the consumers finish the last one); the TN kernel keeps one tile (x split-K) per CTA.
 //
 // The epilogues of the NT kernel are functors (StoreEpi, RankEpi, HighwayEpi, VarEpi, TopKEpi, BceEpi): a struct with
 // the epilogue's data and one operator()(tile, big, small) over the accumulator fragment.  Epilogue<EPI> maps the
 // integer of k_gemm_tf32x3<EPI> to its functor (EPI_STORE = 0 .. EPI_BCE = 5).  A new epilogue is one such struct, one
-// Epilogue<n> line and one launcher that ends in launch_persistent.
+// Epilogue<n> line and one launcher that ends in launch_persistent.  The two-member kernel k_gemm_ensemble<EPI> takes its
+// functor (EnsRankEpi, EnsTopKEpi) directly, over both members' accumulators.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -890,18 +891,21 @@ __global__ void k_split_b_interleave(const float* __restrict__ Wmu, const float*
 }
 
 // ------------------------------------------------------------------------------------------------
-// ENSEMBLE RANKING (R-GCN+: the weighted sum of two models' scores, tools/ensemble.py `weighted_sum`): every tile
+// ENSEMBLE SCORING (R-GCN+: the weighted sum of two models' scores, tools/ensemble.py `weighted_sum`): every tile
 // runs the K blocks of member A (Q_A [M, K_A] against codes_A [N, K_A]) and then those of member B into separate
-// accumulators; the epilogue forms each member's float32 sigmoid score as RankEpi does, combines them in float64,
-//   c = w s_A + (1 - w) s_B   (separately rounded multiplies and add: the reference tool's Python arithmetic),
-// and counts c >= G into raw_cnt / known_cnt by RankEpi's rules, G = w g_A + (1 - w) g_B.  [M, N] is never written.
+// accumulators, and the epilogue k_gemm_ensemble<EPI> was instantiated with combines them.  [M, N] is never written.
+//   EnsRankEpi: each member's float32 sigmoid score as RankEpi forms it, combined in float64,
+//     c = w s_A + (1 - w) s_B   (separately rounded multiplies and add: the reference tool's Python arithmetic),
+//     and c >= G counted into raw_cnt / known_cnt by RankEpi's rules, G = w g_A + (1 - w) g_B.
+//   EnsTopKEpi: each row's best k of the tile by u = w sigma(-E_A) + (1 - w) sigma(-E_B) ascending (see there).
+// The candidates (N columns) are entity codes or, for relation queries (h, ?, t), the first R relation rows.
 //
 // Tile 128 x 64 (wgmma.m64n64k8): two members x (hi*hi, cross terms) x 64 x 64 / 128 threads = 128 accumulator
 // registers per consumer thread, the count of the 128 x 128 single-model kernel.  Both operands come pre-split
 // (the codes by round-to-nearest as for k_gemm_tf32x3, the query rows by the same truncation its producer applies),
 // so the producer only issues asynchronous copies, EN_LOOKAHEAD blocks ahead.  A stage is Q hi/lo (2 x 16 KB) and
 // code hi/lo (2 x 8 KB); four stages fit.  Each output element sees the K steps of its member in the order of the
-// single-model kernel, so w = 1 (w = 0) reproduces member A's (B's) fused ranks.
+// single-model kernel, so w = 1 (w = 0) reproduces member A's (B's) fused ranks and energies.
 // ------------------------------------------------------------------------------------------------
 constexpr int EN_BN = 64;
 constexpr int EN_STAGES = 4;
@@ -918,25 +922,195 @@ static_assert(EN_LOOKAHEAD < EN_STAGES, "the lookahead needs a free stage");
 struct EnsMember {
   const float* q_hi;           // [M, K] query rows, split by truncation
   const float* q_lo;
-  const float* c_hi;           // [N, K] entity codes, split by round-to-nearest
+  const float* c_hi;           // [N, K] candidate codes, split by round-to-nearest
   const float* c_lo;
-  const float* gold_sig;       // [M] sigmoid(energy of the gold entity)
+  const float* gold_sig;       // [M] sigmoid(energy of the gold candidate) (rank; nullptr for top-k)
   int K;                       // K % 4 == 0; the leading dimension of all four planes
 };
-struct EnsEpi {
+// What every ensemble epilogue starts with: the operands the producer copies and the weights.
+struct EnsPair {
   EnsMember a, b;
   double w, omw;               // weight of A and 1 - w (formed once on the host, in double)
+};
+// The accumulators of one tile: member A's and member B's (hi*hi, cross terms)
+using EnsAcc = float[EN_FRAG];
+
+struct EnsRankEpi : EnsPair {
   const int32_t* gold_col;     // [M]
   const uint32_t* known;       // [M, words] or nullptr
   int words;
   int32_t* raw_cnt;            // [M] += #{v : c_v >= G}
   int32_t* known_cnt;          // [M] += #{known v : c_v >= G}
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const EnsAcc& big_a, const EnsAcc& small_a,
+                                             const EnsAcc& big_b, const EnsAcc& small_b) const {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = t.r0 + 8 * h;
+      int raw = 0, kn = 0;
+      if (row < t.M) {
+        const double G = __dadd_rn(__dmul_rn(w, (double)__ldg(a.gold_sig + row)),
+                                   __dmul_rn(omw, (double)__ldg(b.gold_sig + row)));
+        const int gold_c = __ldg(gold_col + row);
+        for_each_col<EN_FRAG>(t, h, known, words, [&](int r, int, int col, uint32_t word) {
+          const float sa = sigmoid_ref(big_a[r] + small_a[r]);
+          const float sb = sigmoid_ref(big_b[r] + small_b[r]);
+          const double cv = __dadd_rn(__dmul_rn(w, (double)sa), __dmul_rn(omw, (double)sb));
+          if (col < t.N && (cv >= G || col == gold_c)) {   // the gold entity always counts
+            ++raw;
+            kn += (int)col_bit(word, col);
+          }
+        });
+      }
+      rank_counts_flush(raw, kn, row, t.M, raw_cnt, known_cnt, t.lane);
+    }
+  }
+};
+
+// exp(-x) for x >= 0 in double: x = n ln2 + r (Cody-Waite, |r| <= ln2 / 2), exp(-r) by its degree-12 Taylor
+// polynomial (within 5e-16 relative of exp over [0, 800]), 2^-n applied as two exact power-of-two factors so that
+// results down to the smallest subnormal come out; x > 800 gives 0.  Written out rather than the library's exp(),
+// whose range handling keeps more registers live than the top-k epilogue has beside its accumulators.
+__device__ __forceinline__ double exp_neg_d(double x) {
+  if (!(x <= 800.0)) return 0.0;
+  const double n = rint(x * 1.4426950408889634);
+  double r = fma(-n, 6.93147180369123816490e-01, x);
+  r = fma(-n, 1.90821492927058770002e-10, r);
+  const double s = -r;
+  double p = 2.08767569878680989792e-09;                     // 1 / 12!
+  p = fma(p, s, 2.50521083854417187751e-08);                 // 1 / 11!
+  p = fma(p, s, 2.75573192239858906526e-07);
+  p = fma(p, s, 2.75573192239858906526e-06);
+  p = fma(p, s, 2.48015873015873015873e-05);
+  p = fma(p, s, 1.98412698412698412698e-04);
+  p = fma(p, s, 1.38888888888888888889e-03);
+  p = fma(p, s, 8.33333333333333333333e-03);
+  p = fma(p, s, 4.16666666666666666667e-02);
+  p = fma(p, s, 1.66666666666666666667e-01);
+  p = fma(p, s, 0.5);
+  p = fma(p, s, 1.0);
+  p = fma(p, s, 1.0);
+  const int ni = (int)n, n1 = ni >> 1, n2 = ni - n1;           // 0 <= n1, n2 <= 578
+  return (p * __hiloint2double((1023 - n1) << 20, 0)) * __hiloint2double((1023 - n2) << 20, 0);
+}
+// sigma(-E) = 1 / (1 + exp(E)) in double from a float32 energy, through t = exp(-|E|) in [0, 1] so that the one
+// reciprocal is of 1 + t in [1, 2]: sigma(-E) = 1 / (1 + t) for E <= 0 and t / (1 + t) for E > 0.  For E > 0 it does
+// not saturate until t underflows (E > 745); for E < 0 it rounds to exactly 1 once exp(E) < 2^-53 (E < about -37).
+// The reciprocal is MUFU's approximation refined by two Newton steps (within an ulp): the IEEE division would call its
+// slow path, and a call spills the epilogue.
+__device__ __forceinline__ double sigmoid_neg_d(float e) {
+  const double t = exp_neg_d(fabs((double)e));
+  const double d = 1.0 + t;
+  double r;
+  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(d));
+  r = fma(r, fma(-d, r, 1.0), r);
+  r = fma(r, fma(-d, r, 1.0), r);
+  return e > 0.f ? t * r : r;
+}
+
+// TOP-K epilogue of the ensemble: for each row the tile's best min(k, 64) eligible (u, column) pairs, u ascending and
+// the smaller column first on ties, where
+//   u = w sigma(-E_A) + (1 - w) sigma(-E_B)   (double; separately rounded products and sum)
+// is 1 - c in exact arithmetic, so ascending u is descending combined score without the saturation of the float32
+// sigmoid.  Columns >= N and columns whose bit is set in `excl` are not eligible.  The pairs go in that order to
+// cand[(row * tn + tile column) * kt + p]; the tail past the eligible columns is (+inf, -1).
+// The energies of both tile rows are formed first (32 floats per member and lane: the accumulators die there), then
+// one row at a time: every lane forms the u of its 16 eligible columns of the row (value i = 2 j + e at column
+// c0 + 8 j + e, so a lane's columns increase with i) into its own slots of a 32 KB shared-memory scratch after the
+// stage ring, and keeps the best of them in registers.  Each round the quad of lanes lane & ~3 (the row's 64 columns)
+// keeps the best of its four by two shuffles on (u, column), and only the lane that owned it rescans its slots, as
+// the merge kernel does.  166 registers, no spills.
+constexpr int EN_TOPK_NV = EN_FRAG / 2;                                   // columns per lane and row
+constexpr int EN_TOPK_SCRATCH = N_CONSUMERS * EN_TOPK_NV * 8;             // 32 KB
+static_assert(EN_SMEM_BYTES + EN_TOPK_SCRATCH <= 227 * 1024, "ensemble top-k scratch exceeds the shared memory");
+
+struct EnsTopKEpi : EnsPair {
+  const uint32_t* excl;        // [M, words] bit v = candidate v never appears in row m (or nullptr)
+  int words;                   // ceil(N / 32)
+  int kt;                      // candidates per row and tile, min(k, EN_BN)
+  int tn;                      // N tiles
+  EnsCand* cand;               // [M, tn, kt]
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const EnsAcc& big_a, const EnsAcc& small_a,
+                                             const EnsAcc& big_b, const EnsAcc& small_b) const {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t raw = smem_u32(smem_raw), aligned = (raw + 1023u) & ~1023u;
+    // this lane's slot i is ubuf[i * N_CONSUMERS]: a warp's accesses are consecutive doubles
+    double* ubuf = reinterpret_cast<double*>(smem_raw + (aligned - raw) + EN_STAGES * EN_STAGE_BYTES) +
+                   (t.warp * 32 + t.lane);
+    const bool writer = (t.lane & 3) == 0;
+    const EnsCand none{INFINITY, -1, 0};
+    float ea[2][EN_TOPK_NV], eb[2][EN_TOPK_NV];   // the members' energies
+    uint32_t eligible[2];                          // bit i: column i of row r0 + 8 h may be returned
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      eligible[h] = 0u;
+      for_each_col<EN_FRAG>(t, h, excl, words, [&](int r, int i, int col, uint32_t word) {
+        ea[h][i] = big_a[r] + small_a[r];
+        eb[h][i] = big_b[r] + small_b[r];
+        if (t.r0 + 8 * h < t.M && col < t.N && !col_bit(word, col)) eligible[h] |= 1u << i;
+      });
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = t.r0 + 8 * h;
+      const bool row_ok = row < t.M;
+      uint32_t left = eligible[h];
+#pragma unroll
+      for (int i = 0; i < EN_TOPK_NV; ++i)   // u of the eligible columns only
+        if ((left >> i) & 1u)
+          ubuf[i * N_CONSUMERS] = __dadd_rn(__dmul_rn(w, sigmoid_neg_d(ea[h][i])),
+                                            __dmul_rn(omw, sigmoid_neg_d(eb[h][i])));
+      int bi;
+      double bu;
+      auto rescan = [&]() {   // the lane's best (u, i) among its slots still left
+        bi = -1;
+        bu = INFINITY;
+#pragma unroll
+        for (int i = 0; i < EN_TOPK_NV; ++i)
+          if ((left >> i) & 1u) {
+            const double x = ubuf[i * N_CONSUMERS];
+            if (bi < 0 || x < bu) {
+              bu = x;
+              bi = i;
+            }
+          }
+      };
+      rescan();
+      // candidate p of this row (formed at the store: a live pointer would cost a register pair)
+      auto slot = [&](int p) { return cand + ((size_t)row * tn + (size_t)(t.n0 / EN_BN)) * kt + p; };
+      int p = 0;
+      for (; p < kt; ++p) {
+        const int mine = bi < 0 ? 0x7fffffff : t.c0 + 8 * (bi >> 1) + (bi & 1);
+        double qu = bu;
+        int qc = mine;
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          const double ou = __shfl_xor_sync(0xffffffffu, qu, o);
+          const int oc = __shfl_xor_sync(0xffffffffu, qc, o);
+          if (oc != 0x7fffffff && (qc == 0x7fffffff || ou < qu || (ou == qu && oc < qc))) {
+            qu = ou;
+            qc = oc;
+          }
+        }
+        if (!__any_sync(0xffffffffu, qc != 0x7fffffff)) break;   // the warp's rows ran dry
+        if (bi >= 0 && qc == mine) {
+          left &= ~(1u << bi);
+          rescan();
+        }
+        if (writer && row_ok) *slot(p) = qc == 0x7fffffff ? none : EnsCand{qu, qc, 0};
+      }
+      if (writer && row_ok)
+        for (; p < kt; ++p) *slot(p) = none;
+    }
+  }
 };
 
 // Persistent like k_gemm_tf32x3 (N tiles fastest); a tile is num_kb_a + num_kb_b consecutive k-blocks of the CTA's
-// stage sequence.
+// stage sequence.  EPI: EnsRankEpi or EnsTopKEpi.
+template <class EPI>
 __global__ void __launch_bounds__(N_THREADS, 1)
-    k_gemm_ensemble_rank(int M, int N, int n_tiles, EnsEpi re) {
+    k_gemm_ensemble(int M, int N, int n_tiles, const EPI re) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[EN_STAGES], empty_bar[EN_STAGES];
   const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -1024,26 +1198,7 @@ __global__ void __launch_bounds__(N_THREADS, 1)
       consume_tile<EnsStage>(smem_base, full_bar, empty_bar, ti * nkb + nkb_a, nkb_b, a_rows, big_b, small_b);
       const int r0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = n0 + 2 * (lane & 3);
       const TileCtx t{tile, m0, n0, r0, c0, M, N, lane, warp};
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = t.r0 + 8 * h;
-        int raw = 0, kn = 0;
-        if (row < M) {
-          const double G = __dadd_rn(__dmul_rn(re.w, (double)__ldg(re.a.gold_sig + row)),
-                                     __dmul_rn(re.omw, (double)__ldg(re.b.gold_sig + row)));
-          const int gold_c = __ldg(re.gold_col + row);
-          for_each_col<EN_FRAG>(t, h, re.known, re.words, [&](int r, int, int col, uint32_t word) {
-            const float sa = sigmoid_ref(big_a[r] + small_a[r]);
-            const float sb = sigmoid_ref(big_b[r] + small_b[r]);
-            const double cv = __dadd_rn(__dmul_rn(re.w, (double)sa), __dmul_rn(re.omw, (double)sb));
-            if (col < N && (cv >= G || col == gold_c)) {   // the gold entity always counts
-              ++raw;
-              kn += (int)col_bit(word, col);
-            }
-          });
-        }
-        rank_counts_flush(raw, kn, row, M, re.raw_cnt, re.known_cnt, lane);
-      }
+      re(t, big_a, small_a, big_b, small_b);
     }
   }
 }
@@ -1189,7 +1344,7 @@ int launch_split_trunc(float* a, float* lo, int64_t count, cudaStream_t st) {
   return rgcn_check_cuda(cudaGetLastError(), "k_split_trunc");
 }
 
-// Two-member ranking GEMM (see k_gemm_ensemble_rank); the counts accumulate (+=) into raw_cnt / known_cnt.
+// Two-member ranking GEMM (see k_gemm_ensemble); the counts accumulate (+=) into raw_cnt / known_cnt.
 int launch_gemm_ensemble_rank_tf32x3(const float* qa_hi, const float* qa_lo, const float* ca_hi, const float* ca_lo,
                                      const float* gold_sig_a, int Ka, const float* qb_hi, const float* qb_lo,
                                      const float* cb_hi, const float* cb_lo, const float* gold_sig_b, int Kb, int M,
@@ -1201,10 +1356,40 @@ int launch_gemm_ensemble_rank_tf32x3(const float* qa_hi, const float* qa_lo, con
     return RGCN_ERR_INVALID;
   }
   const int64_t tiles = tiles_of(M, N, EN_BN);
-  EnsEpi re{{qa_hi, qa_lo, ca_hi, ca_lo, gold_sig_a, Ka}, {qb_hi, qb_lo, cb_hi, cb_lo, gold_sig_b, Kb}, w, omw,
-            gold_col, known, words, raw_cnt, known_cnt};
-  return launch_persistent<k_gemm_ensemble_rank>("gemm_ensemble_rank_tf32x3", "k_gemm_ensemble_rank", EN_SMEM_BYTES,
-                                                 tiles, TILE_LIMIT, st, M, N, (int)tiles, re);
+  EnsRankEpi re;
+  static_cast<EnsPair&>(re) = {{qa_hi, qa_lo, ca_hi, ca_lo, gold_sig_a, Ka}, {qb_hi, qb_lo, cb_hi, cb_lo, gold_sig_b, Kb},
+                               w, omw};
+  re.gold_col = gold_col;
+  re.known = known;
+  re.words = words;
+  re.raw_cnt = raw_cnt;
+  re.known_cnt = known_cnt;
+  return launch_persistent<k_gemm_ensemble<EnsRankEpi>>("gemm_ensemble_rank_tf32x3", "k_gemm_ensemble<rank>",
+                                                        EN_SMEM_BYTES, tiles, TILE_LIMIT, st, M, N, (int)tiles, re);
+}
+
+// Two-member top-k GEMM (see EnsTopKEpi): each row's best min(k, 64) eligible (u, column) pairs of every 64-column
+// tile go to cand [M, ceil(N / 64), min(k, 64)].
+int launch_gemm_ensemble_topk_tf32x3(const float* qa_hi, const float* qa_lo, const float* ca_hi, const float* ca_lo,
+                                     int Ka, const float* qb_hi, const float* qb_lo, const float* cb_hi,
+                                     const float* cb_lo, int Kb, int M, int N, double w, double omw,
+                                     const uint32_t* excl, int words, int k, EnsCand* cand, cudaStream_t st) {
+  if (M == 0 || N == 0) return RGCN_OK;
+  if (Ka <= 0 || Ka % 4 != 0 || Kb <= 0 || Kb % 4 != 0 || k < 1 || k > 128) {
+    rgcn_set_error("gemm_ensemble_topk_tf32x3: K > 0 and K % 4 == 0 for both members; 1 <= k <= 128");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t tiles = tiles_of(M, N, EN_BN);
+  EnsTopKEpi te;
+  static_cast<EnsPair&>(te) = {{qa_hi, qa_lo, ca_hi, ca_lo, nullptr, Ka}, {qb_hi, qb_lo, cb_hi, cb_lo, nullptr, Kb},
+                               w, omw};
+  te.excl = excl;
+  te.words = words;
+  te.kt = ensemble_topk_per_tile(k);
+  te.tn = (N + EN_BN - 1) / EN_BN;
+  te.cand = cand;
+  return launch_persistent<k_gemm_ensemble<EnsTopKEpi>>("gemm_ensemble_topk_tf32x3", "k_gemm_ensemble<topk>",
+                                                        EN_SMEM_BYTES + EN_TOPK_SCRATCH, tiles, TILE_LIMIT, st, M, N, (int)tiles, te);
 }
 
 // Highway gate GEMM with the blend epilogue (EPI = 2): z = c2 @ W + bias with W pre-split as Bt = W^T [d, d];

@@ -174,6 +174,25 @@ int launch_gemm_ensemble_rank_tf32x3(const float* qa_hi, const float* qa_lo, con
                                      const float* cb_hi, const float* cb_lo, const float* gold_sig_b, int Kb, int M,
                                      int N, double w, double omw, const int32_t* gold_col, const uint32_t* known,
                                      int words, int32_t* raw_cnt, int32_t* known_cnt, cudaStream_t st);
+// Ensemble top-k candidate: u = w sigma(-E_A) + (1 - w) sigma(-E_B) in double and the column; id -1 = none (u +inf)
+struct EnsCand {
+  double u;
+  int32_t id;
+  int32_t pad;
+};
+// candidates per row and 64-column tile of the ensemble top-k GEMM: a tile has no more than 64 columns to offer
+inline int ensemble_topk_per_tile(int k) { return k < 64 ? k : 64; }
+// Ensemble top-k GEMM: operands as launch_gemm_ensemble_rank_tf32x3; for every row and every 64-column tile the best
+// ensemble_topk_per_tile(k) eligible (u, column) pairs -- u ascending, smaller column first on ties; excl bit set or
+// column >= N: not eligible -- in order in cand [M, ceil(N / 64), ensemble_topk_per_tile(k)], the tail (+inf, -1).
+int launch_gemm_ensemble_topk_tf32x3(const float* qa_hi, const float* qa_lo, const float* ca_hi, const float* ca_lo,
+                                     int Ka, const float* qb_hi, const float* qb_lo, const float* cb_hi,
+                                     const float* cb_lo, int Kb, int M, int N, double w, double omw,
+                                     const uint32_t* excl, int words, int k, EnsCand* cand, cudaStream_t st);
+// topk.cu -- merge of those candidates: ids [n, k], u [n, k] and c = 1 - u [n, k] (double) of every row's best k in
+// the same order, the tail past the row's eligible columns padded (-1, +inf, 0)
+int launch_ensemble_topk_merge(const EnsCand* cand, int64_t n, int per_row, int k, int32_t* ids, double* u,
+                               double* scores, cudaStream_t st);
 
 int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
                           int M, int N, int K, int accumulate, cudaStream_t st);

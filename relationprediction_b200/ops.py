@@ -909,6 +909,8 @@ class EnsembleRanker(object):
             raise ValueError("the weight must be in [0, 1], got %r" % weight)
         self.a, self.b, self.weight = ranker_a, ranker_b, weight
         self._ws, self._ws_n, self._split_ready = None, -1, False
+        # relation queries keep their own workspace, with both members' splits of rel[0:R] at its head
+        self._rel_ws, self._rel_split_ready = None, False
 
     def rank(self, X, side, known_mask=None):
         """As DistMultRanker.rank, with c = w s_A + (1 - w) s_B in place of the single score.  X int32 [n,3] CUDA;
@@ -935,6 +937,114 @@ class EnsembleRanker(object):
         _lib.check(rc, "rgcn_ensemble_rank")
         self._split_ready = True
         return raw, filt
+
+    def _members(self):
+        """The leading arguments of every ensemble entry point: both members' decoder, codes, relation table,
+        table rows and width."""
+        a, b = self.a, self.b
+        return (a.DECODER, _ptr(a.codes), _ptr(a.rel), a.rel.shape[0], a.codes.shape[1],
+                b.DECODER, _ptr(b.codes), _ptr(b.rel), b.rel.shape[0], b.codes.shape[1])
+
+    def _outputs(self, n, k):
+        dev = self.a.codes.device
+        return (torch.empty((n, k), dtype=torch.int32, device=dev), torch.empty((n, k), dtype=torch.float64, device=dev),
+                torch.empty((n, k), dtype=torch.float64, device=dev))
+
+    def top_k(self, X, side, k, exclude_mask=None):
+        """The k entities of best combined score for every triple of X (int32 [n,3] CUDA; side 0 predicts subjects,
+        1 objects; the predicted column is not read), in the order of u = w sigma(-E_A) + (1 - w) sigma(-E_B)
+        ascending (double), the smaller id first on ties, never one whose bit is set in exclude_mask (uint32
+        [n, ceil(V/32)] CUDA, as int32, or None).  Returns CUDA tensors (ids int32 [n,k], u float64 [n,k], scores
+        float64 [n,k] = 1 - u); rows with fewer than k eligible entities end in (-1, +inf, 0).  Queries go to the
+        library in chunks whose workspace beyond the splits stays under TOPK_CHUNK_BYTES; the entity splits are
+        shared with rank."""
+        lib = _lib.load()
+        a = self.a
+        V, d_a = a.codes.shape
+        d_b = self.b.codes.shape[1]
+        a._check_rows(X, exclude_mask, "exclude_mask")
+        k, n = int(k), X.shape[0]
+        chunk, nb = a._chunk_rows(n, lambda m: lib.rgcn_ensemble_topk_workspace_bytes(V, d_a, d_b, m, k),
+                                  "rgcn_ensemble_topk_workspace_bytes")
+        dev = a.codes.device
+        if self._ws is None or self._ws.numel() < nb:
+            self._ws, self._ws_n, self._split_ready = _workspace(nb, dev), -1, False
+        ids, u, scores = self._outputs(n, k)
+        for c0 in range(0, max(n, 1), chunk):
+            c1 = min(n, c0 + chunk)
+            rc = lib.rgcn_ensemble_topk(*self._members(), V, self.weight, _ptr(X[c0:c1]), c1 - c0, int(side), k,
+                                        _ptr(None if exclude_mask is None else exclude_mask[c0:c1]),
+                                        int(self._split_ready), _ptr(ids[c0:c1]), _ptr(u[c0:c1]),
+                                        _ptr(scores[c0:c1]), _ptr(self._ws), self._ws.numel(), _stream(dev))
+            _lib.check(rc, "rgcn_ensemble_topk")
+            self._split_ready = True
+        return ids, u, scores
+
+    # ---- relation queries (h, ?, t) over the first R relations of both members ----
+    @property
+    def relation_count(self):
+        """R, the relation candidates both members share; ValueError when they differ."""
+        if self.a.relation_count != self.b.relation_count:
+            raise ValueError("the members predict different relation sets (%d and %d relations)"
+                             % (self.a.relation_count, self.b.relation_count))
+        return self.a.relation_count
+
+    def _relation_calls(self, X, mask, name, workspace_bytes):
+        """As DistMultRanker._relation_calls, with the ensemble's own relation workspace (both members' splits of
+        rel[0:R] at its head).  Relation queries need both members to have the same R candidates; entity ranking
+        and top-k do not."""
+        a = self.a
+        a._check_rows(X, mask, name, self.relation_count, "R")
+        n = X.shape[0]
+        chunk, nb = a._chunk_rows(n, workspace_bytes, "relation workspace bytes")
+        if self._rel_ws is None or self._rel_ws.numel() < nb:
+            self._rel_ws, self._rel_split_ready = _workspace(nb, a.codes.device), False
+        for c0 in range(0, max(n, 1), chunk):
+            yield c0, min(n, c0 + chunk)
+            self._rel_split_ready = True
+
+    def rank_relations(self, X, known_mask=None):
+        """Ranks of the relation X[t, 1] in [0, R) among the R relations for the pair (X[t, 0], X[t, 2]) under the
+        combined score, by the rules of rank.  X int32 [n,3] CUDA; known_mask uint32 [n, ceil(R/32)] CUDA (as int32)
+        or None.  Returns (raw_rank, filtered_rank or None) int32 CUDA tensors."""
+        lib = _lib.load()
+        R, V = self.relation_count, self.a.codes.shape[0]
+        d_a, d_b = self.a.codes.shape[1], self.b.codes.shape[1]
+        dev = self.a.codes.device
+        n = X.shape[0]
+        raw = torch.empty(n, dtype=torch.int32, device=dev)
+        filt = torch.empty(n, dtype=torch.int32, device=dev) if known_mask is not None else None
+        for c0, c1 in self._relation_calls(X, known_mask, "known_mask",
+                                           lambda m: lib.rgcn_ensemble_relation_rank_workspace_bytes(R, d_a, d_b, m)):
+            rc = lib.rgcn_ensemble_relation_rank(*self._members(), V, R, self.weight, _ptr(X[c0:c1]), c1 - c0,
+                                                 _ptr(None if known_mask is None else known_mask[c0:c1]),
+                                                 int(self._rel_split_ready), _ptr(raw[c0:c1]),
+                                                 _ptr(None if filt is None else filt[c0:c1]), _ptr(self._rel_ws),
+                                                 self._rel_ws.numel(), _stream(dev))
+            _lib.check(rc, "rgcn_ensemble_relation_rank")
+        return raw, filt
+
+    def top_k_relations(self, X, k, exclude_mask=None):
+        """The k relations of the first R of best combined score for every pair (X[t, 0], ?, X[t, 2]) (the relation
+        column is not read), in top_k's order, never one whose bit is set in exclude_mask (uint32 [n, ceil(R/32)]
+        CUDA, as int32, or None).  Returns CUDA tensors (ids int32 [n,k], u float64 [n,k], scores float64 [n,k]);
+        rows with fewer than k eligible relations end in (-1, +inf, 0)."""
+        lib = _lib.load()
+        R, V, k = self.relation_count, self.a.codes.shape[0], int(k)
+        d_a, d_b = self.a.codes.shape[1], self.b.codes.shape[1]
+        dev = self.a.codes.device
+        n = X.shape[0]
+        ids, u, scores = self._outputs(n, k)
+        for c0, c1 in self._relation_calls(
+                X, exclude_mask, "exclude_mask",
+                lambda m: lib.rgcn_ensemble_relation_topk_workspace_bytes(R, d_a, d_b, m, k)):
+            rc = lib.rgcn_ensemble_relation_topk(*self._members(), V, R, self.weight, _ptr(X[c0:c1]), c1 - c0, k,
+                                                 _ptr(None if exclude_mask is None else exclude_mask[c0:c1]),
+                                                 int(self._rel_split_ready), _ptr(ids[c0:c1]), _ptr(u[c0:c1]),
+                                                 _ptr(scores[c0:c1]), _ptr(self._rel_ws), self._rel_ws.numel(),
+                                                 _stream(dev))
+            _lib.check(rc, "rgcn_ensemble_relation_topk")
+        return ids, u, scores
 
 
 # ---- 1-N training (distmult_one_to_n / rgcn_complex_one_to_n, include/rgcn_b200.h) ----

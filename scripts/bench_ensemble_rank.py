@@ -1,14 +1,18 @@
 """Fused R-GCN+ ensemble ranking next to two single-model fused rankings and the unfused torch composition, at the
 FB15k-237 and FB15k test shapes (both sides, d_A = d_B = 500, DistMult members, random codes, seeded):
 
-  python scripts/bench_ensemble_rank.py [--reps N] [--chunk C]
+  python scripts/bench_ensemble_rank.py [--reps N] [--chunk C] [--topk K] [--relations]
 
   fused ensemble   ops.EnsembleRanker.rank, both sides (two prepare kernels, the dual-accumulator rank GEMM)
   two singles      DistMultRanker.rank of member A plus that of member B, both sides
   torch            per chunk of C queries: fp32 matmuls of both members, sigmoid, the float64 combination
                    w s_A + (1 - w) s_B and the >= counts against the gold score (raw and filtered), both sides
-Times are means of CUDA-event windows (L2 flushed before each), after a warm-up.  The card's name and power limit
-and one JSON line per shape are printed."""
+--topk K times entity top-k instead (EnsembleRanker.top_k, both sides, no exclusions; the singles are
+DistMultRanker.top_k; torch forms u = w sigma(-E_A) + (1 - w) sigma(-E_B) in float64 per chunk and takes torch.topk).
+--relations times the relation queries (h, ?, t) over the R relations: rank_relations, or top_k_relations with
+--topk; these legs alternate the three paths within every repetition and report the median of each.  The ranking
+times are means.  Every time is a CUDA-event window with L2 flushed before it, after a warm-up.  The card's name and
+power limit and one JSON line per shape are printed."""
 import argparse
 import json
 import subprocess
@@ -29,6 +33,8 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--chunk", type=int, default=4096, help="queries per torch matmul")
+    ap.add_argument("--topk", type=int, default=None, metavar="K", help="time top-k prediction with K answers")
+    ap.add_argument("--relations", action="store_true", help="time relation queries (h, ?, t)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_ensemble_rank.py needs a CUDA device")
@@ -69,6 +75,12 @@ def main():
             dense.append((torch.as_tensor(rows, device=dev), torch.as_tensor(np.concatenate(known), device=dev)))
         ra, rb = (ops.DistMultRanker(c, r) for c, r in members)
         ens = ops.EnsembleRanker(ra, rb, W)
+        if args.topk is not None or args.relations:
+            leg = prediction_leg(args, name, n, V, R, members, X, Xl, masks, ra, rb, ens, flush)
+            print(json.dumps({"shape": name, "n": n, "V": V, "R": R, "d": D, "weight": W, "card": card, **leg}))
+            del ra, rb, ens, members
+            torch.cuda.empty_cache()
+            continue
 
         def fused():
             return [ens.rank(X, side, masks[side]) for side in (0, 1)]
@@ -112,6 +124,82 @@ def main():
                           "torch_filtered_mrr": round(np.mean([mrr(t[s][1]) for s in (0, 1)]), 6)}))
         del ra, rb, ens, members, f, t
         torch.cuda.empty_cache()
+
+
+def interleaved_medians(fns, reps, flush):
+    """Median CUDA-event time of each of fns (name -> callable), the calls alternating within every repetition (L2
+    flushed before each call), after one warm-up call of each: host or clock drift hits all of them alike."""
+    for fn in fns.values():
+        fn()
+    torch.cuda.synchronize()
+    times = {name: [] for name in fns}
+    for _ in range(reps):
+        for name, fn in fns.items():
+            flush.zero_()
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            fn()
+            b.record()
+            torch.cuda.synchronize()
+            times[name].append(a.elapsed_time(b))
+    return {name: float(np.median(t)) for name, t in times.items()}
+
+
+def prediction_leg(args, name, n, V, R, members, X, Xl, masks, ra, rb, ens, flush):
+    """The --topk / --relations legs: fused ensemble, the two members' single fused calls, and torch."""
+    k = args.topk
+    rel_masks = None
+    if args.relations and k is None:
+        rng = np.random.RandomState(1)
+        known = [sorted({int(t[1])} | set(rng.randint(0, R, rng.randint(0, 3)).tolist())) for t in X.cpu().numpy()]
+        rel_masks = torch.as_tensor(BilinearDiag.known_bit_mask(known, R), device=X.device)
+
+    def energies(codes, rel, sl, side):
+        if args.relations:
+            return (codes[Xl[sl, 0]] * codes[Xl[sl, 2]]) @ rel.T
+        q = rel[Xl[sl, 1]] * (codes[Xl[sl, 2]] if side == 0 else codes[Xl[sl, 0]])
+        return q @ codes.T
+
+    sides = (0,) if args.relations else (0, 1)
+    if args.relations and k is None:
+        fused = lambda: ens.rank_relations(X, rel_masks)
+        singles = lambda: (ra.rank_relations(X, rel_masks), rb.rank_relations(X, rel_masks))
+
+        def torch_path():
+            out = []
+            for c0 in range(0, n, args.chunk):
+                sl = slice(c0, min(n, c0 + args.chunk))
+                comb = None
+                for codes, rel in members:
+                    s = torch.sigmoid(energies(codes, rel, sl, 0)).double()
+                    comb = W * s if comb is None else comb + (1.0 - W) * s
+                out.append((comb >= comb.gather(1, Xl[sl, 1:2])).sum(1))
+            return torch.cat(out)
+    else:
+        if args.relations:
+            fused = lambda: ens.top_k_relations(X, k)
+            singles = lambda: (ra.top_k_relations(X, k), rb.top_k_relations(X, k))
+        else:
+            fused = lambda: [ens.top_k(X, side, k) for side in sides]
+            singles = lambda: [(ra.top_k(X, side, k), rb.top_k(X, side, k)) for side in sides]
+
+        def torch_path():
+            out = []
+            for side in sides:
+                for c0 in range(0, n, args.chunk):
+                    sl = slice(c0, min(n, c0 + args.chunk))
+                    u = None
+                    for codes, rel in members:
+                        s = torch.sigmoid(-energies(codes, rel, sl, side).double())
+                        u = W * s if u is None else u + (1.0 - W) * s
+                    out.append(torch.topk(u, k, dim=1, largest=False, sorted=True))
+            return out
+    times = interleaved_medians({"fused_ensemble_ms": fused, "two_single_calls_ms": singles, "torch_ms": torch_path},
+                                args.reps, flush)
+    times["fused_over_singles"] = times["fused_ensemble_ms"] / times["two_single_calls_ms"]
+    leg = "relation " if args.relations else "entity "
+    leg += "top-%d" % k if k is not None else "ranks"
+    return {"leg": leg, **{key: round(v, 3) for key, v in times.items()}}
 
 
 if __name__ == "__main__":
