@@ -40,6 +40,12 @@ extern "C" {
 #define RGCN_NORM_CANONICAL 0 /* 1 / (#messages of that direction into the destination)        */
 #define RGCN_NORM_EXPLICIT 1  /* caller supplies norm_f[E], norm_b[E] (e.g. tf_unsorted_compat) */
 #define RGCN_NORM_NONE 2      /* all ones ('none' branch, :70-82)                               */
+/* 1 / (#messages with the same destination AND weight id): the R-GCN paper's per-relation c_{i,r} = |N_i^r|,
+ * the 'local' branch of forward_/backward_incidence_matrix (:94-107, :134-147; softmax grouped by (relation,
+ * receiver)).  Forward message k gets 1 / #{k' : o_k' = o_k, r_k' = r_k}, backward message E+k gets
+ * 1 / #{k' : s_k' = s_k, r_k' = r_k}; duplicate triples count as often as they occur.  Triple constructors only
+ * (the message-list constructors take explicit norms). */
+#define RGCN_NORM_RELATION 3
 
 typedef struct rgcn_graph rgcn_graph_t; /* opaque */
 

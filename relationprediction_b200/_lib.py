@@ -42,7 +42,7 @@ EXPORTED_SYMBOLS = [
 
 RGCN_DECODER_DISTMULT, RGCN_DECODER_COMPLEX = 0, 1
 
-RGCN_NORM_CANONICAL, RGCN_NORM_EXPLICIT, RGCN_NORM_NONE = 0, 1, 2
+RGCN_NORM_CANONICAL, RGCN_NORM_EXPLICIT, RGCN_NORM_NONE, RGCN_NORM_RELATION = 0, 1, 2, 3
 
 (X_DST_ROWPTR, X_DST_SRC, X_DST_RELW, X_DST_NORM, X_DST_MID, X_SRC_ROWPTR, X_SRC_DST, X_SRC_RELW,
  X_SRC_NORM, X_SRC_MID, X_REL_PTR, X_REL_DST, X_REL_SRC, X_REL_NORM, X_REL_MID, X_MSG_NORM,

@@ -379,7 +379,7 @@ extern "C" int rgcn_graph_create(const int32_t* triples_host, int64_t E, int32_t
     rgcn_set_error("rgcn_graph_create: RGCN_NORM_EXPLICIT needs norm_f_host and norm_b_host");
     return RGCN_ERR_INVALID;
   }
-  if (norm_mode < 0 || norm_mode > 2) {
+  if (norm_mode < 0 || norm_mode > RGCN_NORM_RELATION) {
     rgcn_set_error("rgcn_graph_create: unknown norm_mode");
     return RGCN_ERR_INVALID;
   }
@@ -451,6 +451,22 @@ extern "C" int rgcn_graph_create(const int32_t* triples_host, int64_t E, int32_t
       norm[k] = 1.0f / (float)cf[dst[k]];
       norm[E + k] = 1.0f / (float)cb[dst[E + k]];
     }
+  } else if (norm_mode == RGCN_NORM_RELATION) {
+    // 1 / (#messages in the message's (dst, weight id) group) -- the 'local' branch
+    // (graph_representations.py:94-107, :134-147).  The groups are the runs of the by_dst order.
+    std::vector<int32_t> perm, ptr;
+    try {
+      sort_two_keys(dst.data(), std::max(V, 1), relw.data(), 2 * R, M, perm, ptr);
+    } catch (const std::bad_alloc&) {
+      return RGCN_ERR_NOMEM;
+    }
+    for (int64_t i = 0; i < M;) {
+      const int32_t d = dst[perm[i]], w = relw[perm[i]];
+      int64_t j = i + 1;
+      while (j < M && dst[perm[j]] == d && relw[perm[j]] == w) ++j;
+      const float v = 1.0f / (float)(j - i);
+      for (; i < j; ++i) norm[perm[i]] = v;
+    }
   } else if (norm_mode == RGCN_NORM_EXPLICIT) {
     for (int64_t k = 0; k < E; ++k) {
       norm[k] = norm_f_host[k];
@@ -512,7 +528,7 @@ extern "C" int rgcn_graph_create_device(const int32_t* triples_dev, int64_t E, i
     return RGCN_ERR_NODEVICE;
   }
   if (E < 0 || V < 0 || R <= 0 || (E > 0 && !triples_dev) || 2 * E > 0x7fffffffLL || norm_mode < 0 ||
-      norm_mode > 2 || (norm_mode == RGCN_NORM_EXPLICIT && E > 0 && (!norm_f_dev || !norm_b_dev))) {
+      norm_mode > RGCN_NORM_RELATION || (norm_mode == RGCN_NORM_EXPLICIT && E > 0 && (!norm_f_dev || !norm_b_dev))) {
     rgcn_set_error("rgcn_graph_create_device: bad arguments");
     return RGCN_ERR_INVALID;
   }

@@ -102,7 +102,7 @@ int rgcn_build_on_device(rgcn_graph* g, const int32_t* d_dst, const int32_t* d_s
                          const int32_t* d_relw, const float* d_norm, cudaStream_t st);
 int rgcn_build_on_device_checked(rgcn_graph* g, const int32_t* d_dst, const int32_t* d_src,
                                  const int32_t* d_relw, const float* d_norm, const int* d_bad,
-                                 cudaStream_t st);
+                                 cudaStream_t st, float* d_run_norm);
 int rgcn_build_from_triples_device(rgcn_graph* g, const int32_t* d_triples, int64_t E, int32_t V,
                                    int32_t R, int norm_mode, const float* d_norm_f,
                                    const float* d_norm_b, cudaStream_t st);

@@ -1,7 +1,8 @@
 // graph_device.cu -- graph preparation ON THE GPU (the default when a device is given).
 //
 // Same result, bit for bit, as the host builder in graph.cu (tests compare the exported arrays):
-//   messages -> per-direction 1/in-degree norm -> four stable sorts (CUB LSD radix sort on a packed
+//   messages -> per-direction 1/in-degree norm (or, RGCN_NORM_RELATION, 1/run length taken from the first
+//   destination-keyed sort) -> four stable sorts (CUB LSD radix sort on a packed
 //   64-bit (major, minor) key with the message id as payload; ties keep message-id order exactly
 //   like the host counting sorts) -> CSR pointers (histogram + exclusive scan) -> warp work lists.
 // The reference does this implicitly inside TF (extras/graph_representations.py:21-27, :84-93,
@@ -180,6 +181,38 @@ __global__ void k_count_runs(const uint64_t* __restrict__ keys, int64_t M,
   if ((threadIdx.x & 31) == 0 && local) atomicAdd(out, local);
 }
 
+// RGCN_NORM_RELATION: a (dst, weight id) group is one run of equal keys in the sorted keys of a destination-keyed view
+// (by_dst: dst * n_relw + relw; by_rel: ((dst / st_rows) * n_relw + relw) * V + dst).  Each sorted position finds
+// the ends of its run by a galloping search from itself (a run of L messages costs O(log L) probes per message,
+// neighbouring threads probe the same lines) and scatters 1/L to its message through the sort permutation.  No
+// temporaries; the result is an integer count converted exactly like the host builder's.
+__device__ __forceinline__ int64_t run_edge(const uint64_t* __restrict__ keys, int64_t M, int64_t i, int64_t dir) {
+  const uint64_t k = keys[i];
+  int64_t in = i, out = i, step = 1;  // keys[in] == k; `out` becomes the first probe past the run (or -1 / M)
+  for (;;) {
+    out = in + dir * step;
+    if (out < 0 || out >= M || keys[out] != k) break;
+    in = out;
+    step <<= 1;
+  }
+  if (out < 0) out = -1;
+  if (out > M) out = M;
+  while (out - in > 1 || in - out > 1) {
+    const int64_t mid = in + (out - in) / 2;
+    if (keys[mid] == k) in = mid; else out = mid;
+  }
+  return in;  // last position of the run in direction `dir`
+}
+
+__global__ void k_norm_relation(const uint64_t* __restrict__ keys, const int32_t* __restrict__ perm, int64_t M,
+                                float* __restrict__ norm) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < M;
+       i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t len = run_edge(keys, M, i, 1) - run_edge(keys, M, i, -1) + 1;
+    norm[perm[i]] = 1.0f / (float)len;
+  }
+}
+
 int grid_for(int64_t n) {
   int64_t b = (n + 255) / 256;
   if (b > 132 * 8) b = 132 * 8;
@@ -274,10 +307,12 @@ struct ViewTmp {
 // in a phase-local Scratch and return to the stream-ordered pool before the next view is built, so a
 // 200 M-message graph peaks at one view's temporaries instead of four.
 
+// run_norm (RGCN_NORM_RELATION, destination-keyed view built first): the message-order `norm` buffer, filled here from
+// the sorted keys before this view -- and every later one -- gathers it
 int csr_phase_a(rgcn_graph* g, CsrSide& side, ViewTmp& t, const int32_t* row, int32_t n_rows,
                 const int32_t* nbr, const int32_t* relw, const float* norm, int64_t M,
                 bool count_runs, unsigned long long* d_runs, int32_t* h_totals /* pinned [2] */,
-                cudaStream_t st, int64_t& bytes) {
+                float* run_norm, cudaStream_t st, int64_t& bytes) {
   Scratch sc(st);
   int rc;
   if ((rc = dalloc(&side.d_rowptr, (int64_t)n_rows + 1, st, &bytes))) return rc;
@@ -290,6 +325,10 @@ int csr_phase_a(rgcn_graph* g, CsrSide& side, ViewTmp& t, const int32_t* row, in
   if ((rc = dalloc(&side.d_relw, M, st, &bytes))) return rc;
   if ((rc = dalloc(&side.d_norm, M, st, &bytes))) return rc;
   if (M > 0) {
+    if (run_norm) {
+      k_norm_relation<<<grid_for(M), 256, 0, st>>>(keys, perm, M, run_norm);
+      ++g_rgcn_launches;
+    }
     k_gather3<<<grid_for(M), 256, 0, st>>>(perm, M, nbr, relw, norm, side.d_nbr, side.d_relw,
                                            side.d_norm);
     ++g_rgcn_launches;
@@ -340,7 +379,8 @@ int csr_phase_b(rgcn_graph* g, CsrSide& side, ViewTmp& t, int32_t n_rows, const 
 
 int rel_phase_a(rgcn_graph* g, RelSide& side, ViewTmp& t, const int32_t* row, int32_t n_rows,
                 const int32_t* nbr, const int32_t* relw, const float* norm, int64_t M,
-                int32_t* h_total /* pinned [1] */, cudaStream_t st, int64_t& bytes) {
+                int32_t* h_total /* pinned [1] */, float* run_norm /* as in csr_phase_a */, cudaStream_t st,
+                int64_t& bytes) {
   Scratch sc(st);
   int rc;
   const int st_rows = view_supertile_rows(g, n_rows, M);
@@ -358,6 +398,10 @@ int rel_phase_a(rgcn_graph* g, RelSide& side, ViewTmp& t, const int32_t* row, in
   if ((rc = dalloc(&side.d_nbr, M, st, &bytes))) return rc;
   if ((rc = dalloc(&side.d_norm, M, st, &bytes))) return rc;
   if (M > 0) {
+    if (run_norm) {
+      k_norm_relation<<<grid_for(M), 256, 0, st>>>(keys, perm, M, run_norm);
+      ++g_rgcn_launches;
+    }
     k_gather3<<<grid_for(M), 256, 0, st>>>(perm, M, row, nbr, norm, side.d_row, side.d_nbr,
                                            side.d_norm);
     ++g_rgcn_launches;
@@ -415,9 +459,12 @@ void tune_mempool_once(int device) {
 
 // Builds every device-side structure of `g` from DEVICE message arrays (length M).
 // d_bad (optional): device flag set by the caller's validation kernel; checked at the single sync.
+// d_run_norm (optional, RGCN_NORM_RELATION): the buffer d_norm points to, not yet written; the first view built (by_dst,
+// or by_rel when the CSR views are off -- both destination-keyed) fills it with 1 / (length of the (dst, weight id)
+// run) before anything reads it.
 int rgcn_build_on_device_checked(rgcn_graph* g, const int32_t* d_dst, const int32_t* d_src,
                                  const int32_t* d_relw, const float* d_norm, const int* d_bad,
-                                 cudaStream_t st) {
+                                 cudaStream_t st, float* d_run_norm) {
   static thread_local HostSlots hs;
   if (!hs.p || !hs.runs) {
     rgcn_set_error("cudaHostAlloc failed in graph prep");
@@ -432,20 +479,26 @@ int rgcn_build_on_device_checked(rgcn_graph* g, const int32_t* d_dst, const int3
   DCK(cudaMemsetAsync(d_runs, 0, sizeof(unsigned long long), st));
   if (g->keep_mid) {
     if ((rc = dalloc(&g->d_msg_norm, M, st, &bytes))) return rc;
-    DCK(cudaMemcpyAsync(g->d_msg_norm, d_norm, (size_t)M * 4, cudaMemcpyDeviceToDevice, st));
   }
   ViewTmp t0(st), t1(st), t2(st), t3(st);
   for (int i = 0; i < 8; ++i) hs.p[i] = 0;
   *hs.runs = 0;
   rc = RGCN_OK;
   if (g->has_csr) {
-    rc = csr_phase_a(g, g->by_dst, t0, d_dst, g->V_dst, d_src, d_relw, d_norm, M, true, d_runs, hs.p + 0, st, bytes);
-    if (!rc) rc = csr_phase_a(g, g->by_src, t1, d_src, g->V_src, d_dst, d_relw, d_norm, M, false, nullptr, hs.p + 2, st, bytes);
+    rc = csr_phase_a(g, g->by_dst, t0, d_dst, g->V_dst, d_src, d_relw, d_norm, M, true, d_runs, hs.p + 0, d_run_norm,
+                     st, bytes);
+    d_run_norm = nullptr;
+    if (!rc) rc = csr_phase_a(g, g->by_src, t1, d_src, g->V_src, d_dst, d_relw, d_norm, M, false, nullptr, hs.p + 2,
+                              nullptr, st, bytes);
   }
   if (!rc && g->has_rel) {
-    rc = rel_phase_a(g, g->by_rel, t2, d_dst, g->V_dst, d_src, d_relw, d_norm, M, hs.p + 4, st, bytes);
-    if (!rc) rc = rel_phase_a(g, g->by_rel_src, t3, d_src, g->V_src, d_dst, d_relw, d_norm, M, hs.p + 5, st, bytes);
+    rc = rel_phase_a(g, g->by_rel, t2, d_dst, g->V_dst, d_src, d_relw, d_norm, M, hs.p + 4, d_run_norm, st, bytes);
+    if (!rc) rc = rel_phase_a(g, g->by_rel_src, t3, d_src, g->V_src, d_dst, d_relw, d_norm, M, hs.p + 5, nullptr, st,
+                              bytes);
   }
+  if (!rc && g->keep_mid && M > 0)
+    rc = rgcn_check_cuda(cudaMemcpyAsync(g->d_msg_norm, d_norm, (size_t)M * 4, cudaMemcpyDeviceToDevice, st),
+                         "copy msg norm");
   if (!rc) rc = rgcn_check_cuda(cudaMemcpyAsync(hs.runs, d_runs, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st), "copy runs");
   if (!rc && d_bad) rc = rgcn_check_cuda(cudaMemcpyAsync(hs.p + 6, d_bad, 4, cudaMemcpyDeviceToHost, st), "copy flag");
   if (!rc) rc = rgcn_check_cuda(cudaStreamSynchronize(st), "sync(graph prep)");
@@ -477,7 +530,7 @@ int rgcn_build_on_device_checked(rgcn_graph* g, const int32_t* d_dst, const int3
 
 int rgcn_build_on_device(rgcn_graph* g, const int32_t* d_dst, const int32_t* d_src,
                          const int32_t* d_relw, const float* d_norm, cudaStream_t st) {
-  return rgcn_build_on_device_checked(g, d_dst, d_src, d_relw, d_norm, nullptr, st);
+  return rgcn_build_on_device_checked(g, d_dst, d_src, d_relw, d_norm, nullptr, st, nullptr);
 }
 
 // triples (DEVICE, int32 [E,3]) -> messages + norm -> rgcn_build_on_device
@@ -505,15 +558,18 @@ int rgcn_build_from_triples_device(rgcn_graph* g, const int32_t* d_triples, int6
     ++g_rgcn_launches;
     if (norm_mode == RGCN_NORM_CANONICAL) {
       k_norm_canonical<<<grid_for(E), 256, 0, st>>>(dst, E, cnt_f, cnt_b, norm);
+      ++g_rgcn_launches;
     } else if (norm_mode == RGCN_NORM_EXPLICIT) {
       DCK(cudaMemcpyAsync(norm, d_norm_f, (size_t)E * 4, cudaMemcpyDeviceToDevice, st));
       DCK(cudaMemcpyAsync(norm + E, d_norm_b, (size_t)E * 4, cudaMemcpyDeviceToDevice, st));
-    } else {
+      ++g_rgcn_launches;
+    } else if (norm_mode == RGCN_NORM_NONE) {
       k_fill<<<grid_for(M), 256, 0, st>>>(norm, M, 1.0f);
-    }
-    ++g_rgcn_launches;
+      ++g_rgcn_launches;
+    }  // RGCN_NORM_RELATION: written by the first view build (k_norm_relation)
   }
-  return rgcn_build_on_device_checked(g, dst, src, relw, norm, bad, st);
+  return rgcn_build_on_device_checked(g, dst, src, relw, norm, bad, st,
+                                      norm_mode == RGCN_NORM_RELATION ? norm : nullptr);
 }
 
 int rgcn_check_messages_device(const int32_t* d_dst, const int32_t* d_src, const int32_t* d_relw,

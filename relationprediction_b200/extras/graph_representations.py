@@ -56,7 +56,7 @@ class MessageGraph(object):
 
 class Representation(Model):
     normalization = "global"
-    norm_mode = "canonical"   # or "tf_unsorted_compat" (quirk Q1, see DESIGN.md)
+    norm_mode = "canonical"   # or "tf_unsorted_compat" (quirk Q1, see DESIGN.md), or "relation" (the 'local' branch)
 
     def __init__(self, triples, settings, bipartite=False):
         self.settings = settings
@@ -99,6 +99,9 @@ class Representation(Model):
             if self.norm_mode == "tf_unsorted_compat":
                 kw = dict(norm_mode="explicit", norm_f=_tf_compat(edges[:, 2], self.entity_count),
                           norm_b=_tf_compat(edges[:, 0], self.entity_count))
+            elif self.norm_mode == "relation":
+                # per-relation c_{i,r}: the 'local' branch of the incidence matrices (:94-107, :134-147)
+                kw = dict(norm_mode="relation")
             g = MessageGraph(edges, self.entity_count, self.relation_count, self.get_device(), **kw)
             self._graphs[key] = g
         return g

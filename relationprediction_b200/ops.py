@@ -13,7 +13,7 @@ import torch
 from . import _lib
 
 _NORM = {"canonical": _lib.RGCN_NORM_CANONICAL, "explicit": _lib.RGCN_NORM_EXPLICIT,
-         "none": _lib.RGCN_NORM_NONE}
+         "none": _lib.RGCN_NORM_NONE, "relation": _lib.RGCN_NORM_RELATION}
 
 
 def _ptr(t):
@@ -42,6 +42,8 @@ class Graph:
 
     Replaces Representation/MessageGraph (extras/graph_representations.py): triples [E,3] (s,r,o)
     -> 2E messages, per-direction 1/in-degree normalisation, three sorted views + warp work lists.
+    norm_mode: "canonical" (1 / #messages of the direction into the destination), "relation" (1 / #messages with
+    the same destination and weight id: the paper's c_{i,r}), "explicit" (norm_f / norm_b given) or "none".
     `device=None` builds the host structure only (used by the CPU tests of the index work).
     """
 

@@ -5,7 +5,8 @@ whose destination it owns.  Sources are addressed in an extended local row space
 [local rows | halo rows]; the halo rows (unique remote sources) arrive once per layer forward -- pushed
 by their owners into this rank's peer-mapped halo buffer (PeerHalo), or by ONE all-to-all-v (NCCL
 transport) -- and their gradients return the same way per layer backward (then a local row add).  Weights are replicated; their gradients are summed with one all-reduce.  The
-per-message normalisation uses GLOBAL degrees, so sharded results equal the single-GPU ones.
+per-message normalisation uses GLOBAL degrees (per destination, or per (destination, weight id) in relation mode), so
+sharded results equal the single-GPU ones.
 
 The reference has no distributed code at all (single tf.Session, train.py:278); this module is the
 multi-GPU design for the hot path only.
@@ -40,6 +41,10 @@ def global_messages(triples, n_nodes, n_relations, norm_mode="canonical", norm_f
         cf = np.bincount(o, minlength=n_nodes).astype(np.float32)
         cb = np.bincount(s, minlength=n_nodes).astype(np.float32)
         norm = np.concatenate([np.float32(1) / cf[o], np.float32(1) / cb[s]]).astype(np.float32)
+    elif norm_mode == "relation":      # 1 / #messages with the same (dst, weight id), over the whole graph
+        _, inv, cnt = np.unique(dst.astype(np.int64) * (2 * n_relations) + relw, return_inverse=True,
+                                return_counts=True)
+        norm = (np.float32(1) / cnt[inv.reshape(-1)].astype(np.float32)).astype(np.float32)
     elif norm_mode == "explicit":
         norm = np.concatenate([norm_f, norm_b]).astype(np.float32)
     else:
@@ -108,6 +113,16 @@ class ShardPlanDevice(object):
             cb = torch.bincount(s.long(), minlength=n_nodes).to(torch.float32)
             one = torch.ones((), dtype=torch.float32, device=dev)
             inv_f, inv_b = one / cf, one / cb      # fp32 division, as in ShardPlan / rgcn_graph_create
+        elif norm_mode == "relation":
+            # global per-(dst, weight id) counts, one direction at a time: key = dst * R + r (the weight ids of a
+            # direction differ by the constant R)
+            one = torch.ones((), dtype=torch.float32, device=dev)
+
+            def relation_norm(dn):
+                _, inv, cnt = torch.unique(dn.long() * n_relations + r.long(), return_inverse=True,
+                                           return_counts=True)
+                return one / cnt.to(torch.float32)[inv]
+            rel_f = relation_norm(o)
         inner = torch.as_tensor(self.bounds[1:], dtype=torch.int32, device=dev)
 
         def owner(nodes):
@@ -125,6 +140,8 @@ class ShardPlanDevice(object):
             parts["relw"].append((r[mine] + direction * n_relations).to(torch.int32))
             if norm_mode == "canonical":
                 parts["norm"].append((inv_f if direction == 0 else inv_b)[dn[mine].long()])
+            elif norm_mode == "relation":
+                parts["norm"].append((rel_f if direction == 0 else relation_norm(s))[mine])
             elif norm_mode == "explicit":
                 parts["norm"].append((norm_f if direction == 0 else norm_b)[mine].to(torch.float32))
             else:
