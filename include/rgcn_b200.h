@@ -721,6 +721,30 @@ int rgcn_one_to_n_labels(const int64_t* keys, const int64_t* offsets, const int3
                          int32_t V, int32_t R, const int32_t* queries, int64_t n, uint32_t* bits, void* workspace,
                          int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) for the DistMult or ComplEx decoder
+ * (decoder = RGCN_DECODER_*).  X : int32 [N, 3] device in the negative sampler's layout: N = n (K + 1), rows 0..n-1
+ * the positives, row i + n j (j = 1..K) the j-th corruption of positive i.  With s_i the positive's energy and s_ij
+ * its corruptions' (the energies of distmult_forward / rgcn_complex_forward),
+ *   p_ij        = exp(alpha s_ij) / sum_j' exp(alpha s_ij')               (the group maximum is subtracted first)
+ *   loss_out[0] = 1 / (2n) sum_i [ softplus(-s_i) + sum_j p_ij softplus(s_ij) ],  softplus(x) = max(x,0) + log1p(exp(-|x|))
+ *   loss_out[1] = the L2 term of distmult_forward over all N triples (un-scaled)
+ * energies [N] and coef [N] device: coef is d loss_out[0] / d energy with p held constant, -sigmoid(-s_i) / (2n) for a
+ * positive and p_ij sigmoid(s_ij) / (2n) for a corruption.  The gradient of g_loss loss_out[0] + g_reg loss_out[1] is
+ * the scorer's backward (distmult_backward_slices / rgcn_complex_backward) with Y = NULL and g_energy = g_loss coef;
+ * its rel_slice_sumsq is then the relation table's IndexedSlices norm under these per-triple weights.  Both loss parts
+ * are summed in a fixed order, so they are bitwise repeatable.  K = 1 gives p = 1 and the NegativeSampling loss;
+ * alpha = 0 gives p = 1 / K.  Y is not read.
+ * workspace : rgcn_self_adversarial_workspace_bytes(N, K).
+ * Errors, before any device work: RGCN_ERR_INVALID (unknown decoder kind, null pointers, V or Vrel <= 0, d % 4 != 0,
+ * K < 1, N % (K + 1) != 0, alpha negative or not finite), RGCN_ERR_WORKSPACE, RGCN_ERR_NODEVICE.  The
+ * *_workspace_bytes function returns RGCN_ERR_INVALID (-1) on bad arguments.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_self_adversarial_workspace_bytes(int64_t N, int32_t K);
+int rgcn_self_adversarial_forward(int32_t decoder, const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                                  int32_t d, const int32_t* X, int64_t N, int32_t K, float alpha, float* energies,
+                                  float* coef, float* loss_out, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

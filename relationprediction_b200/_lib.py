@@ -38,6 +38,7 @@ EXPORTED_SYMBOLS = [
     "rgcn_one_to_n_workspace_bytes", "distmult_one_to_n", "rgcn_complex_one_to_n",
     "rgcn_one_to_n_labels_workspace_bytes", "rgcn_one_to_n_labels",
     "rgcn_one_to_n_finish_workspace_bytes", "rgcn_one_to_n_finish",
+    "rgcn_self_adversarial_workspace_bytes", "rgcn_self_adversarial_forward",
 ]
 
 RGCN_DECODER_DISTMULT, RGCN_DECODER_COMPLEX = 0, 1
@@ -254,6 +255,11 @@ def _declare(lib):
     lib.rgcn_one_to_n_labels_workspace_bytes.argtypes = [c_int64]
     lib.rgcn_one_to_n_labels.restype = c_int
     lib.rgcn_one_to_n_labels.argtypes = [vp, vp, vp, c_int64, c_int32, c_int32, vp, c_int64, vp, vp, c_int64, vp]
+    lib.rgcn_self_adversarial_workspace_bytes.restype = c_int64
+    lib.rgcn_self_adversarial_workspace_bytes.argtypes = [c_int64, c_int32]
+    lib.rgcn_self_adversarial_forward.restype = c_int
+    lib.rgcn_self_adversarial_forward.argtypes = [c_int32, vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int32,
+                                                  c_float, vp, vp, vp, vp, c_int64, vp]
 
 
 def load():

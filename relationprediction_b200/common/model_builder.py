@@ -163,10 +163,11 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
 
 
 def build_decoder(encoder, decoder_settings):
-    if decoder_settings['Name'] not in ("bilinear-diag", "complex") and \
-            parse_training_objective(decoder_settings)[0] == '1-N':
-        raise ValueError("TrainingObjective=1-N needs the bilinear-diag or complex decoder, not %r"
-                         % (decoder_settings['Name'],))
+    if decoder_settings['Name'] not in ("bilinear-diag", "complex"):
+        objective = parse_training_objective(decoder_settings)[0]
+        if objective != 'NegativeSampling':
+            raise ValueError("TrainingObjective=%s needs the bilinear-diag or complex decoder, not %r"
+                             % (objective, decoder_settings['Name']))
     if decoder_settings['Name'] == "bilinear-diag":
         return BilinearDiag(encoder, decoder_settings)
     if decoder_settings['Name'] == "complex":

@@ -2184,3 +2184,55 @@ extern "C" int rgcn_one_to_n_labels(const int64_t* keys, const int64_t* offsets,
   }
   return rc;
 }
+
+// ------------------------------------------------------------------------------------------------
+// Self-adversarial negative sampling (DistMult and ComplEx): the per-positive softmax weights over its corruptions
+// and the weighted loss in one kernel (self_adversarial.cu); the backward is the scorer's own with g_energy = coef.
+// Workspace layout: [loss parts n | norm parts n], n = N / (K + 1).
+// ------------------------------------------------------------------------------------------------
+extern "C" int64_t rgcn_self_adversarial_workspace_bytes(int64_t N, int32_t K) {
+  if (N < 0 || K < 1 || N % ((int64_t)K + 1) != 0) {
+    rgcn_set_error("rgcn_self_adversarial_workspace_bytes: bad arguments (need N >= 0, K >= 1, N % (K + 1) == 0)");
+    return RGCN_ERR_INVALID;
+  }
+  return align_up(2 * (N / ((int64_t)K + 1)) * 4) + 256;
+}
+
+extern "C" int rgcn_self_adversarial_forward(int32_t decoder, const float* codes, const float* rel, int32_t V,
+                                             int32_t Vrel, int32_t d, const int32_t* X, int64_t N, int32_t K,
+                                             float alpha, float* energies, float* coef, float* loss_out,
+                                             void* workspace, int64_t workspace_bytes, void* stream) {
+  const std::string who = "rgcn_self_adversarial_forward";
+  if (decoder != RGCN_DECODER_DISTMULT && decoder != RGCN_DECODER_COMPLEX) {
+    rgcn_set_error(who + ": unknown decoder kind (RGCN_DECODER_DISTMULT or RGCN_DECODER_COMPLEX)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!codes || !rel || !loss_out || !workspace || (N > 0 && (!X || !energies || !coef))) {
+    rgcn_set_error(who + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 || N < 0) {
+    rgcn_set_error(who + ": bad sizes (need V > 0, Vrel > 0, d > 0, d % 4 == 0, N >= 0)");
+    return RGCN_ERR_INVALID;
+  }
+  if (K < 1 || N % ((int64_t)K + 1) != 0) {
+    rgcn_set_error(who + ": N = " + std::to_string(N) + " triples are not n positives with K = " + std::to_string(K) +
+                   " corruptions each (need K >= 1 and N % (K + 1) == 0)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!(alpha >= 0.0f && alpha < INFINITY)) {   // also refuses NaN
+    rgcn_set_error(who + ": the adversarial temperature must be finite and >= 0");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_self_adversarial_workspace_bytes(N, K)) {
+    rgcn_set_error(who + ": workspace too small (rgcn_self_adversarial_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  int rc = onen_device_checks(who.c_str());
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver ws(workspace, workspace_bytes);
+  float* parts = ws.take<float>(2 * (N / ((int64_t)K + 1)));
+  return launch_self_adversarial_forward(decoder == RGCN_DECODER_COMPLEX, codes, rel, d, X, N, K, alpha, energies,
+                                         coef, loss_out, parts, st);
+}

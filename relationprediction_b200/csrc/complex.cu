@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 
 #include "kernels.cuh"
+#include "triple_rows.cuh"
 
 #define FULL 0xffffffffu
 
@@ -19,38 +20,6 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
   return v;
 }
-
-// W consecutive floats (W = 4: 16-byte aligned, W = 2: 8-byte aligned)
-template <int W>
-struct Vec;
-template <>
-struct Vec<4> {
-  __device__ __forceinline__ static void load(const float* p, float (&v)[4]) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(p));
-    v[0] = t.x, v[1] = t.y, v[2] = t.z, v[3] = t.w;
-  }
-  __device__ __forceinline__ static void store(float* p, const float (&v)[4]) {
-    *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
-  }
-  __device__ __forceinline__ static void red(float* p, const float (&v)[4]) {
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]),
-                 "f"(v[3])
-                 : "memory");
-  }
-};
-template <>
-struct Vec<2> {
-  __device__ __forceinline__ static void load(const float* p, float (&v)[2]) {
-    const float2 t = __ldg(reinterpret_cast<const float2*>(p));
-    v[0] = t.x, v[1] = t.y;
-  }
-  __device__ __forceinline__ static void store(float* p, const float (&v)[2]) {
-    *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]);
-  }
-  __device__ __forceinline__ static void red(float* p, const float (&v)[2]) {
-    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(v[0]), "f"(v[1]) : "memory");
-  }
-};
 
 // loss_acc[0] += sum of per-triple cross-entropy terms, loss_acc[1] += sum of squares of the gathered rows
 template <int W>
@@ -63,28 +32,10 @@ __global__ void __launch_bounds__(256)
   const int64_t wid0 = (int64_t)blockIdx.x * 8 + warp;
   const int64_t wstride = (int64_t)gridDim.x * 8;
   double lsum = 0.0, qsum = 0.0;
-  const int h = d >> 1;
   for (int64_t n = wid0; n < N; n += wstride) {
     const int s = __ldg(X + 3 * n), r = __ldg(X + 3 * n + 1), o = __ldg(X + 3 * n + 2);
-    const float* e1 = codes + (size_t)s * d;
-    const float* rr = rel + (size_t)r * d;
-    const float* e2 = codes + (size_t)o * d;
     float e = 0.f, q = 0.f;
-    for (int k = lane * W; k < h; k += 32 * W) {
-      float ar[W], ai[W], br[W], bi[W], cr[W], ci[W];
-      Vec<W>::load(e1 + k, ar), Vec<W>::load(e1 + h + k, ai);
-      Vec<W>::load(rr + k, br), Vec<W>::load(rr + h + k, bi);
-      Vec<W>::load(e2 + k, cr), Vec<W>::load(e2 + h + k, ci);
-#pragma unroll
-      for (int j = 0; j < W; ++j) {
-        // complex.py:38-41: e1r*rr*e2r + e1i*rr*e2i + e1r*ri*e2i - e1i*ri*e2r
-        e = fmaf(br[j], fmaf(ar[j], cr[j], ai[j] * ci[j]), e);
-        e = fmaf(bi[j], fmaf(ar[j], ci[j], -ai[j] * cr[j]), e);
-        q += ar[j] * ar[j] + ai[j] * ai[j];
-        q += br[j] * br[j] + bi[j] * bi[j];
-        q += cr[j] * cr[j] + ci[j] * ci[j];
-      }
-    }
+    ComplexRows<W>::partial(codes, rel, d, s, r, o, lane, e, q);   // complex.py:38-41
     e = warp_sum(e);
     q = warp_sum(q);
     if (lane == 0) {

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include "kernels.cuh"
+#include "triple_rows.cuh"
 
 #define FULL 0xffffffffu
 
@@ -32,23 +33,10 @@ __global__ void __launch_bounds__(256)
   const int64_t wid0 = (int64_t)blockIdx.x * 8 + warp;
   const int64_t wstride = (int64_t)gridDim.x * 8;
   double lsum = 0.0, qsum = 0.0;
-  const int d4 = d >> 2;
   for (int64_t n = wid0; n < N; n += wstride) {
     const int s = __ldg(X + 3 * n), r = __ldg(X + 3 * n + 1), o = __ldg(X + 3 * n + 2);
-    const float4* e1 = reinterpret_cast<const float4*>(codes + (size_t)s * d);
-    const float4* rr = reinterpret_cast<const float4*>(rel + (size_t)r * d);
-    const float4* e2 = reinterpret_cast<const float4*>(codes + (size_t)o * d);
     float e = 0.f, q = 0.f;
-    for (int i = lane; i < d4; i += 32) {
-      const float4 a = __ldg(e1 + i), b = __ldg(rr + i), c = __ldg(e2 + i);
-      e = fmaf(a.x * b.x, c.x, e);
-      e = fmaf(a.y * b.y, c.y, e);
-      e = fmaf(a.z * b.z, c.z, e);
-      e = fmaf(a.w * b.w, c.w, e);
-      q += a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
-      q += b.x * b.x + b.y * b.y + b.z * b.z + b.w * b.w;
-      q += c.x * c.x + c.y * c.y + c.z * c.z + c.w * c.w;
-    }
+    DistMultRows::partial(codes, rel, d, s, r, o, lane, e, q);
     e = warp_sum(e);
     q = warp_sum(q);
     if (lane == 0) {

@@ -298,3 +298,10 @@ int launch_complex_rank_prepare(const float* codes, const float* rel, int d, con
 // (gold_sig == nullptr: Q only; the relation column of X is then not read)
 int launch_complex_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n,
                                     float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
+
+// self_adversarial.cu -- self-adversarial objective over N = n (K + 1) triples in the sampler's layout (complex = 0
+// DistMult, 1 ComplEx): energies [N], the energy-gradient coefficients coef [N], loss_out[0] the loss, loss_out[1] the
+// L2 term of distmult_forward; parts: 2n floats of scratch for the per-group loss and norm parts
+int launch_self_adversarial_forward(int complex, const float* codes, const float* rel, int d, const int32_t* X,
+                                    int64_t N, int K, float alpha, float* energies, float* coef, float* loss_out,
+                                    float* parts, cudaStream_t st);

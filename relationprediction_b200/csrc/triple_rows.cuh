@@ -1,0 +1,89 @@
+// triple_rows.cuh -- the row arithmetic of the DistMult and ComplEx triple scorers: one warp owns one triple
+// (s, r, o) and each lane forms its share of the energy and of the squared norms of the three gathered rows.  Shared by
+// the NegativeSampling scorers (distmult.cu / complex.cu) and the self-adversarial scorer (self_adversarial.cu), so
+// both objectives score a triple with the same float operations in the same order.
+#pragma once
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+// W consecutive floats (W = 4: 16-byte aligned, W = 2: 8-byte aligned)
+template <int W>
+struct Vec;
+template <>
+struct Vec<4> {
+  __device__ __forceinline__ static void load(const float* p, float (&v)[4]) {
+    const float4 t = __ldg(reinterpret_cast<const float4*>(p));
+    v[0] = t.x, v[1] = t.y, v[2] = t.z, v[3] = t.w;
+  }
+  __device__ __forceinline__ static void store(float* p, const float (&v)[4]) {
+    *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+  }
+  __device__ __forceinline__ static void red(float* p, const float (&v)[4]) {
+    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]),
+                 "f"(v[3])
+                 : "memory");
+  }
+};
+template <>
+struct Vec<2> {
+  __device__ __forceinline__ static void load(const float* p, float (&v)[2]) {
+    const float2 t = __ldg(reinterpret_cast<const float2*>(p));
+    v[0] = t.x, v[1] = t.y;
+  }
+  __device__ __forceinline__ static void store(float* p, const float (&v)[2]) {
+    *reinterpret_cast<float2*>(p) = make_float2(v[0], v[1]);
+  }
+  __device__ __forceinline__ static void red(float* p, const float (&v)[2]) {
+    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(v[0]), "f"(v[1]) : "memory");
+  }
+};
+
+// DistMult (bilinear_diag.py:14-24): e = sum_k e1 r e2, rows read as float4 (d % 4 == 0)
+struct DistMultRows {
+  // this lane's share of the energy (e) and of the squared norms of the three rows (q), both starting from 0
+  __device__ __forceinline__ static void partial(const float* __restrict__ codes, const float* __restrict__ rel, int d,
+                                                 int s, int r, int o, int lane, float& e, float& q) {
+    const float4* e1 = reinterpret_cast<const float4*>(codes + (size_t)s * d);
+    const float4* rr = reinterpret_cast<const float4*>(rel + (size_t)r * d);
+    const float4* e2 = reinterpret_cast<const float4*>(codes + (size_t)o * d);
+    const int d4 = d >> 2;
+    for (int i = lane; i < d4; i += 32) {
+      const float4 a = __ldg(e1 + i), b = __ldg(rr + i), c = __ldg(e2 + i);
+      e = fmaf(a.x * b.x, c.x, e);
+      e = fmaf(a.y * b.y, c.y, e);
+      e = fmaf(a.z * b.z, c.z, e);
+      e = fmaf(a.w * b.w, c.w, e);
+      q += a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
+      q += b.x * b.x + b.y * b.y + b.z * b.z + b.w * b.w;
+      q += c.x * c.x + c.y * c.y + c.z * c.z + c.w * c.w;
+    }
+  }
+};
+
+// ComplEx (complex.py:38-41): a lane owns the column pairs (k, k + h) of all three rows, h = d / 2; W = 4 when
+// d % 8 == 0, else 2 (the imaginary half is then only 8-byte aligned)
+template <int W>
+struct ComplexRows {
+  __device__ __forceinline__ static void partial(const float* __restrict__ codes, const float* __restrict__ rel, int d,
+                                                 int s, int r, int o, int lane, float& e, float& q) {
+    const float* e1 = codes + (size_t)s * d;
+    const float* rr = rel + (size_t)r * d;
+    const float* e2 = codes + (size_t)o * d;
+    const int h = d >> 1;
+    for (int k = lane * W; k < h; k += 32 * W) {
+      float ar[W], ai[W], br[W], bi[W], cr[W], ci[W];
+      Vec<W>::load(e1 + k, ar), Vec<W>::load(e1 + h + k, ai);
+      Vec<W>::load(rr + k, br), Vec<W>::load(rr + h + k, bi);
+      Vec<W>::load(e2 + k, cr), Vec<W>::load(e2 + h + k, ci);
+#pragma unroll
+      for (int j = 0; j < W; ++j) {
+        // e1r*rr*e2r + e1i*rr*e2i + e1r*ri*e2i - e1i*ri*e2r
+        e = fmaf(br[j], fmaf(ar[j], cr[j], ai[j] * ci[j]), e);
+        e = fmaf(bi[j], fmaf(ar[j], ci[j], -ai[j] * cr[j]), e);
+        q += ar[j] * ar[j] + ai[j] * ai[j];
+        q += br[j] * br[j] + bi[j] * bi[j];
+        q += cr[j] * cr[j] + ci[j] * ci[j];
+      }
+    }
+  }
+};

@@ -5,29 +5,45 @@ import torch
 from ..model import Model, Placeholder
 from .. import ops
 
-TRAINING_OBJECTIVES = ('NegativeSampling', '1-N')
+TRAINING_OBJECTIVES = ('NegativeSampling', '1-N', 'SelfAdversarial')
 
 
 def parse_training_objective(settings):
     """(TrainingObjective, LabelSmoothing) of [General]: 'NegativeSampling' (the default: the reference's objective
-    over NegativeSampleRate corruptions per positive) or '1-N' (every query scored against every entity, ops.one_to_n_loss),
-    and the label smoothing eps in [0, 1) of the 1-N targets (default 0)."""
+    over NegativeSampleRate corruptions per positive), '1-N' (every query scored against every entity, ops.one_to_n_loss)
+    or 'SelfAdversarial' (the NegativeSampling corruptions weighted by a softmax over their own energies,
+    ops.self_adversarial_loss), and the label smoothing eps in [0, 1) of the 1-N targets (default 0).  The temperature
+    of SelfAdversarial is checked here too (parse_adversarial_temperature)."""
     objective = str(settings['TrainingObjective']) if 'TrainingObjective' in settings else 'NegativeSampling'
     if objective not in TRAINING_OBJECTIVES:
         raise ValueError("TrainingObjective must be one of %s, got %r" % (", ".join(TRAINING_OBJECTIVES), objective))
     eps = float(settings['LabelSmoothing']) if 'LabelSmoothing' in settings else 0.0
     if not 0.0 <= eps < 1.0:
         raise ValueError("LabelSmoothing must be in [0, 1), got %r" % (eps,))
+    if objective == 'SelfAdversarial':
+        if 'LabelSmoothing' in settings:
+            raise ValueError("LabelSmoothing applies to TrainingObjective=1-N only, not to SelfAdversarial")
+        parse_adversarial_temperature(settings)
     return objective, eps
 
 
+def parse_adversarial_temperature(settings):
+    """AdversarialTemperature alpha >= 0 of [General] (default 1): the self-adversarial weights of a positive's
+    corruptions are softmax(alpha * energy)."""
+    alpha = float(settings['AdversarialTemperature']) if 'AdversarialTemperature' in settings else 1.0
+    if not 0.0 <= alpha < float('inf'):
+        raise ValueError("AdversarialTemperature must be finite and >= 0, got %r" % (alpha,))
+    return alpha
+
+
 class BilinearDiag(Model):
-    ONE_TO_N = "distmult"   # the decoder kind of ops.one_to_n_loss
+    ONE_TO_N = "distmult"   # the decoder kind of ops.one_to_n_loss and ops.self_adversarial_loss
 
     def __init__(self, next_component, settings):
         self.encoder_cache = {'train': None, 'test': None}
         self._scored = {'train': None, 'test': None}
         self._one_to_n_loss = None
+        self._self_adversarial_loss = None
         self._one_to_n_feed = None   # (fed X, its queries, their label rows)
         self.one_to_n_labels = None
         Model.__init__(self, next_component, settings)
@@ -35,6 +51,9 @@ class BilinearDiag(Model):
     def parse_settings(self):
         self.regularization_parameter = float(self.settings['RegularizationParameter'])
         self.training_objective, self.label_smoothing = parse_training_objective(self.settings)
+        if self.training_objective == 'SelfAdversarial':
+            self.adversarial_temperature = parse_adversarial_temperature(self.settings)
+            self.negative_sample_rate = int(self.settings['NegativeSampleRate'])
 
     def set_one_to_n_labels(self, labels):
         """The ops.OneToNLabels of the training split, which 1-N training reads its targets from."""
@@ -49,6 +68,7 @@ class BilinearDiag(Model):
         self.encoder_cache = {'train': None, 'test': None}
         self._scored = {'train': None, 'test': None}
         self._one_to_n_loss = None
+        self._self_adversarial_loss = None
 
     def local_get_train_input_variables(self):
         return [self.X, self.Y]
@@ -107,14 +127,29 @@ class BilinearDiag(Model):
                                                     labels, self.label_smoothing, self.ONE_TO_N, self.relation_count)
         return self._one_to_n_loss
 
+    def _self_adversarial(self):
+        """(loss, reg, energies) of self-adversarial negative sampling over the fed X in the sampler's layout (n
+        positives, then NegativeSampleRate blocks of their corruptions); Y is not read (ops.self_adversarial_loss)."""
+        if self._self_adversarial_loss is None:
+            subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='train')
+            assert subject_codes is object_codes, "self-adversarial training expects one shared entity code matrix"
+            self._self_adversarial_loss = ops.self_adversarial_loss(
+                subject_codes.contiguous(), relation_codes.contiguous(), self._x_device(), self.negative_sample_rate,
+                self.adversarial_temperature, self.ONE_TO_N)
+        return self._self_adversarial_loss
+
     def get_loss(self, mode='train'):
         if mode == 'train' and self.training_objective == '1-N':
             return self._one_to_n()[0]
+        if mode == 'train' and self.training_objective == 'SelfAdversarial':
+            return self._self_adversarial()[0]
         return self._fused(mode)[1]  # reduce_mean(weighted CE, pos_weight forced to 1) (:27-34)
 
     def local_get_regularization(self):
         if self.training_objective == '1-N':
             return self.regularization_parameter * self._one_to_n()[1]   # L2 of the two rows a query gathers
+        if self.training_objective == 'SelfAdversarial':
+            return self.regularization_parameter * self._self_adversarial()[1]   # L2 of all N triples, as (:63-69)
         return self.regularization_parameter * self._fused('train')[2]  # (:63-69)
 
     def predict(self):

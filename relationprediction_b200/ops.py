@@ -642,6 +642,81 @@ def complex_score(codes, rel, X, Y=None):
     return _ComplexFn.apply(codes, rel, X, Y)
 
 
+SELF_ADVERSARIAL_DECODERS = {"distmult": (_lib.RGCN_DECODER_DISTMULT, "distmult_backward_slices"),
+                             "complex": (_lib.RGCN_DECODER_COMPLEX, "rgcn_complex_backward")}
+
+
+class _SelfAdversarialFn(torch.autograd.Function):
+    """Returns (loss, reg, energies) of rgcn_self_adversarial_forward.  The forward also writes each triple's energy
+    gradient coefficient; the backward is the scorer's own (Y = NULL) with g_energy = g_loss * coef (+ the upstream
+    gradient of the energies) and the L2 term scaled on the device."""
+
+    @staticmethod
+    def forward(ctx, codes, rel, X, K, alpha, decoder):
+        kind, bwd = SELF_ADVERSARIAL_DECODERS[decoder]
+        V, d = codes.shape
+        dev = codes.device
+        N = X.shape[0]
+        energies = torch.empty(N, dtype=torch.float32, device=dev)
+        coef = torch.empty(N, dtype=torch.float32, device=dev)
+        loss2 = torch.empty(2, dtype=torch.float32, device=dev)
+        _call("rgcn_self_adversarial_forward", "rgcn_self_adversarial_workspace_bytes", (N, K),
+              (kind, _ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, K, alpha, _ptr(energies), _ptr(coef),
+               _ptr(loss2)), dev)
+        ctx.bwd = bwd
+        ctx.rel_param = rel
+        ctx.save_for_backward(codes, rel, X, coef)
+        return loss2[0], loss2[1], energies
+
+    @staticmethod
+    def backward(ctx, g_loss, g_reg, g_energy):
+        lib = _lib.load()
+        codes, rel, X, coef = ctx.saved_tensors
+        V, d = codes.shape
+        dev = codes.device
+        ge = None
+        if g_loss is not None:
+            ge = coef * g_loss
+        if g_energy is not None:
+            ge = g_energy.contiguous() if ge is None else ge + g_energy
+        gs = torch.zeros(2, dtype=torch.float32, device=dev)
+        if g_reg is not None:
+            gs[1] = g_reg
+        dcodes = torch.zeros_like(codes)
+        drel = torch.zeros_like(rel)
+        ss = torch.zeros(1, dtype=torch.float32, device=dev) if _SLICE_NORMS else None
+        rc = getattr(lib, ctx.bwd)(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), X.shape[0], None, None, 0.0,
+                                   1.0, _ptr(gs), _ptr(ge), _ptr(dcodes), _ptr(drel), _ptr(ss), _stream(dev))
+        _lib.check(rc, ctx.bwd)
+        if ss is not None:
+            _add_slice_sumsq(ctx.rel_param, ss[0])
+        return dcodes, drel, None, None, None, None
+
+
+def self_adversarial_loss(codes, rel, X, K, alpha, decoder):
+    """Self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) over the fed triples X (CUDA int32 [N, 3]) in
+    the negative sampler's layout: rows 0..n-1 the positives, row i + n j (j = 1..K) the j-th corruption of positive i,
+    N = n (K + 1).  Returns (loss, reg, energies): loss = 1/(2n) sum_i [softplus(-s_i) + sum_j p_ij softplus(s_ij)] with
+    p_ij = softmax_j(alpha s_ij) held constant, reg = the L2 term of ops.distmult over all N triples, energies [N].
+    decoder is "distmult" or "complex".  Differentiable in codes and rel."""
+    if decoder not in SELF_ADVERSARIAL_DECODERS:
+        raise ValueError("self_adversarial_loss: decoder must be one of %s, got %r"
+                         % (sorted(SELF_ADVERSARIAL_DECODERS), decoder))
+    K, alpha = int(K), float(alpha)
+    if K < 1:
+        raise ValueError("self_adversarial_loss: NegativeSampleRate must be >= 1, got %d" % K)
+    if not 0.0 <= alpha < float("inf"):
+        raise ValueError("self_adversarial_loss: AdversarialTemperature must be finite and >= 0, got %r" % (alpha,))
+    _check_cuda_f32("codes", codes)
+    _check_cuda_f32("relation table", rel)
+    if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
+        raise _lib.RgcnError("X must be a contiguous CUDA int32 [N,3] tensor")
+    if X.shape[0] % (K + 1):
+        raise ValueError("self_adversarial_loss: %d fed triples are not n positives with NegativeSampleRate=%d "
+                         "corruptions each (N %% (K + 1) != 0)" % (X.shape[0], K))
+    return _SelfAdversarialFn.apply(codes, rel, X, K, alpha, decoder)
+
+
 def gemm_tf32x3(A, B, b_is_nk=False, out=None, accumulate=False):
     """C = A @ B (B [K,N]) or A @ B.T (B [N,K], b_is_nk=True) on the wgmma tensor cores with the
     3xTF32 split (fp32-level accuracy).  Thin wrapper over rgcn_gemm_tf32x3 (include/rgcn_b200.h)."""

@@ -304,6 +304,8 @@ def main(argv=None):
         from . import ops
         model.set_one_to_n_labels(ops.OneToNLabels(train, len(entities), len(relations), args.device))
         print("Training objective: 1-N, label smoothing %g" % model.label_smoothing)
+    if model.training_objective == 'SelfAdversarial':
+        print("Training objective: SelfAdversarial, temperature %s" % model.adversarial_temperature)
     no_y = np.zeros(0, dtype=np.float32)
 
     def sample():
