@@ -745,6 +745,53 @@ int rgcn_self_adversarial_forward(int32_t decoder, const float* codes, const flo
                                   int32_t d, const int32_t* X, int64_t N, int32_t K, float alpha, float* energies,
                                   float* coef, float* loss_out, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * RotatE decoder (Sun et al., ICLR 2019).  d % 4 == 0 is required (else RGCN_ERR_INVALID); h = d/2.  Entity rows are
+ * [re | im] as for ComplEx; the first h columns of relation row r are its phases theta (radians, any real value);
+ * columns h..d-1 of a relation row are never read and get no gradient.  With a = codes[X[n,0]], c = codes[X[n,2]],
+ * theta = rel[X[n,1]][0..h-1] and gamma the margin (finite, else RGCN_ERR_INVALID):
+ *
+ *   u_k = a_k e^{i theta_k} - c_k,   energy[n] = gamma - sum_k |u_k|
+ *   loss_out[0] = mean_n( (1-y)x + log1p(exp(-|x|)) + max(-x,0) )          (only if Y != NULL)
+ *   loss_out[1] = mean(a^2) + mean(c^2) over the gathered entity rows, each mean over N*d (un-scaled; phases are
+ *                 not regularised)
+ * Shapes, pointers and the backward's upstream gradients (g_loss, g_reg, g_scale_dev[2], g_energy[N]) are those of
+ * rgcn_complex_forward / rgcn_complex_backward; gamma is checked, the backward reads the energies.  The backward
+ * ACCUMULATES (+=) into dcodes [V,d] and drel [Vrel,d], with m = |u|, w = u/m (0 where m = 0), p = a e^{i theta}:
+ *   dD/dc = -w,  dD/da = [w_re cos + w_im sin, -w_re sin + w_im cos],  dD/dtheta = w_im p_re - w_re p_im,  dE = -dD
+ * plus 2*g_reg*x/(N*d) on the entity rows, and, when rel_slice_sumsq != NULL, adds to that device float the sum over
+ * triples of |dL/dtheta|^2 (the relation table's IndexedSlices term).
+ *
+ * rgcn_rotate_self_adversarial_forward: rgcn_self_adversarial_forward for RotatE (same layout, loss, coef, workspace
+ * rgcn_self_adversarial_workspace_bytes(N, K) and errors) with the L2 term above; its backward is rgcn_rotate_backward
+ * with Y = NULL and g_energy = g_loss coef.
+ *
+ * rgcn_rotate_rank: all-entity ranking by distance.  Side 1 (objects corrupted, gold o) uses q = a e^{i theta}, side 0
+ * (subjects corrupted, gold s) q = c e^{-i theta}; for every entity v, D_v = sum_k |q_k - v_k| in float32, and
+ *   raw_rank[t]      = #{ v : D_v <= D_gold }                                   (the gold always counts itself)
+ *   filtered_rank[t] = raw_rank[t] - #{ v in known(t) : D_v <= D_gold } + 1
+ * -- distmult_rank's counting rules on the distance, so the ranks do not depend on gamma.  Every D_v, the gold's
+ * included, is summed in one fixed order, so equal rows tie exactly.  known_mask, raw_rank, filtered_rank as
+ * distmult_rank; workspace rgcn_rotate_rank_workspace_bytes(V, d, n) (no split to reuse).
+ * Errors, before any device work: RGCN_ERR_INVALID (null pointers, sizes, d % 4 != 0, gamma not finite, side,
+ * filtered ranks without a known mask, and those of rgcn_self_adversarial_forward), RGCN_ERR_WORKSPACE,
+ * RGCN_ERR_NODEVICE.  rgcn_rotate_rank_workspace_bytes returns RGCN_ERR_INVALID (-1) on bad arguments.
+ * ---------------------------------------------------------------------------------------------- */
+int rgcn_rotate_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                        int64_t N, const float* Y, float gamma, float* energies, float* loss_out, void* stream);
+int rgcn_rotate_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                         int64_t N, const float* Y, float gamma, const float* energies, float g_loss, float g_reg,
+                         const float* g_scale_dev, const float* g_energy, float* dcodes, float* drel,
+                         float* rel_slice_sumsq, void* stream);
+int rgcn_rotate_self_adversarial_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                         const int32_t* X, int64_t N, int32_t K, float alpha, float gamma,
+                                         float* energies, float* coef, float* loss_out, void* workspace,
+                                         int64_t workspace_bytes, void* stream);
+int64_t rgcn_rotate_rank_workspace_bytes(int32_t V, int32_t d, int64_t n);
+int rgcn_rotate_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                     int64_t n, int side, const uint32_t* known_mask, int32_t* raw_rank, int32_t* filtered_rank,
+                     void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

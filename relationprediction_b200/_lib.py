@@ -39,6 +39,8 @@ EXPORTED_SYMBOLS = [
     "rgcn_one_to_n_labels_workspace_bytes", "rgcn_one_to_n_labels",
     "rgcn_one_to_n_finish_workspace_bytes", "rgcn_one_to_n_finish",
     "rgcn_self_adversarial_workspace_bytes", "rgcn_self_adversarial_forward",
+    "rgcn_rotate_forward", "rgcn_rotate_backward", "rgcn_rotate_self_adversarial_forward",
+    "rgcn_rotate_rank_workspace_bytes", "rgcn_rotate_rank",
 ]
 
 RGCN_DECODER_DISTMULT, RGCN_DECODER_COMPLEX = 0, 1
@@ -260,6 +262,19 @@ def _declare(lib):
     lib.rgcn_self_adversarial_forward.restype = c_int
     lib.rgcn_self_adversarial_forward.argtypes = [c_int32, vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int32,
                                                   c_float, vp, vp, vp, vp, c_int64, vp]
+    lib.rgcn_rotate_forward.restype = c_int
+    lib.rgcn_rotate_forward.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, vp, c_float, vp, vp, vp]
+    lib.rgcn_rotate_backward.restype = c_int
+    lib.rgcn_rotate_backward.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, vp, c_float, vp, c_float,
+                                         c_float, vp, vp, vp, vp, vp, vp]
+    lib.rgcn_rotate_self_adversarial_forward.restype = c_int
+    lib.rgcn_rotate_self_adversarial_forward.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int32,
+                                                         c_float, c_float, vp, vp, vp, vp, c_int64, vp]
+    lib.rgcn_rotate_rank_workspace_bytes.restype = c_int64
+    lib.rgcn_rotate_rank_workspace_bytes.argtypes = [c_int32, c_int32, c_int64]
+    lib.rgcn_rotate_rank.restype = c_int
+    lib.rgcn_rotate_rank.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, vp, vp, vp, vp, c_int64,
+                                     vp]
 
 
 def load():

@@ -4,10 +4,12 @@ Only the branches on the accelerated path are built: encoders `gcn_diag` (DiagGc
 when Concatenation=Yes, BasisGcnTimesDiag when DiagonalCoefficients=Yes; with UseInputTransform=No layer 0 is a one-hot
 BasisGcn; SkipConnections=Highway wraps every
 feature-input layer in a HighwayLayer), `embedding`, and the variational encoders `variational_embedding` and
-`variational_gcn_basis` (a VariationalEncoding over two linear AffineTransform heads); decoders `bilinear-diag` and `complex`.  Unknown names return None exactly
+`variational_gcn_basis` (a VariationalEncoding over two linear AffineTransform heads); decoders `bilinear-diag`, `complex` and
+`rotate` (RotatE, which the reference does not have).  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag, parse_training_objective
 from ..decoders.complex import Complex
+from ..decoders.rotate import Rotate
 from ..encoders.affine_transform import AffineTransform
 from ..encoders.message_gcns.gcn_basis import BasisGcn
 from ..encoders.message_gcns.gcn_basis_concat import ConcatGcn
@@ -165,11 +167,15 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
 def build_decoder(encoder, decoder_settings):
     if decoder_settings['Name'] not in ("bilinear-diag", "complex"):
         objective = parse_training_objective(decoder_settings)[0]
-        if objective != 'NegativeSampling':
+        # RotatE trains under SelfAdversarial (the objective of its paper) but has no 1-N scoring GEMM
+        if objective != 'NegativeSampling' and not (decoder_settings['Name'] == "rotate"
+                                                    and objective == 'SelfAdversarial'):
             raise ValueError("TrainingObjective=%s needs the bilinear-diag or complex decoder, not %r"
                              % (objective, decoder_settings['Name']))
     if decoder_settings['Name'] == "bilinear-diag":
         return BilinearDiag(encoder, decoder_settings)
     if decoder_settings['Name'] == "complex":
         return Complex(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
+    if decoder_settings['Name'] == "rotate":
+        return Rotate(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
     return None

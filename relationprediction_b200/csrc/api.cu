@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <string>
@@ -2198,16 +2199,10 @@ extern "C" int64_t rgcn_self_adversarial_workspace_bytes(int64_t N, int32_t K) {
   return align_up(2 * (N / ((int64_t)K + 1)) * 4) + 256;
 }
 
-extern "C" int rgcn_self_adversarial_forward(int32_t decoder, const float* codes, const float* rel, int32_t V,
-                                             int32_t Vrel, int32_t d, const int32_t* X, int64_t N, int32_t K,
-                                             float alpha, float* energies, float* coef, float* loss_out,
-                                             void* workspace, int64_t workspace_bytes, void* stream) {
-  const std::string who = "rgcn_self_adversarial_forward";
-  if (decoder != RGCN_DECODER_DISTMULT && decoder != RGCN_DECODER_COMPLEX) {
-    rgcn_set_error(who + ": unknown decoder kind (RGCN_DECODER_DISTMULT or RGCN_DECODER_COMPLEX)");
-    return RGCN_ERR_INVALID;
-  }
-  if (!codes || !rel || !loss_out || !workspace || (N > 0 && (!X || !energies || !coef))) {
+// the argument checks of both self-adversarial entry points, in order, before any device work
+static int self_adversarial_checks(const std::string& who, bool pointers_ok, int32_t V, int32_t Vrel, int32_t d,
+                                   int64_t N, int32_t K, float alpha, int64_t workspace_bytes) {
+  if (!pointers_ok) {
     rgcn_set_error(who + ": null pointer");
     return RGCN_ERR_INVALID;
   }
@@ -2228,11 +2223,132 @@ extern "C" int rgcn_self_adversarial_forward(int32_t decoder, const float* codes
     rgcn_set_error(who + ": workspace too small (rgcn_self_adversarial_workspace_bytes)");
     return RGCN_ERR_WORKSPACE;
   }
-  int rc = onen_device_checks(who.c_str());
+  return onen_device_checks(who.c_str());
+}
+
+extern "C" int rgcn_self_adversarial_forward(int32_t decoder, const float* codes, const float* rel, int32_t V,
+                                             int32_t Vrel, int32_t d, const int32_t* X, int64_t N, int32_t K,
+                                             float alpha, float* energies, float* coef, float* loss_out,
+                                             void* workspace, int64_t workspace_bytes, void* stream) {
+  const std::string who = "rgcn_self_adversarial_forward";
+  if (decoder != RGCN_DECODER_DISTMULT && decoder != RGCN_DECODER_COMPLEX) {
+    rgcn_set_error(who + ": unknown decoder kind (RGCN_DECODER_DISTMULT or RGCN_DECODER_COMPLEX)");
+    return RGCN_ERR_INVALID;
+  }
+  const int rc = self_adversarial_checks(
+      who, codes && rel && loss_out && workspace && (N <= 0 || (X && energies && coef)), V, Vrel, d, N, K, alpha,
+      workspace_bytes);
   if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
   Carver ws(workspace, workspace_bytes);
   float* parts = ws.take<float>(2 * (N / ((int64_t)K + 1)));
-  return launch_self_adversarial_forward(decoder == RGCN_DECODER_COMPLEX, codes, rel, d, X, N, K, alpha, energies,
-                                         coef, loss_out, parts, st);
+  return launch_self_adversarial_forward(decoder == RGCN_DECODER_COMPLEX ? SELFADV_COMPLEX : SELFADV_DISTMULT, codes,
+                                         rel, d, X, N, K, alpha, 0.f, energies, coef, loss_out, parts,
+                                         (cudaStream_t)stream);
+}
+
+// ------------------------------------------------------------------------------------------------
+// RotatE (rotate.cu): scorer, backward, self-adversarial forward and all-entity ranking by distance.  Every argument
+// is checked before any device work, with the ComplEx rules plus a finite gamma.
+// ------------------------------------------------------------------------------------------------
+static int rotate_checks(const std::string& who, bool pointers_ok, int32_t V, int32_t Vrel, int32_t d, int64_t N,
+                         float gamma) {
+  if (!pointers_ok) {
+    rgcn_set_error(who + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 || N < 0) {
+    rgcn_set_error(who + ": bad sizes (need V > 0, Vrel > 0, d > 0, d % 4 == 0, N >= 0)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!std::isfinite(gamma)) {
+    rgcn_set_error(who + ": the margin gamma must be finite");
+    return RGCN_ERR_INVALID;
+  }
+  return onen_device_checks(who.c_str());
+}
+
+extern "C" int rgcn_rotate_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                   const int32_t* X, int64_t N, const float* Y, float gamma, float* energies,
+                                   float* loss_out, void* stream) {
+  const int rc = rotate_checks("rgcn_rotate_forward", codes && rel && loss_out && (N <= 0 || (X && energies)), V, Vrel,
+                               d, N, gamma);
+  if (rc) return rc;
+  return launch_rotate_forward(codes, rel, d, X, N, Y, gamma, energies, loss_out, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_rotate_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                    const int32_t* X, int64_t N, const float* Y, float gamma, const float* energies,
+                                    float g_loss, float g_reg, const float* g_scale_dev, const float* g_energy,
+                                    float* dcodes, float* drel, float* rel_slice_sumsq, void* stream) {
+  const int rc = rotate_checks("rgcn_rotate_backward",
+                               codes && rel && dcodes && drel && (N <= 0 || X) && (!Y || energies), V, Vrel, d, N,
+                               gamma);
+  if (rc) return rc;
+  return launch_rotate_backward(codes, rel, d, X, N, Y, energies, g_loss, g_reg, g_scale_dev, g_energy, dcodes, drel,
+                                rel_slice_sumsq, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_rotate_self_adversarial_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                                                    int32_t d, const int32_t* X, int64_t N, int32_t K, float alpha,
+                                                    float gamma, float* energies, float* coef, float* loss_out,
+                                                    void* workspace, int64_t workspace_bytes, void* stream) {
+  const std::string who = "rgcn_rotate_self_adversarial_forward";
+  if (!std::isfinite(gamma)) {
+    rgcn_set_error(who + ": the margin gamma must be finite");
+    return RGCN_ERR_INVALID;
+  }
+  const int rc = self_adversarial_checks(
+      who, codes && rel && loss_out && workspace && (N <= 0 || (X && energies && coef)), V, Vrel, d, N, K, alpha,
+      workspace_bytes);
+  if (rc) return rc;
+  Carver ws(workspace, workspace_bytes);
+  float* parts = ws.take<float>(2 * (N / ((int64_t)K + 1)));
+  return launch_self_adversarial_forward(SELFADV_ROTATE, codes, rel, d, X, N, K, alpha, gamma, energies, coef,
+                                         loss_out, parts, (cudaStream_t)stream);
+}
+
+// Workspace layout: [Q n*d | gold_D n | gold_col n | raw_cnt n | known_cnt n]
+extern "C" int64_t rgcn_rotate_rank_workspace_bytes(int32_t V, int32_t d, int64_t n) {
+  if (V <= 0 || d <= 0 || d % 4 != 0 || n < 0) {
+    rgcn_set_error("rgcn_rotate_rank_workspace_bytes: bad arguments (need V > 0, d % 4 == 0, n >= 0)");
+    return RGCN_ERR_INVALID;
+  }
+  return align_up(n * d * 4) + 4 * align_up(n * 4) + 256;
+}
+
+extern "C" int rgcn_rotate_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                const int32_t* X, int64_t n, int side, const uint32_t* known_mask,
+                                int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                                void* stream) {
+  const std::string who = "rgcn_rotate_rank";
+  if (!codes || !rel || !workspace || (n > 0 && (!X || !raw_rank))) {
+    rgcn_set_error(who + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 || n < 0 || n > 0x7fffffffLL || (side != 0 && side != 1)) {
+    rgcn_set_error(who + ": bad arguments (need V > 0, Vrel > 0, d % 4 == 0, 0 <= n < 2^31, side in {0,1})");
+    return RGCN_ERR_INVALID;
+  }
+  if (filtered_rank && !known_mask) {
+    rgcn_set_error(who + ": bad arguments (filtered ranks need a known mask)");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_rotate_rank_workspace_bytes(V, d, n)) {
+    rgcn_set_error(who + ": workspace too small (rgcn_rotate_rank_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  int rc = onen_device_checks(who.c_str());
+  if (rc || n == 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver ws(workspace, workspace_bytes);
+  float* Q = ws.take<float>(n * d);
+  float* gold_D = ws.take<float>(n);
+  int32_t* gold_col = ws.take<int32_t>(n);
+  int32_t* raw_cnt = ws.take<int32_t>(n);
+  int32_t* known_cnt = ws.take<int32_t>(n);
+  rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
+  if (!rc) rc = launch_rotate_rank_prepare(codes, rel, d, X, n, side, Q, gold_D, gold_col, st);
+  if (!rc) rc = launch_rotate_rank(Q, codes, V, d, n, gold_D, gold_col, known_mask, raw_cnt, known_cnt, st);
+  if (!rc) rc = launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
+  return rc;
 }

@@ -299,9 +299,27 @@ int launch_complex_rank_prepare(const float* codes, const float* rel, int d, con
 int launch_complex_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n,
                                     float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
 
-// self_adversarial.cu -- self-adversarial objective over N = n (K + 1) triples in the sampler's layout (complex = 0
-// DistMult, 1 ComplEx): energies [N], the energy-gradient coefficients coef [N], loss_out[0] the loss, loss_out[1] the
-// L2 term of distmult_forward; parts: 2n floats of scratch for the per-group loss and norm parts
-int launch_self_adversarial_forward(int complex, const float* codes, const float* rel, int d, const int32_t* X,
-                                    int64_t N, int K, float alpha, float* energies, float* coef, float* loss_out,
-                                    float* parts, cudaStream_t st);
+// self_adversarial.cu -- self-adversarial objective over N = n (K + 1) triples in the sampler's layout (decoder: one of
+// the SELFADV_* kinds; gamma is read by RotatE only): energies [N], the energy-gradient coefficients coef [N],
+// loss_out[0] the loss, loss_out[1] the decoder's L2 term of its NegativeSampling forward; parts: 2n floats of scratch
+// for the per-group loss and norm parts
+enum { SELFADV_DISTMULT = 0, SELFADV_COMPLEX = 1, SELFADV_ROTATE = 2 };
+int launch_self_adversarial_forward(int decoder, const float* codes, const float* rel, int d, const int32_t* X,
+                                    int64_t N, int K, float alpha, float gamma, float* energies, float* coef,
+                                    float* loss_out, float* parts, cudaStream_t st);
+
+// rotate.cu -- RotatE (DESIGN.md section 1).  Scorer and backward: the contracts of the ComplEx launchers with the
+// margin gamma; rows [re | im], the phases in the first d / 2 columns of the relation row.
+int launch_rotate_forward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                          float gamma, float* energies, float* loss_out, cudaStream_t st);
+int launch_rotate_backward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                           const float* energies, float g_loss, float g_reg, const float* g_scale_dev,
+                           const float* g_energy, float* dcodes, float* drel, float* rel_slice_sumsq, cudaStream_t st);
+// all-entity ranking by distance: query rows Q [n, d] ([re | im]; side 1: codes[s] e^{i theta}, side 0:
+// codes[o] e^{-i theta}), gold_D[t] the gold's distance and gold_col[t] its id; then raw_cnt / known_cnt (zeroed by the
+// caller) += the counts of D_v <= gold_D (the gold always counts) over all V entities
+int launch_rotate_rank_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
+                               float* Q, float* gold_D, int32_t* gold_col, cudaStream_t st);
+int launch_rotate_rank(const float* Q, const float* codes, int V, int d, int64_t n, const float* gold_D,
+                       const int32_t* gold_col, const uint32_t* known, int32_t* raw_cnt, int32_t* known_cnt,
+                       cudaStream_t st);

@@ -1,5 +1,5 @@
-// self_adversarial.cu -- self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) for the DistMult and
-// ComplEx decoders, sm_90a: the forward of the objective, which also writes each triple's energy gradient.
+// self_adversarial.cu -- self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) for the DistMult, ComplEx
+// and RotatE decoders, sm_90a: the forward of the objective, which also writes each triple's energy gradient.
 //
 // The fed triples follow the negative sampler's layout (auxilliaries.py:13-33): for N = n (K + 1) rows, rows 0..n-1
 // are the positives and row i + n j (j = 1..K) is the j-th corruption of positive i.  With s_i the positive's energy
@@ -33,12 +33,13 @@ __device__ __forceinline__ float sigmoid(float x) { return 1.f / (1.f + expf(-x)
 // triples in order with the decoder's row arithmetic (Rows) and keeps a running max m and sum S of exp(alpha s - m)
 // over the corruptions; lane j % 32 stores energy j.  Pass 2 walks the group in strides of 32 -- so any K works -- and
 // every lane reads back only the energies it stored itself, forms p, the coefficient and its loss terms.  The loss and
-// the squared norms of the group's rows go to one part each per group, for a reduction in a fixed order.
+// the squared norms of the group's rows go to one part each per group, for a reduction in a fixed order.  `rows` is
+// the decoder's functor (RotateRows carries gamma); it comes last so the other parameters keep their offsets.
 template <class Rows>
 __global__ void __launch_bounds__(256)
     k_selfadv_fwd(const float* __restrict__ codes, const float* __restrict__ rel, int d, const int32_t* __restrict__ X,
                   int64_t n, int K, float alpha, float inv_2n, float* energies, float* __restrict__ coef,
-                  float* __restrict__ loss_part, float* __restrict__ reg_part) {
+                  float* __restrict__ loss_part, float* __restrict__ reg_part, Rows rows) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int64_t i = (int64_t)blockIdx.x * 8 + warp; i < n; i += (int64_t)gridDim.x * 8) {
     float m = -INFINITY, S = 0.f, q = 0.f;
@@ -46,7 +47,7 @@ __global__ void __launch_bounds__(256)
       const int64_t t = i + n * j;
       const int s = __ldg(X + 3 * t), r = __ldg(X + 3 * t + 1), o = __ldg(X + 3 * t + 2);
       float e = 0.f;
-      Rows::partial(codes, rel, d, s, r, o, lane, e, q);
+      rows.partial(codes, rel, d, s, r, o, lane, e, q);
       e = warp_sum(e);   // the xor butterfly leaves the same sum in every lane
       if (lane == (j & 31)) energies[t] = e;
       if (j > 0) {
@@ -88,24 +89,30 @@ int check_launch(const char* what) {
 
 }  // namespace
 
-int launch_self_adversarial_forward(int complex, const float* codes, const float* rel, int d, const int32_t* X,
-                                    int64_t N, int K, float alpha, float* energies, float* coef, float* loss_out,
-                                    float* parts, cudaStream_t st) {
+int launch_self_adversarial_forward(int decoder, const float* codes, const float* rel, int d, const int32_t* X,
+                                    int64_t N, int K, float alpha, float gamma, float* energies, float* coef,
+                                    float* loss_out, float* parts, cudaStream_t st) {
   if (N == 0) return rgcn_check_cuda(cudaMemsetAsync(loss_out, 0, 2 * sizeof(float), st), "memset(loss)");
   const int64_t n = N / (K + 1);
   float* loss_part = parts;
   float* reg_part = parts + n;
   const int blocks = (int)std::min<int64_t>((n + 7) / 8, 132 * 8);
   const float inv_2n = (float)(0.5 / (double)n);
-  if (!complex)
-    k_selfadv_fwd<DistMultRows><<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef,
-                                                        loss_part, reg_part);
+  if (decoder == SELFADV_DISTMULT)
+    k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
+                                          DistMultRows{});
+  else if (decoder == SELFADV_COMPLEX && d % 8 == 0)
+    k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
+                                          ComplexRows<4>{});
+  else if (decoder == SELFADV_COMPLEX)
+    k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
+                                          ComplexRows<2>{});
   else if (d % 8 == 0)
-    k_selfadv_fwd<ComplexRows<4>><<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef,
-                                                          loss_part, reg_part);
+    k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
+                                          RotateRows<4>{gamma});
   else
-    k_selfadv_fwd<ComplexRows<2>><<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef,
-                                                          loss_part, reg_part);
+    k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
+                                          RotateRows<2>{gamma});
   int rc = check_launch("k_selfadv_fwd");
   if (rc) return rc;
   // loss[0] = (sum of the loss parts) / (2n), loss[1] = (sum of the squared norms) / (N d): the NegativeSampling L2 term

@@ -1,7 +1,7 @@
-// triple_rows.cuh -- the row arithmetic of the DistMult and ComplEx triple scorers: one warp owns one triple
-// (s, r, o) and each lane forms its share of the energy and of the squared norms of the three gathered rows.  Shared by
-// the NegativeSampling scorers (distmult.cu / complex.cu) and the self-adversarial scorer (self_adversarial.cu), so
-// both objectives score a triple with the same float operations in the same order.
+// triple_rows.cuh -- the row arithmetic of the DistMult, ComplEx and RotatE triple scorers: one warp owns one triple
+// (s, r, o) and each lane forms its share of the energy and of the squared norms of the gathered rows.  Shared by
+// the NegativeSampling scorers (distmult.cu / complex.cu / rotate.cu) and the self-adversarial scorer
+// (self_adversarial.cu), so both objectives score a triple with the same float operations in the same order.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -82,6 +82,56 @@ struct ComplexRows {
         e = fmaf(bi[j], fmaf(ar[j], ci[j], -ai[j] * cr[j]), e);
         q += ar[j] * ar[j] + ai[j] * ai[j];
         q += br[j] * br[j] + bi[j] * bi[j];
+        q += cr[j] * cr[j] + ci[j] * ci[j];
+      }
+    }
+  }
+};
+
+// |u| for RotatE: the hardware square root (sqrt.approx.ftz.f32, one MUFU instruction).  The IEEE sqrtf calls a
+// slow-path subroutine, and the registers live across that call go to local memory.
+__device__ __forceinline__ float rotate_modulus(float ur, float ui) {
+  float m;
+  asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(m) : "f"(__fmaf_rn(ur, ur, __fmul_rn(ui, ui))));
+  return m;
+}
+
+// RotatE: u = a e^{i theta} - c for one column pair (a = ar + i ai, c = cr + i ci), with (sn, cs) = sincos(theta) --
+// full range reduction: phases are unbounded.  The scorer, its backward and the self-adversarial scorer all form u
+// here, so the backward differentiates exactly the forward's residual.
+__device__ __forceinline__ void rotate_residual(float ar, float ai, float th, float cr, float ci, float& ur, float& ui,
+                                                float& sn, float& cs) {
+  sincosf(th, &sn, &cs);
+  ur = fmaf(ar, cs, fmaf(-ai, sn, -cr));
+  ui = fmaf(ar, sn, fmaf(ai, cs, -ci));
+}
+
+// RotatE (DESIGN.md section 1): energy gamma - sum_k |a_k e^{i theta_k} - c_k| with entity rows [re | im] (h = d / 2
+// columns each) and the phases theta in the first h columns of the relation row; the other h are never read.  A lane
+// owns the column pairs (k, k + h) as ComplexRows<W> does; lane 0's share carries gamma.  q gets the squared norms of
+// the two entity rows only: phases are not regularised.
+template <int W>
+struct RotateRows {
+  float gamma;
+
+  __device__ __forceinline__ void partial(const float* __restrict__ codes, const float* __restrict__ rel, int d, int s,
+                                          int r, int o, int lane, float& e, float& q) const {
+    const float* e1 = codes + (size_t)s * d;
+    const float* th = rel + (size_t)r * d;
+    const float* e2 = codes + (size_t)o * d;
+    const int h = d >> 1;
+    if (lane == 0) e += gamma;
+    for (int k = lane * W; k < h; k += 32 * W) {
+      float ar[W], ai[W], t[W], cr[W], ci[W];
+      Vec<W>::load(e1 + k, ar), Vec<W>::load(e1 + h + k, ai);
+      Vec<W>::load(th + k, t);
+      Vec<W>::load(e2 + k, cr), Vec<W>::load(e2 + h + k, ci);
+#pragma unroll
+      for (int j = 0; j < W; ++j) {
+        float ur, ui, sn, cs;
+        rotate_residual(ar[j], ai[j], t[j], cr[j], ci[j], ur, ui, sn, cs);
+        e -= rotate_modulus(ur, ui);
+        q += ar[j] * ar[j] + ai[j] * ai[j];
         q += cr[j] * cr[j] + ci[j] * ci[j];
       }
     }

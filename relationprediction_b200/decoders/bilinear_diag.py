@@ -135,8 +135,12 @@ class BilinearDiag(Model):
             assert subject_codes is object_codes, "self-adversarial training expects one shared entity code matrix"
             self._self_adversarial_loss = ops.self_adversarial_loss(
                 subject_codes.contiguous(), relation_codes.contiguous(), self._x_device(), self.negative_sample_rate,
-                self.adversarial_temperature, self.ONE_TO_N)
+                self.adversarial_temperature, self.ONE_TO_N, **self._self_adversarial_args())
         return self._self_adversarial_loss
+
+    def _self_adversarial_args(self):
+        """decoder parameters ops.self_adversarial_loss takes by keyword (the RotatE margin)"""
+        return {}
 
     def get_loss(self, mode='train'):
         if mode == 'train' and self.training_objective == '1-N':

@@ -63,9 +63,11 @@ class Ensemble(object):
 
     # ---- fused path (Scorer.compute_mrr_scores prefers it) ----
     def supports_fused_ranking(self):
-        """Both members have a fused ranker (DistMult or ComplEx decoder) and live on the same CUDA device."""
+        """Both members have a fused ranker (DistMult or ComplEx decoder) and live on the same CUDA device.  A RotatE
+        member ranks by distance, which the ensemble's scoring GEMM cannot combine: its ranks come from the score
+        matrices."""
         for m in (self.a, self.b):
-            if not (hasattr(m, 'test_ranker') and m.supports_fused_ranking()):
+            if not (hasattr(m, 'test_ranker') and getattr(m, 'ensemble_fused', True) and m.supports_fused_ranking()):
                 return False
         return self.a.get_device() == self.b.get_device()
 

@@ -555,8 +555,9 @@ def variational(H, W_mu, b_mu, W_sigma, b_sigma, eps):
     return _VariationalFn.apply(H, W_mu, b_mu, W_sigma, b_sigma, eps)
 
 
-def _triple_forward(ctx, entry, codes, rel, X, Y):
-    """Forward of a triple scorer entry point with the distmult_forward argument list."""
+def _triple_forward(ctx, entry, codes, rel, X, Y, extra=()):
+    """Forward of a triple scorer entry point with the distmult_forward argument list; `extra` goes after Y (the
+    margin of rgcn_rotate_forward)."""
     lib = _lib.load()
     _check_cuda_f32("codes", codes)
     _check_cuda_f32("relation table", rel)
@@ -570,10 +571,11 @@ def _triple_forward(ctx, entry, codes, rel, X, Y):
     N = X.shape[0]
     energies = torch.empty(N, dtype=torch.float32, device=dev)
     loss2 = torch.empty(2, dtype=torch.float32, device=dev)
-    rc = getattr(lib, entry)(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, _ptr(Y),
+    rc = getattr(lib, entry)(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, _ptr(Y), *extra,
                              _ptr(energies), _ptr(loss2), _stream(dev))
     _lib.check(rc, entry)
     ctx.has_y = Y is not None
+    ctx.extra = extra
     ctx.rel_param = rel
     ctx.save_for_backward(codes, rel, X, Y if Y is not None else torch.empty(0, device=dev),
                           energies)
@@ -581,7 +583,8 @@ def _triple_forward(ctx, entry, codes, rel, X, Y):
 
 
 def _triple_backward(ctx, entry, g_energy, g_loss, g_reg):
-    """Backward of a triple scorer entry point with the distmult_backward_slices argument list."""
+    """Backward of a triple scorer entry point with the distmult_backward_slices argument list; the forward's `extra`
+    goes after Y."""
     lib = _lib.load()
     codes, rel, X, Y, energies = ctx.saved_tensors
     Y = Y if ctx.has_y else None
@@ -600,7 +603,7 @@ def _triple_backward(ctx, entry, g_energy, g_loss, g_reg):
         gs[1] = g_reg
     ss = torch.zeros(1, dtype=torch.float32, device=dev) if _SLICE_NORMS else None
     rc = getattr(lib, entry)(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), X.shape[0],
-                             _ptr(Y), _ptr(energies), 1.0, 1.0, _ptr(gs), _ptr(ge),
+                             _ptr(Y), *ctx.extra, _ptr(energies), 1.0, 1.0, _ptr(gs), _ptr(ge),
                              _ptr(dcodes), _ptr(drel), _ptr(ss), _stream(dev))
     _lib.check(rc, entry)
     if ss is not None:
@@ -642,8 +645,36 @@ def complex_score(codes, rel, X, Y=None):
     return _ComplexFn.apply(codes, rel, X, Y)
 
 
+def _check_gamma(gamma):
+    gamma = float(gamma)
+    if not np.isfinite(gamma):
+        raise ValueError("the RotatE margin gamma must be finite, got %r" % (gamma,))
+    return gamma
+
+
+class _RotateFn(torch.autograd.Function):
+    """Returns (energies[N], loss, reg) of the RotatE scorer, same conventions as _DistMultFn."""
+
+    @staticmethod
+    def forward(ctx, codes, rel, X, Y, gamma):
+        return _triple_forward(ctx, "rgcn_rotate_forward", codes, rel, X, Y, (gamma,))
+
+    @staticmethod
+    def backward(ctx, g_energy, g_loss, g_reg):
+        return _triple_backward(ctx, "rgcn_rotate_backward", g_energy, g_loss, g_reg) + (None,)
+
+
+def rotate_score(codes, rel, X, Y=None, *, gamma):
+    """RotatE energies gamma - sum_k |a_k e^{i theta_k} - c_k| (entity rows [re | im], the phases theta in the first
+    d/2 columns of the relation row), the mean sigmoid cross-entropy (0 if Y is None) and the L2 term
+    mean(a^2) + mean(c^2) of the gathered entity rows (include/rgcn_b200.h, rgcn_rotate_forward)."""
+    return _RotateFn.apply(codes, rel, X, Y, _check_gamma(gamma))
+
+
+# decoder -> (the decoder kind of rgcn_self_adversarial_forward, or None: its own entry point; the scorer's backward)
 SELF_ADVERSARIAL_DECODERS = {"distmult": (_lib.RGCN_DECODER_DISTMULT, "distmult_backward_slices"),
-                             "complex": (_lib.RGCN_DECODER_COMPLEX, "rgcn_complex_backward")}
+                             "complex": (_lib.RGCN_DECODER_COMPLEX, "rgcn_complex_backward"),
+                             "rotate": (None, "rgcn_rotate_backward")}
 
 
 class _SelfAdversarialFn(torch.autograd.Function):
@@ -652,7 +683,7 @@ class _SelfAdversarialFn(torch.autograd.Function):
     gradient of the energies) and the L2 term scaled on the device."""
 
     @staticmethod
-    def forward(ctx, codes, rel, X, K, alpha, decoder):
+    def forward(ctx, codes, rel, X, K, alpha, decoder, gamma):
         kind, bwd = SELF_ADVERSARIAL_DECODERS[decoder]
         V, d = codes.shape
         dev = codes.device
@@ -660,10 +691,16 @@ class _SelfAdversarialFn(torch.autograd.Function):
         energies = torch.empty(N, dtype=torch.float32, device=dev)
         coef = torch.empty(N, dtype=torch.float32, device=dev)
         loss2 = torch.empty(2, dtype=torch.float32, device=dev)
-        _call("rgcn_self_adversarial_forward", "rgcn_self_adversarial_workspace_bytes", (N, K),
-              (kind, _ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, K, alpha, _ptr(energies), _ptr(coef),
-               _ptr(loss2)), dev)
+        rows = (_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, K, alpha)
+        outs = (_ptr(energies), _ptr(coef), _ptr(loss2))
+        if kind is None:
+            _call("rgcn_rotate_self_adversarial_forward", "rgcn_self_adversarial_workspace_bytes", (N, K),
+                  rows + (gamma,) + outs, dev)
+        else:
+            _call("rgcn_self_adversarial_forward", "rgcn_self_adversarial_workspace_bytes", (N, K),
+                  (kind,) + rows + outs, dev)
         ctx.bwd = bwd
+        ctx.extra = () if kind is not None else (gamma,)
         ctx.rel_param = rel
         ctx.save_for_backward(codes, rel, X, coef)
         return loss2[0], loss2[1], energies
@@ -685,23 +722,30 @@ class _SelfAdversarialFn(torch.autograd.Function):
         dcodes = torch.zeros_like(codes)
         drel = torch.zeros_like(rel)
         ss = torch.zeros(1, dtype=torch.float32, device=dev) if _SLICE_NORMS else None
-        rc = getattr(lib, ctx.bwd)(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), X.shape[0], None, None, 0.0,
-                                   1.0, _ptr(gs), _ptr(ge), _ptr(dcodes), _ptr(drel), _ptr(ss), _stream(dev))
+        rc = getattr(lib, ctx.bwd)(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), X.shape[0], None, *ctx.extra,
+                                   None, 0.0, 1.0, _ptr(gs), _ptr(ge), _ptr(dcodes), _ptr(drel), _ptr(ss),
+                                   _stream(dev))
         _lib.check(rc, ctx.bwd)
         if ss is not None:
             _add_slice_sumsq(ctx.rel_param, ss[0])
-        return dcodes, drel, None, None, None, None
+        return dcodes, drel, None, None, None, None, None
 
 
-def self_adversarial_loss(codes, rel, X, K, alpha, decoder):
+def self_adversarial_loss(codes, rel, X, K, alpha, decoder, *, gamma=None):
     """Self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) over the fed triples X (CUDA int32 [N, 3]) in
     the negative sampler's layout: rows 0..n-1 the positives, row i + n j (j = 1..K) the j-th corruption of positive i,
     N = n (K + 1).  Returns (loss, reg, energies): loss = 1/(2n) sum_i [softplus(-s_i) + sum_j p_ij softplus(s_ij)] with
-    p_ij = softmax_j(alpha s_ij) held constant, reg = the L2 term of ops.distmult over all N triples, energies [N].
-    decoder is "distmult" or "complex".  Differentiable in codes and rel."""
+    p_ij = softmax_j(alpha s_ij) held constant, reg = the decoder's L2 term over all N triples, energies [N].
+    decoder is "distmult", "complex" or "rotate"; gamma is the RotatE margin, needed by "rotate" only.
+    Differentiable in codes and rel."""
     if decoder not in SELF_ADVERSARIAL_DECODERS:
         raise ValueError("self_adversarial_loss: decoder must be one of %s, got %r"
                          % (sorted(SELF_ADVERSARIAL_DECODERS), decoder))
+    if (decoder == "rotate") != (gamma is not None):
+        raise ValueError("self_adversarial_loss: the margin gamma goes with decoder 'rotate' only (got decoder %r, "
+                         "gamma %r)" % (decoder, gamma))
+    if gamma is not None:
+        gamma = _check_gamma(gamma)
     K, alpha = int(K), float(alpha)
     if K < 1:
         raise ValueError("self_adversarial_loss: NegativeSampleRate must be >= 1, got %d" % K)
@@ -714,7 +758,7 @@ def self_adversarial_loss(codes, rel, X, K, alpha, decoder):
     if X.shape[0] % (K + 1):
         raise ValueError("self_adversarial_loss: %d fed triples are not n positives with NegativeSampleRate=%d "
                          "corruptions each (N %% (K + 1) != 0)" % (X.shape[0], K))
-    return _SelfAdversarialFn.apply(codes, rel, X, K, alpha, decoder)
+    return _SelfAdversarialFn.apply(codes, rel, X, K, alpha, decoder, gamma)
 
 
 def gemm_tf32x3(A, B, b_is_nk=False, out=None, accumulate=False):
@@ -963,6 +1007,52 @@ class ComplexRanker(DistMultRanker):
     _RANK, _WORKSPACE, _TOPK = "rgcn_complex_rank", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_topk"
     _REL_RANK, _REL_TOPK = "rgcn_complex_relation_rank", "rgcn_complex_relation_topk"
     DECODER = _lib.RGCN_DECODER_COMPLEX
+
+
+class RotateRanker(object):
+    """All-entity ranking of the RotatE decoder by distance (rgcn_rotate_rank): rank(X, side, known_mask) as
+    DistMultRanker.rank, with D_v = sum_k |q_k - v_k| <= D_gold in place of score >= gold score, so the ranks do not
+    depend on the margin.  RotatE has no fused top-k or relation prediction, and is no member of the fused ensemble
+    (EnsembleRanker takes DistMultRanker objects only)."""
+
+    def __init__(self, codes, rel, relation_count=None):
+        _check_cuda_f32("codes", codes)
+        _check_cuda_f32("relation table", rel)
+        self.codes, self.rel = codes, rel
+        self.relation_count = rel.shape[0] if relation_count is None else int(relation_count)
+        self._ws, self._ws_n = None, -1
+
+    _check_rows = DistMultRanker._check_rows
+
+    def rank(self, X, side, known_mask=None):
+        """X int32 [n,3] CUDA; side 0 = subjects corrupted, 1 = objects; known_mask uint32 [n, ceil(V/32)] CUDA (as
+        int32) or None.  Returns (raw_rank, filtered_rank or None) int32 CUDA tensors."""
+        lib = _lib.load()
+        V, d = self.codes.shape
+        self._check_rows(X, known_mask, "known_mask")
+        n = X.shape[0]
+        dev = self.codes.device
+        if self._ws is None or n > self._ws_n:
+            nb = lib.rgcn_rotate_rank_workspace_bytes(V, d, n)
+            if nb < 0:
+                _lib.check(int(nb), "rgcn_rotate_rank_workspace_bytes")
+            self._ws, self._ws_n = _workspace(nb, dev), n
+        raw = torch.empty(n, dtype=torch.int32, device=dev)
+        filt = torch.empty(n, dtype=torch.int32, device=dev) if known_mask is not None else None
+        rc = lib.rgcn_rotate_rank(_ptr(self.codes), _ptr(self.rel), V, self.rel.shape[0], d, _ptr(X), n, int(side),
+                                  _ptr(known_mask), _ptr(raw), _ptr(filt), _ptr(self._ws), self._ws.numel(),
+                                  _stream(dev))
+        _lib.check(rc, "rgcn_rotate_rank")
+        return raw, filt
+
+    def top_k(self, X, side, k, exclude_mask=None):
+        raise NotImplementedError("the RotatE decoder has no top-k entity prediction")
+
+    def rank_relations(self, X, known_mask=None):
+        raise NotImplementedError("the RotatE decoder has no relation prediction")
+
+    def top_k_relations(self, X, k, exclude_mask=None):
+        raise NotImplementedError("the RotatE decoder has no relation prediction")
 
 
 class EnsembleRanker(object):

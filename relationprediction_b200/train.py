@@ -19,6 +19,7 @@ import numpy as np
 
 from .optim import ClippedAdam
 from .common import auxilliaries, evaluation, io, model_builder, settings_reader
+from .decoders.rotate import Rotate
 
 
 def load_dataset(dataset):
@@ -234,7 +235,7 @@ def main(argv=None):
     ap.add_argument("--relation-metrics", action="store_true",
                     help="also rank every test triple's relation among all relations for its (head, tail) pair and "
                          "report Raw / Filtered MRR and H@1/3/10 for relation prediction after the entity metrics "
-                         "(DistMult and ComplEx decoders on CUDA)")
+                         "(DistMult and ComplEx decoders on CUDA; refused for RotatE)")
     ap.add_argument("--set", action="append", default=[], metavar="Section.Key=Value",
                     help="override one settings entry after the file is read, e.g. "
                          "--set Encoder.NumberOfBasisFunctions=2 (repeatable)")
@@ -285,6 +286,8 @@ def main(argv=None):
     train, valid, test = splits['train'], splits['valid'], splits['test']
     encoder, model, scorer = build_chain(settings, splits, len(entities), len(relations), args.device)
     general, opt = settings['General'], settings['Optimizer']
+    if args.relation_metrics and isinstance(model, Rotate):
+        raise SystemExit("--relation-metrics: the RotatE decoder has no relation prediction")
 
     ns = auxilliaries.NegativeSampler(int(general['NegativeSampleRate']), len(entities))
     adj_list = [[] for _ in entities]
