@@ -792,6 +792,75 @@ int rgcn_rotate_rank(const float* codes, const float* rel, int32_t V, int32_t Vr
                      int64_t n, int side, const uint32_t* known_mask, int32_t* raw_rank, int32_t* filtered_rank,
                      void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- ConvE decoder (DESIGN.md section 1): query rows q = f(anchor row, relation row), energy <q, codes[v]> ----
+ * A query (anchor a, relation r, side) reads codes[a] and rel[r] (side 1, object query (a, r, ?)) or rel_inv[r]
+ * (side 0, subject query (?, r, a), the reciprocal relation).  f: the two rows reshaped to h x w (d = h w) and stacked into a
+ * 2h x w image (anchor on top); input dropout; C valid 3x3 filters + bias; ReLU; feature dropout (one bit per query and
+ * filter); flattened channel-major to F = C (2h - 2)(w - 2) features; q = ReLU(hidden dropout(features W_fc + b_fc)).
+ * Masks are uint8 keep-masks of the queries of the call (row t = query t), scaled by 1 / keep; NULL = no dropout.
+ * Every entry checks its arguments before any device work: d % 4 == 0, h >= 2, d % h == 0, w = d / h >= 3, C >= 1,
+ * every keep in (0, 1], non-null weights, ids and sides (host queries), the workspace size; RGCN_ERR_INVALID /
+ * RGCN_ERR_WORKSPACE / RGCN_ERR_NODEVICE as the 1-N entry points. */
+typedef struct {
+  int32_t h;                   /* image height of one row: d = h w */
+  int32_t C;                   /* filters */
+  const float* rel_inv;        /* [R, d] reciprocal relation rows */
+  const float* filters;        /* [C, 3, 3] */
+  const float* conv_bias;      /* [C] */
+  const float* W_fc;           /* [F, d] */
+  const float* b_fc;           /* [d] */
+  const uint8_t* input_mask;   /* [n, 2d] or NULL */
+  const uint8_t* feature_mask; /* [n, C] or NULL */
+  const uint8_t* hidden_mask;  /* [n, d] or NULL */
+  float input_keep, feature_keep, hidden_keep;
+} rgcn_conve_net_t;
+
+/* gradients of the decoder's own weights, shapes as in rgcn_conve_net_t */
+typedef struct {
+  float* rel_inv;
+  float* filters;
+  float* conv_bias;
+  float* W_fc;
+  float* b_fc;
+} rgcn_conve_grads_t;
+
+/* rgcn_conve_one_to_n: the 1-N loss of distmult_one_to_n with ConvE query rows (host queries (anchor, r, side), the
+ * same label bits, smoothing and chunking; loss[1] the L2 term of the anchor row and rel[r] or rel_inv[r]).  With
+ * dcodes non-NULL, dcodes / drel [Vrel, d] and the five gradients of `grads` are written (g_scale as there); the
+ * gradients of the network weights and of the loss are summed in a fixed order, so they and the loss are bitwise
+ * repeatable.  rgcn_conve_one_to_n_finish: the backward of a call made with g_scale = (1, 0), as rgcn_one_to_n_finish,
+ * for all seven gradients. */
+int64_t rgcn_conve_one_to_n_workspace_bytes(int32_t V, int32_t R, int32_t d, int32_t h, int32_t C, int64_t n,
+                                            int64_t chunk);
+int rgcn_conve_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                        const rgcn_conve_net_t* net, const int32_t* queries, int64_t n, const uint32_t* labels,
+                        float smoothing, const float* g_scale, float* loss, float* dcodes, float* drel,
+                        const rgcn_conve_grads_t* grads, int64_t chunk, void* workspace, int64_t workspace_bytes,
+                        void* stream);
+int64_t rgcn_conve_one_to_n_finish_workspace_bytes(int64_t n);
+int rgcn_conve_one_to_n_finish(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                               const rgcn_conve_net_t* net, const int32_t* queries, int64_t n, const float* g_scale,
+                               const float* dcodes_loss, const float* drel_loss, const rgcn_conve_grads_t* loss_grads,
+                               float* dcodes, float* drel, const rgcn_conve_grads_t* grads, void* workspace,
+                               int64_t workspace_bytes, void* stream);
+/* rgcn_conve_query_rows: Q [n, d] of the device triples X [n, 3]: side 1 q = f(codes[s], rel[r]), side 0
+ * q = f(codes[o], rel_inv[r]).  rgcn_conve_rank / rgcn_conve_topk: distmult_rank / distmult_topk over these rows (the
+ * same workspace head, so the split of `codes` is reused as there); relation ids must be below R. */
+int64_t rgcn_conve_query_rows_workspace_bytes(int32_t d, int32_t h, int32_t C, int64_t n);
+int rgcn_conve_query_rows(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                          const rgcn_conve_net_t* net, const int32_t* X, int64_t n, int side, float* Q,
+                          void* workspace, int64_t workspace_bytes, void* stream);
+int64_t rgcn_conve_rank_workspace_bytes(int32_t V, int32_t d, int32_t h, int32_t C, int64_t n);
+int rgcn_conve_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                    const rgcn_conve_net_t* net, const int32_t* X, int64_t n, int side, const uint32_t* known_mask,
+                    int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+int64_t rgcn_conve_topk_workspace_bytes(int32_t V, int32_t d, int32_t h, int32_t C, int64_t n, int32_t k);
+int rgcn_conve_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                    const rgcn_conve_net_t* net, const int32_t* X, int64_t n, int side, int32_t k,
+                    const uint32_t* exclude_mask, int reuse_split, int32_t* ids, float* energies, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -41,6 +41,9 @@ EXPORTED_SYMBOLS = [
     "rgcn_self_adversarial_workspace_bytes", "rgcn_self_adversarial_forward",
     "rgcn_rotate_forward", "rgcn_rotate_backward", "rgcn_rotate_self_adversarial_forward",
     "rgcn_rotate_rank_workspace_bytes", "rgcn_rotate_rank",
+    "rgcn_conve_one_to_n_workspace_bytes", "rgcn_conve_one_to_n", "rgcn_conve_one_to_n_finish_workspace_bytes",
+    "rgcn_conve_one_to_n_finish", "rgcn_conve_query_rows_workspace_bytes", "rgcn_conve_query_rows",
+    "rgcn_conve_rank_workspace_bytes", "rgcn_conve_rank", "rgcn_conve_topk_workspace_bytes", "rgcn_conve_topk",
 ]
 
 RGCN_DECODER_DISTMULT, RGCN_DECODER_COMPLEX = 0, 1
@@ -56,6 +59,20 @@ _lib = None
 
 class RgcnError(RuntimeError):
     pass
+
+
+class ConvENet(ctypes.Structure):
+    """rgcn_conve_net_t: the ConvE query network's shape, weights (device pointers) and dropout masks."""
+    _fields_ = [("h", c_int32), ("C", c_int32), ("rel_inv", c_void_p), ("filters", c_void_p),
+                ("conv_bias", c_void_p), ("W_fc", c_void_p), ("b_fc", c_void_p), ("input_mask", c_void_p),
+                ("feature_mask", c_void_p), ("hidden_mask", c_void_p), ("input_keep", c_float),
+                ("feature_keep", c_float), ("hidden_keep", c_float)]
+
+
+class ConvEGrads(ctypes.Structure):
+    """rgcn_conve_grads_t: the gradients of the ConvE decoder's own weights (device pointers)."""
+    _fields_ = [("rel_inv", c_void_p), ("filters", c_void_p), ("conv_bias", c_void_p), ("W_fc", c_void_p),
+                ("b_fc", c_void_p)]
 
 
 def _declare(lib):
@@ -275,6 +292,32 @@ def _declare(lib):
     lib.rgcn_rotate_rank.restype = c_int
     lib.rgcn_rotate_rank.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, vp, vp, vp, vp, c_int64,
                                      vp]
+    net, grads = POINTER(ConvENet), POINTER(ConvEGrads)
+    lib.rgcn_conve_one_to_n_workspace_bytes.restype = c_int64
+    lib.rgcn_conve_one_to_n_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_int64, c_int64]
+    lib.rgcn_conve_one_to_n.restype = c_int
+    lib.rgcn_conve_one_to_n.argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, net, vp, c_int64, vp, c_float, vp,
+                                        vp, vp, vp, grads, c_int64, vp, c_int64, vp]
+    lib.rgcn_conve_one_to_n_finish_workspace_bytes.restype = c_int64
+    lib.rgcn_conve_one_to_n_finish_workspace_bytes.argtypes = [c_int64]
+    lib.rgcn_conve_one_to_n_finish.restype = c_int
+    lib.rgcn_conve_one_to_n_finish.argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, net, vp, c_int64, vp, vp,
+                                               vp, grads, vp, vp, grads, vp, c_int64, vp]
+    lib.rgcn_conve_query_rows_workspace_bytes.restype = c_int64
+    lib.rgcn_conve_query_rows_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int64]
+    lib.rgcn_conve_query_rows.restype = c_int
+    lib.rgcn_conve_query_rows.argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, net, vp, c_int64, c_int, vp, vp,
+                                          c_int64, vp]
+    lib.rgcn_conve_rank_workspace_bytes.restype = c_int64
+    lib.rgcn_conve_rank_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int64]
+    lib.rgcn_conve_rank.restype = c_int
+    lib.rgcn_conve_rank.argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, net, vp, c_int64, c_int, vp, c_int, vp,
+                                    vp, vp, c_int64, vp]
+    lib.rgcn_conve_topk_workspace_bytes.restype = c_int64
+    lib.rgcn_conve_topk_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int64, c_int32]
+    lib.rgcn_conve_topk.restype = c_int
+    lib.rgcn_conve_topk.argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, net, vp, c_int64, c_int, c_int32, vp,
+                                    c_int, vp, vp, vp, c_int64, vp]
 
 
 def load():

@@ -5,10 +5,11 @@ when Concatenation=Yes, BasisGcnTimesDiag when DiagonalCoefficients=Yes; with Us
 BasisGcn; SkipConnections=Highway wraps every
 feature-input layer in a HighwayLayer), `embedding`, and the variational encoders `variational_embedding` and
 `variational_gcn_basis` (a VariationalEncoding over two linear AffineTransform heads); decoders `bilinear-diag`, `complex` and
-`rotate` (RotatE, which the reference does not have).  Unknown names return None exactly
+`rotate` (RotatE, which the reference does not have) and `conve` (ConvE, 1-N training only).  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag, parse_training_objective
 from ..decoders.complex import Complex
+from ..decoders.conve import ConvE
 from ..decoders.rotate import Rotate
 from ..encoders.affine_transform import AffineTransform
 from ..encoders.message_gcns.gcn_basis import BasisGcn
@@ -165,6 +166,12 @@ def apply_basis_gcn(encoder_settings, encoding, internal_shape, layers):
 
 
 def build_decoder(encoder, decoder_settings):
+    if decoder_settings['Name'] == "conve":
+        # ConvE scores every entity per query: 1-N is its only objective
+        objective = parse_training_objective(decoder_settings)[0]
+        if objective != '1-N':
+            raise ValueError("the conve decoder trains under TrainingObjective=1-N only, not %r" % objective)
+        return ConvE(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
     if decoder_settings['Name'] not in ("bilinear-diag", "complex"):
         objective = parse_training_objective(decoder_settings)[0]
         # RotatE trains under SelfAdversarial (the objective of its paper) but has no 1-N scoring GEMM

@@ -7,10 +7,12 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
 #include "kernels.cuh"
+#include "rgcn_b200.h"
 
 namespace {
 
@@ -1342,9 +1344,13 @@ extern "C" int rgcn_block_slice_sumsq(const rgcn_graph_t* g, int32_t d, int32_t 
 // Workspace layout: [hi N*d | lo N*d | Q n*d | gold_sig n | gold_col n | raw_cnt n | known_cnt n].
 typedef int (*RankPrepareFn)(const float*, const float*, int, const int32_t*, int64_t, int, float*, float*, int32_t*,
                              cudaStream_t);
+// the prepare step of the rank and top-k bodies: a RankPrepareFn, or a callable that owns more state (ConvE's network)
+typedef std::function<int(const float*, const float*, int, const int32_t*, int64_t, int, float*, float*, int32_t*,
+                          cudaStream_t)>
+    RankPrepare;
 typedef int64_t (*RankWorkspaceFn)(int32_t, int32_t, int64_t);
 
-static int rank_with_queries(const char* who, RankPrepareFn prepare, const float* table, int32_t N,
+static int rank_with_queries(const char* who, const RankPrepare& prepare, const float* table, int32_t N,
                              RankWorkspaceFn workspace_fn, const float* codes, const float* rel, int32_t V,
                              int32_t Vrel, int32_t d, const int32_t* X, int64_t n, int side,
                              const uint32_t* known_mask, int reuse_split, int32_t* raw_rank, int32_t* filtered_rank,
@@ -1605,7 +1611,7 @@ extern "C" int64_t rgcn_topk_workspace_bytes(int32_t V, int32_t d, int64_t n, in
 // The candidates are the first N rows of `table`, as in rank_with_queries.
 typedef int64_t (*TopkWorkspaceFn)(int32_t, int32_t, int64_t, int32_t);
 
-static int topk_with_queries(const char* who, RankPrepareFn prepare, const float* table, int32_t N,
+static int topk_with_queries(const char* who, const RankPrepare& prepare, const float* table, int32_t N,
                              TopkWorkspaceFn workspace_fn, const float* codes, const float* rel, int32_t V,
                              int32_t Vrel, int32_t d, const int32_t* X, int64_t n, int side, int32_t k,
                              const uint32_t* exclude_mask, int reuse_split, int32_t* ids, float* energies,
@@ -1983,10 +1989,48 @@ extern "C" int64_t rgcn_one_to_n_workspace_bytes(int32_t V, int32_t d, int64_t n
          align_up((int64_t)V * cp * 4) + 256;
 }
 
-static int one_to_n(const char* who, int complex, const float* codes, const float* rel, int32_t V, int32_t Vrel,
-                    int32_t R, int32_t d, const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
-                    const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk, void* workspace,
-                    int64_t workspace_bytes, cudaStream_t st) {
+// The decoder's two per-chunk steps: prepare writes the query rows Q [c1 - c0, d] of queries c0 .. c1 - 1, query_bwd
+// turns their dQ and the L2 term (c_reg) into the row gradients.  X holds the uploaded queries, runs their side runs.
+struct OnenChunk {
+  const int32_t* X;
+  const std::vector<OnenRun>* runs;
+  int64_t c0, c1;
+  float c_reg;
+  const float* Q;   // the chunk's query rows, as prepare wrote them
+};
+typedef std::function<int(const OnenChunk&, float*)> OnenStep;
+
+// DistMult and ComplEx: the rank prepare and query-backward kernels, one launch per side run in the chunk
+static void onen_row_steps(int complex, const float* codes, const float* rel, int d, const float* g_scale,
+                           float* dcodes, float* drel, cudaStream_t st, OnenStep* prepare, OnenStep* query_bwd) {
+  const RankPrepareFn prep = complex ? launch_complex_rank_prepare : launch_distmult_rank_prepare;
+  *prepare = [=](const OnenChunk& k, float* Q) {
+    int rc = RGCN_OK;
+    for (const OnenRun& run : *k.runs) {
+      const int64_t b = std::max(run.begin, k.c0), e = std::min(run.end, k.c1);
+      if (b < e) rc = prep(codes, rel, d, k.X + 3 * b, e - b, run.side, Q + (b - k.c0) * d, nullptr, nullptr, st);
+      if (rc) return rc;
+    }
+    return rc;
+  };
+  *query_bwd = [=](const OnenChunk& k, float* dQ) {
+    int rc = RGCN_OK;
+    for (const OnenRun& run : *k.runs) {
+      const int64_t b = std::max(run.begin, k.c0), e = std::min(run.end, k.c1);
+      if (!rc && b < e)
+        rc = launch_onen_query_bwd(complex, codes, rel, d, k.X + 3 * b, e - b, run.side, dQ + (b - k.c0) * d, g_scale,
+                                   k.c_reg, dcodes, drel, st);
+    }
+    return rc;
+  };
+}
+
+// repeatable: the dQ GEMM runs without split-K, so dQ and what query_bwd derives from it are bitwise repeatable
+static int one_to_n(const char* who, const OnenStep& prepare, const OnenStep& query_bwd, bool repeatable,
+                    const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                    const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing, const float* g_scale,
+                    float* loss, float* dcodes, float* drel, int64_t chunk, void* workspace, int64_t workspace_bytes,
+                    cudaStream_t st) {
   if (!codes || !rel || !loss || !workspace || (n > 0 && (!queries || !labels)) || (!dcodes != !drel)) {
     rgcn_set_error(std::string(who) + ": null pointer (dcodes and drel are both given or both NULL)");
     return RGCN_ERR_INVALID;
@@ -2030,7 +2074,6 @@ static int one_to_n(const char* who, int complex, const float* codes, const floa
   float* qt_hi = ws.take<float>((int64_t)d * cp);
   float* qt_lo = ws.take<float>((int64_t)d * cp);
   float* Gt = ws.take<float>((int64_t)V * cp);
-  const RankPrepareFn prepare = complex ? launch_complex_rank_prepare : launch_distmult_rank_prepare;
   const float pos = (float)((1.0 - smoothing) + (double)smoothing / V), neg = (float)((double)smoothing / V);
   const float scale = (float)(1.0 / ((double)n * V));
   const float c_reg = (float)(2.0 / ((double)n * d));
@@ -2045,11 +2088,9 @@ static int one_to_n(const char* who, int complex, const float* codes, const floa
   int64_t part = 0;
   for (int64_t c0 = 0; c0 < n; c0 += c) {
     const int64_t c1 = std::min(n, c0 + c), m = c1 - c0, mp = (m + 7) / 8 * 8;
-    for (const OnenRun& run : runs) {
-      const int64_t b = std::max(run.begin, c0), e = std::min(run.end, c1);
-      if (b < e) rc = prepare(codes, rel, d, X + 3 * b, e - b, run.side, Q + (b - c0) * d, nullptr, nullptr, st);
-      if (rc) return rc;
-    }
+    const OnenChunk k{X, &runs, c0, c1, c_reg, Q};
+    rc = prepare(k, Q);
+    if (rc) return rc;
     rc = launch_gemm_onen_tf32x3(Q, d, hi, lo, d, (int)m, V, d, labels + c0 * words, pos, neg, scale, g_scale,
                                  grads ? Gt : nullptr, mp, loss_part + part, st);
     if (rc) return rc;
@@ -2063,17 +2104,12 @@ static int one_to_n(const char* who, int complex, const float* codes, const floa
                              "memset(Gt pad)");
       if (rc) return rc;
     }
-    rc = launch_gemm_tn_tf32x3(Gt, mp, codes, d, dQ, d, (int)mp, d, V, /*accumulate=*/0, st);
+    rc = launch_gemm_tn_tf32x3(Gt, mp, codes, d, dQ, d, (int)mp, d, V, /*accumulate=*/0, st, repeatable ? 1 : 0);
     MARK("onen_dQ_gemm");
     if (!rc) rc = launch_gemm_split_b(Q, d, d, (int)mp, /*transposed=*/1, qt_hi, qt_lo, st);
     if (!rc) rc = launch_gemm_tf32x3(Gt, mp, qt_hi, qt_lo, mp, dcodes, d, V, d, (int)mp, c0 > 0, st);
     MARK("onen_dcodes_gemm");
-    for (const OnenRun& run : runs) {
-      const int64_t b = std::max(run.begin, c0), e = std::min(run.end, c1);
-      if (!rc && b < e)
-        rc = launch_onen_query_bwd(complex, codes, rel, d, X + 3 * b, e - b, run.side, dQ + (b - c0) * d, g_scale,
-                                   c_reg, dcodes, drel, st);
-    }
+    if (!rc) rc = query_bwd(k, dQ);
     if (rc) return rc;
     MARK("onen_query_bwd");
   }
@@ -2085,16 +2121,20 @@ extern "C" int distmult_one_to_n(const float* codes, const float* rel, int32_t V
                                  const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
                                  const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk,
                                  void* workspace, int64_t workspace_bytes, void* stream) {
-  return one_to_n("distmult_one_to_n", 0, codes, rel, V, Vrel, R, d, queries, n, labels, smoothing, g_scale, loss,
-                  dcodes, drel, chunk, workspace, workspace_bytes, (cudaStream_t)stream);
+  OnenStep prepare, query_bwd;
+  onen_row_steps(0, codes, rel, d, g_scale, dcodes, drel, (cudaStream_t)stream, &prepare, &query_bwd);
+  return one_to_n("distmult_one_to_n", prepare, query_bwd, false, codes, rel, V, Vrel, R, d, queries, n, labels,
+                  smoothing, g_scale, loss, dcodes, drel, chunk, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int rgcn_complex_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
                                      int32_t d, const int32_t* queries, int64_t n, const uint32_t* labels,
                                      float smoothing, const float* g_scale, float* loss, float* dcodes, float* drel,
                                      int64_t chunk, void* workspace, int64_t workspace_bytes, void* stream) {
-  return one_to_n("rgcn_complex_one_to_n", 1, codes, rel, V, Vrel, R, d, queries, n, labels, smoothing, g_scale, loss,
-                  dcodes, drel, chunk, workspace, workspace_bytes, (cudaStream_t)stream);
+  OnenStep prepare, query_bwd;
+  onen_row_steps(1, codes, rel, d, g_scale, dcodes, drel, (cudaStream_t)stream, &prepare, &query_bwd);
+  return one_to_n("rgcn_complex_one_to_n", prepare, query_bwd, false, codes, rel, V, Vrel, R, d, queries, n, labels,
+                  smoothing, g_scale, loss, dcodes, drel, chunk, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 // The backward of a call made with g_scale = (1, 0): its dcodes / drel are the loss's gradient alone, so the gradient
@@ -2184,6 +2224,410 @@ extern "C" int rgcn_one_to_n_labels(const int64_t* keys, const int64_t* offsets,
                               words, bits + run.begin * words, st);
   }
   return rc;
+}
+
+// ------------------------------------------------------------------------------------------------
+// ConvE (conve.cu): the query network in front of the 1-N, rank and top-k bodies above
+// ------------------------------------------------------------------------------------------------
+// Evaluation queries run through the network in passes of this many rows (the feature rows of a pass are F floats
+// each, about 112 KB at d = 500, h = 20, C = 32)
+constexpr int64_t CONVE_EVAL_CHUNK = 1024;
+
+static int64_t conve_F(int32_t d, int32_t h, int32_t C) { return (int64_t)C * (2 * h - 2) * (d / h - 2); }
+static int64_t conve_Fp(int32_t d, int32_t h, int32_t C) { return (conve_F(d, h, C) + 3) / 4 * 4; }
+
+static bool conve_shape_ok(int32_t d, int32_t h, int32_t C) {
+  return d > 0 && d % 4 == 0 && h >= 2 && d % h == 0 && d / h >= 3 && C >= 1 && conve_F(d, h, C) < (1LL << 30) &&
+         conve_smem_bytes(d, h, d / h, C) <= 227 * 1024;
+}
+
+static int conve_net_checks(const char* who, int32_t d, const rgcn_conve_net_t* net) {
+  const std::string w(who);
+  if (!net || !net->rel_inv || !net->filters || !net->conv_bias || !net->W_fc || !net->b_fc) {
+    rgcn_set_error(w + ": null pointer in the network (rel_inv, filters, conv_bias, W_fc, b_fc)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!conve_shape_ok(d, net->h, net->C)) {
+    rgcn_set_error(w + ": bad shape (need d % 4 == 0, h >= 2, d = h w with w >= 3, C >= 1)");
+    return RGCN_ERR_INVALID;
+  }
+  for (float k : {net->input_keep, net->feature_keep, net->hidden_keep}) {
+    if (!(k > 0.f && k <= 1.f)) {   // also refuses NaN
+      rgcn_set_error(w + ": keep probabilities must be in (0, 1]");
+      return RGCN_ERR_INVALID;
+    }
+  }
+  return RGCN_OK;
+}
+
+// The network's workspace for passes of up to c queries (cp = c rounded up to 8): the splits of W_fc for the forward
+// ([d, Fp]) and the backward ([Fp, d]), the feature rows [cp, Fp]; with grads, the split of the feature rows'
+// transpose [Fp, cp] (whose hi plane then holds dF [cp, Fp]), dZ [cp, d], dZt [d, cp], dWt [d, Fp] and the filter
+// parts.
+struct ConvEWork {
+  float *wt_hi, *wt_lo, *w_hi, *w_lo, *feat, *ft_hi, *ft_lo, *dz, *dzt, *dwt, *part;
+};
+
+static int64_t conve_work_bytes(int32_t d, int32_t h, int32_t C, int64_t c, bool grads) {
+  const int64_t Fp = conve_Fp(d, h, C), cp = (std::max<int64_t>(c, 1) + 7) / 8 * 8;
+  int64_t b = 2 * align_up(d * Fp * 4) + align_up(cp * Fp * 4);
+  if (grads)
+    b += 2 * align_up(Fp * d * 4) + 2 * align_up(Fp * cp * 4) + 2 * align_up(cp * d * 4) + align_up(d * Fp * 4) +
+         align_up(conve_conv_parts(cp) * 10 * C * 4);
+  return b;
+}
+
+static ConvEWork conve_carve(Carver& ws, int32_t d, int32_t h, int32_t C, int64_t c, bool grads) {
+  const int64_t Fp = conve_Fp(d, h, C), cp = (std::max<int64_t>(c, 1) + 7) / 8 * 8;
+  ConvEWork w{};
+  w.wt_hi = ws.take<float>(d * Fp);
+  w.wt_lo = ws.take<float>(d * Fp);
+  w.feat = ws.take<float>(cp * Fp);
+  if (grads) {
+    w.w_hi = ws.take<float>(Fp * d);
+    w.w_lo = ws.take<float>(Fp * d);
+    w.ft_hi = ws.take<float>(Fp * cp);
+    w.ft_lo = ws.take<float>(Fp * cp);
+    w.dz = ws.take<float>(cp * d);
+    w.dzt = ws.take<float>(d * cp);
+    w.dwt = ws.take<float>(d * Fp);
+    w.part = ws.take<float>(conve_conv_parts(cp) * 10 * C);
+  }
+  return w;
+}
+
+static const uint8_t* mask_rows(const uint8_t* m, int64_t row0, int64_t width) {
+  return m ? m + row0 * width : nullptr;
+}
+
+// Q [m, d] of the queries X[0 .. m) (anchor in column acol, relation row reltab[X[t][1]], mask rows from row0); the
+// feature rows stay in w.feat for the backward.  The forward split of W_fc must be in w.wt_hi / w.wt_lo.
+static int conve_forward(const float* codes, const float* reltab, int32_t d, const rgcn_conve_net_t* net,
+                         const int32_t* X, int acol, int64_t m, int64_t row0, const ConvEWork& w, float* Q,
+                         cudaStream_t st) {
+  const int Fp = (int)conve_Fp(d, net->h, net->C);
+  int rc = launch_conve_conv_fwd(codes, reltab, d, net->h, net->C, X, acol, m, net->filters, net->conv_bias,
+                                 mask_rows(net->input_mask, row0, 2 * d), 1.f / net->input_keep,
+                                 mask_rows(net->feature_mask, row0, net->C), 1.f / net->feature_keep, Fp, w.feat, st);
+  if (!rc) rc = launch_gemm_tf32x3(w.feat, Fp, w.wt_hi, w.wt_lo, Fp, Q, d, (int)m, d, Fp, /*accumulate=*/0, st);
+  if (!rc)
+    rc = launch_conve_fc_act(Q, m, d, net->b_fc, mask_rows(net->hidden_mask, row0, d), 1.f / net->hidden_keep, st);
+  return rc;
+}
+
+// The evaluation prepare: the forward split of W_fc, then Q of the n triples X of one side in passes of
+// CONVE_EVAL_CHUNK, and (gold_sig non-null) the gold scores
+static RankPrepare conve_prepare(const rgcn_conve_net_t* net, const ConvEWork& w) {
+  return [net, w](const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side, float* Q,
+                  float* gold_sig, int32_t* gold_col, cudaStream_t st) {
+    const int F = (int)conve_F(d, net->h, net->C), Fp = (int)conve_Fp(d, net->h, net->C);
+    int rc = launch_conve_split_w(net->W_fc, F, d, Fp, /*transposed=*/1, w.wt_hi, w.wt_lo, st);
+    const float* reltab = side == 0 ? net->rel_inv : rel;
+    for (int64_t c0 = 0; !rc && c0 < n; c0 += CONVE_EVAL_CHUNK) {
+      const int64_t m = std::min(CONVE_EVAL_CHUNK, n - c0);
+      rc = conve_forward(codes, reltab, d, net, X + 3 * c0, side == 0 ? 2 : 0, m, c0, w, Q + c0 * d, st);
+    }
+    if (!rc && gold_sig) rc = launch_conve_gold(Q, codes, d, X, n, side, gold_sig, gold_col, st);
+    return rc;
+  };
+}
+
+extern "C" int64_t rgcn_conve_one_to_n_workspace_bytes(int32_t V, int32_t R, int32_t d, int32_t h, int32_t C,
+                                                       int64_t n, int64_t chunk) {
+  if (R < 1 || !conve_shape_ok(d, h, C) || V <= 0 || n < 0 || n > 0x7fffffffLL || chunk < 1) {
+    rgcn_set_error("rgcn_conve_one_to_n_workspace_bytes: bad arguments (need V > 0, R > 0, a valid ConvE shape, "
+                   "0 <= n < 2^31, chunk >= 1)");
+    return RGCN_ERR_INVALID;
+  }
+  // [1-N body | relation rows [rel ; rel_inv] and their gradient | network]
+  return rgcn_one_to_n_workspace_bytes(V, d, n, chunk) + 2 * align_up((int64_t)2 * R * d * 4) +
+         conve_work_bytes(d, h, C, onen_chunk(n, chunk), true) + 256;
+}
+
+static bool conve_grads_ok(const rgcn_conve_grads_t* g) {
+  return g && g->rel_inv && g->filters && g->conv_bias && g->W_fc && g->b_fc;
+}
+
+// The 1-N body with the relation table [rel[0:R] ; rel_inv] (2R rows): a subject query (a, r, 0) reads row R + r, so
+// the body's L2 term and the network's image gradient need no side; drel and grads->rel_inv are split from its
+// gradient afterwards.
+extern "C" int rgcn_conve_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                                   const rgcn_conve_net_t* net, const int32_t* queries, int64_t n,
+                                   const uint32_t* labels, float smoothing, const float* g_scale, float* loss,
+                                   float* dcodes, float* drel, const rgcn_conve_grads_t* grads, int64_t chunk,
+                                   void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_conve_one_to_n";
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!codes || !rel || !loss || !workspace || (n > 0 && (!queries || !labels)) || (!dcodes != !drel) ||
+      (dcodes && !conve_grads_ok(grads))) {
+    rgcn_set_error(std::string(who) + ": null pointer (dcodes, drel and the five network gradients are all given or "
+                   "dcodes and drel are both NULL)");
+    return RGCN_ERR_INVALID;
+  }
+  int rc = conve_net_checks(who, d, net);
+  if (rc) return rc;
+  if (V <= 0 || Vrel <= 0 || R < 1 || R > Vrel || n < 0 || n > 0x7fffffffLL || chunk < 1) {
+    rgcn_set_error(std::string(who) + ": bad sizes (need V > 0, 1 <= R <= Vrel, 0 <= n < 2^31, chunk >= 1)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!(smoothing >= 0.f && smoothing < 1.f)) {
+    rgcn_set_error(std::string(who) + ": label smoothing must be in [0, 1)");
+    return RGCN_ERR_INVALID;
+  }
+  std::vector<OnenRun> runs;
+  rc = onen_query_checks(who, queries, n, V, R, &runs);
+  if (rc) return rc;
+  const int64_t body = rgcn_one_to_n_workspace_bytes(V, d, n, chunk);
+  if (body < 0 || workspace_bytes < rgcn_conve_one_to_n_workspace_bytes(V, R, d, net->h, net->C, n, chunk)) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_conve_one_to_n_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who);
+  if (rc) return rc;
+
+  const bool grads_on = dcodes != nullptr;
+  const int h = net->h, C = net->C, F = (int)conve_F(d, h, C), Fp = (int)conve_Fp(d, h, C);
+  if (n == 0) {   // no queries: zero loss and gradients
+    rc = rgcn_check_cuda(cudaMemsetAsync(loss, 0, 2 * sizeof(float), st), "memset(loss)");
+    if (grads_on) {
+      const std::pair<float*, int64_t> zero[] = {{dcodes, (int64_t)V * d}, {drel, (int64_t)Vrel * d},
+                                                 {grads->rel_inv, (int64_t)R * d}, {grads->filters, 9LL * C},
+                                                 {grads->conv_bias, C}, {grads->W_fc, (int64_t)F * d},
+                                                 {grads->b_fc, d}};
+      for (const auto& z : zero)
+        if (!rc) rc = rgcn_check_cuda(cudaMemsetAsync(z.first, 0, (size_t)z.second * 4, st), "memset(gradient)");
+    }
+    return rc;
+  }
+  Carver ws((char*)workspace + body, workspace_bytes - body);
+  float* relcat = ws.take<float>((int64_t)2 * R * d);
+  float* drelcat = ws.take<float>((int64_t)2 * R * d);
+  const ConvEWork w = conve_carve(ws, d, h, C, onen_chunk(n, chunk), grads_on);
+  std::vector<int32_t> q2(queries, queries + 3 * n);
+  for (int64_t t = 0; t < n; ++t)
+    if (q2[3 * t + 2] == 0) q2[3 * t + 1] += R;
+
+  rc = rgcn_check_cuda(cudaMemcpyAsync(relcat, rel, (size_t)R * d * 4, cudaMemcpyDeviceToDevice, st), "copy(rel)");
+  if (!rc)
+    rc = rgcn_check_cuda(cudaMemcpyAsync(relcat + (size_t)R * d, net->rel_inv, (size_t)R * d * 4,
+                                         cudaMemcpyDeviceToDevice, st), "copy(rel_inv)");
+  if (!rc) rc = launch_conve_split_w(net->W_fc, F, d, Fp, /*transposed=*/1, w.wt_hi, w.wt_lo, st);
+  if (!rc && grads_on) rc = launch_conve_split_w(net->W_fc, F, d, Fp, /*transposed=*/0, w.w_hi, w.w_lo, st);
+  if (rc) return rc;
+
+  const OnenStep prepare = [=](const OnenChunk& k, float* Q) {
+    return conve_forward(codes, relcat, d, net, k.X + 3 * k.c0, 0, k.c1 - k.c0, k.c0, w, Q, st);
+  };
+  // dZ through the ReLU and the hidden mask; db_fc, dW_fc^T (+)= dZ^T Feat, dF = dZ W_fc^T, the convolution backward;
+  // then the L2 term of the two gathered rows
+  const OnenStep query_bwd = [=](const OnenChunk& k, float* dQ) {
+    const int64_t c0 = k.c0, m = k.c1 - c0, mp = (m + 7) / 8 * 8;
+    const int acc = c0 > 0;   // the network gradients accumulate over the chunks
+    int rc = launch_conve_dz(k.Q, dQ, m, d, mask_rows(net->hidden_mask, c0, d), 1.f / net->hidden_keep, w.dz, w.dzt,
+                             mp, st);
+    if (!rc) rc = launch_conve_rowsum(w.dzt, d, m, mp, grads->b_fc, acc, st);
+    if (!rc && mp > m)   // the K padding of the dW GEMM: zero feature rows, zero columns of dZt
+      rc = rgcn_check_cuda(cudaMemsetAsync(w.feat + m * Fp, 0, (size_t)(mp - m) * Fp * 4, st), "memset(Feat pad)");
+    if (!rc) rc = launch_gemm_split_b(w.feat, Fp, Fp, (int)mp, /*transposed=*/1, w.ft_hi, w.ft_lo, st);
+    if (!rc) rc = launch_gemm_tf32x3(w.dzt, mp, w.ft_hi, w.ft_lo, mp, w.dwt, Fp, d, Fp, (int)mp, acc, st);
+    float* dF = w.ft_hi;   // the split of Feat^T is consumed
+    if (!rc) rc = launch_gemm_tf32x3(w.dz, d, w.w_hi, w.w_lo, d, dF, Fp, (int)m, Fp, d, /*accumulate=*/0, st);
+    if (!rc)
+      rc = launch_conve_conv_bwd(codes, relcat, d, h, C, k.X + 3 * c0, m, net->filters,
+                                 mask_rows(net->input_mask, c0, 2 * d), 1.f / net->input_keep, w.feat, dF,
+                                 1.f / net->feature_keep, Fp, w.part, dcodes, drelcat, st);
+    if (!rc)
+      rc = launch_conve_filter_reduce(w.part, (int)conve_conv_parts(m), C, grads->filters, grads->conv_bias, acc,
+                                      st);
+    if (!rc)
+      rc = launch_onen_query_bwd(0, codes, relcat, d, k.X + 3 * c0, m, 1, nullptr, g_scale, k.c_reg, dcodes, drelcat,
+                                 st);
+    return rc;
+  };
+  rc = one_to_n(who, prepare, query_bwd, true, codes, relcat, V, 2 * R, 2 * R, d, q2.data(), n, labels, smoothing,
+                g_scale, loss, dcodes, grads_on ? drelcat : nullptr, chunk, workspace, workspace_bytes, st);
+  if (rc || !grads_on) return rc;
+  rc = launch_conve_transpose(w.dwt, F, d, Fp, grads->W_fc, st);
+  if (!rc)
+    rc = rgcn_check_cuda(cudaMemcpyAsync(drel, drelcat, (size_t)R * d * 4, cudaMemcpyDeviceToDevice, st), "copy(drel)");
+  if (!rc && Vrel > R)
+    rc = rgcn_check_cuda(cudaMemsetAsync(drel + (size_t)R * d, 0, (size_t)(Vrel - R) * d * 4, st), "memset(drel)");
+  if (!rc)
+    rc = rgcn_check_cuda(cudaMemcpyAsync(grads->rel_inv, drelcat + (size_t)R * d, (size_t)R * d * 4,
+                                         cudaMemcpyDeviceToDevice, st), "copy(drel_inv)");
+  return rc;
+}
+
+extern "C" int64_t rgcn_conve_one_to_n_finish_workspace_bytes(int64_t n) {
+  if (n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_conve_one_to_n_finish_workspace_bytes: need 0 <= n < 2^31");
+    return RGCN_ERR_INVALID;
+  }
+  return align_up(n * 12) + 256;
+}
+
+extern "C" int rgcn_conve_one_to_n_finish(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                          int32_t d, const rgcn_conve_net_t* net, const int32_t* queries, int64_t n,
+                                          const float* g_scale, const float* dcodes_loss, const float* drel_loss,
+                                          const rgcn_conve_grads_t* loss_grads, float* dcodes, float* drel,
+                                          const rgcn_conve_grads_t* grads, void* workspace, int64_t workspace_bytes,
+                                          void* stream) {
+  const char* who = "rgcn_conve_one_to_n_finish";
+  if (!codes || !rel || !g_scale || !dcodes_loss || !drel_loss || !conve_grads_ok(loss_grads) || !dcodes || !drel ||
+      !conve_grads_ok(grads) || !workspace || (n > 0 && !queries)) {
+    rgcn_set_error(std::string(who) + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  int rc = conve_net_checks(who, d, net);
+  if (rc) return rc;
+  if (V <= 0 || Vrel <= 0 || R < 1 || R > Vrel || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error(std::string(who) + ": bad sizes (need V > 0, 1 <= R <= Vrel, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  std::vector<OnenRun> runs;
+  rc = onen_query_checks(who, queries, n, V, R, &runs);
+  if (rc) return rc;
+  if (workspace_bytes < rgcn_conve_one_to_n_finish_workspace_bytes(n)) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_conve_one_to_n_finish_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int C = net->C;
+  rc = launch_onen_scale(dcodes_loss, g_scale, (int64_t)V * d, dcodes, st);
+  if (!rc) rc = launch_onen_scale(drel_loss, g_scale, (int64_t)Vrel * d, drel, st);
+  if (!rc) rc = launch_onen_scale(loss_grads->rel_inv, g_scale, (int64_t)R * d, grads->rel_inv, st);
+  if (!rc) rc = launch_conve_scale(loss_grads->filters, g_scale, 9LL * C, grads->filters, st);
+  if (!rc) rc = launch_conve_scale(loss_grads->conv_bias, g_scale, C, grads->conv_bias, st);
+  if (!rc) rc = launch_conve_scale(loss_grads->W_fc, g_scale, conve_F(d, net->h, C) * d, grads->W_fc, st);
+  if (!rc) rc = launch_conve_scale(loss_grads->b_fc, g_scale, d, grads->b_fc, st);
+  if (rc || n == 0) return rc;
+  int32_t* X = (int32_t*)workspace;
+  rc = onen_upload(queries, n, X, st);
+  const float c_reg = (float)(2.0 / ((double)n * d));
+  for (const OnenRun& run : runs) {   // the L2 term: object queries read rel, subject queries rel_inv
+    const bool inv = run.side == 0;
+    if (!rc)
+      rc = launch_onen_query_bwd(0, codes, inv ? net->rel_inv : rel, d, X + 3 * run.begin, run.end - run.begin,
+                                 run.side, nullptr, g_scale, c_reg, dcodes, inv ? grads->rel_inv : drel, st);
+  }
+  return rc;
+}
+
+// the evaluation entries' shared checks (X, side, R)
+static int conve_eval_checks(const char* who, const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                             int32_t R, int32_t d, const rgcn_conve_net_t* net, const int32_t* X, int64_t n, int side) {
+  if (!codes || !rel || (n > 0 && !X)) {
+    rgcn_set_error(std::string(who) + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  int rc = conve_net_checks(who, d, net);
+  if (rc) return rc;
+  if (V <= 0 || Vrel <= 0 || R < 1 || R > Vrel || n < 0 || n > 0x7fffffffLL || (side != 0 && side != 1)) {
+    rgcn_set_error(std::string(who) + ": bad sizes (need V > 0, 1 <= R <= Vrel, 0 <= n < 2^31, side in {0,1})");
+    return RGCN_ERR_INVALID;
+  }
+  return RGCN_OK;
+}
+
+extern "C" int64_t rgcn_conve_query_rows_workspace_bytes(int32_t d, int32_t h, int32_t C, int64_t n) {
+  if (!conve_shape_ok(d, h, C) || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_conve_query_rows_workspace_bytes: bad arguments (need a valid ConvE shape, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  return conve_work_bytes(d, h, C, std::min(n, CONVE_EVAL_CHUNK), false) + 256;
+}
+
+extern "C" int rgcn_conve_query_rows(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                     int32_t d, const rgcn_conve_net_t* net, const int32_t* X, int64_t n, int side,
+                                     float* Q, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_conve_query_rows";
+  int rc = conve_eval_checks(who, codes, rel, V, Vrel, R, d, net, X, n, side);
+  if (rc) return rc;
+  if (!workspace || (n > 0 && !Q)) {
+    rgcn_set_error(std::string(who) + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_conve_query_rows_workspace_bytes(d, net->h, net->C, n)) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_conve_query_rows_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who);
+  if (rc || n == 0) return rc;
+  Carver ws(workspace, workspace_bytes);
+  const ConvEWork w = conve_carve(ws, d, net->h, net->C, std::min(n, CONVE_EVAL_CHUNK), false);
+  return conve_prepare(net, w)(codes, rel, d, X, n, side, Q, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int64_t rgcn_conve_rank_workspace_bytes(int32_t V, int32_t d, int32_t h, int32_t C, int64_t n) {
+  if (!conve_shape_ok(d, h, C) || V <= 0 || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_conve_rank_workspace_bytes: bad arguments (need V > 0, a valid ConvE shape, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  // [distmult_rank's workspace (its split of codes reused) | network]
+  return distmult_rank_workspace_bytes(V, d, n) + conve_work_bytes(d, h, C, std::min(n, CONVE_EVAL_CHUNK), false);
+}
+
+extern "C" int rgcn_conve_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                               const rgcn_conve_net_t* net, const int32_t* X, int64_t n, int side,
+                               const uint32_t* known_mask, int reuse_split, int32_t* raw_rank, int32_t* filtered_rank,
+                               void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_conve_rank";
+  int rc = conve_eval_checks(who, codes, rel, V, Vrel, R, d, net, X, n, side);
+  if (rc) return rc;
+  if (!workspace) {
+    rgcn_set_error(std::string(who) + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_conve_rank_workspace_bytes(V, d, net->h, net->C, n)) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_conve_rank_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who);
+  if (rc) return rc;
+  const int64_t body = distmult_rank_workspace_bytes(V, d, n);
+  Carver ws((char*)workspace + body, workspace_bytes - body);
+  const ConvEWork w = conve_carve(ws, d, net->h, net->C, std::min(n, CONVE_EVAL_CHUNK), false);
+  return rank_with_queries(who, conve_prepare(net, w), codes, V, distmult_rank_workspace_bytes, codes, rel, V, Vrel, d,
+                           X, n, side, known_mask, reuse_split, raw_rank, filtered_rank, workspace, body,
+                           (cudaStream_t)stream);
+}
+
+extern "C" int64_t rgcn_conve_topk_workspace_bytes(int32_t V, int32_t d, int32_t h, int32_t C, int64_t n, int32_t k) {
+  if (!conve_shape_ok(d, h, C) || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error("rgcn_conve_topk_workspace_bytes: bad arguments (need a valid ConvE shape, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t body = rgcn_topk_workspace_bytes(V, d, n, k);
+  if (body < 0) return body;
+  return body + conve_work_bytes(d, h, C, std::min(n, CONVE_EVAL_CHUNK), false);
+}
+
+extern "C" int rgcn_conve_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                               const rgcn_conve_net_t* net, const int32_t* X, int64_t n, int side, int32_t k,
+                               const uint32_t* exclude_mask, int reuse_split, int32_t* ids, float* energies,
+                               void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_conve_topk";
+  int rc = conve_eval_checks(who, codes, rel, V, Vrel, R, d, net, X, n, side);
+  if (rc) return rc;
+  if (!workspace) {
+    rgcn_set_error(std::string(who) + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  const int64_t need = rgcn_conve_topk_workspace_bytes(V, d, net->h, net->C, n, k);
+  if (need < 0) return (int)need;
+  if (workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small (rgcn_conve_topk_workspace_bytes)");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who);
+  if (rc) return rc;
+  const int64_t body = rgcn_topk_workspace_bytes(V, d, n, k);
+  Carver ws((char*)workspace + body, workspace_bytes - body);
+  const ConvEWork w = conve_carve(ws, d, net->h, net->C, std::min(n, CONVE_EVAL_CHUNK), false);
+  return topk_with_queries(who, conve_prepare(net, w), codes, V, rgcn_topk_workspace_bytes, codes, rel, V, Vrel, d, X,
+                           n, side, k, exclude_mask, reuse_split, ids, energies, workspace, body, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1432,7 +1432,7 @@ int launch_gemm_variational_tf32x3(const float* H, const float* Bt_hi, const flo
 
 // C[M,N] (+)= A^T B, A [K,M] row-major, B [K,N] row-major (see k_gemm_tn_tf32x3)
 int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
-                          int M, int N, int K, int accumulate, cudaStream_t st) {
+                          int M, int N, int K, int accumulate, cudaStream_t st, int max_splits) {
   if (M == 0 || N == 0) return RGCN_OK;
   if (M % 4 != 0 || N % 4 != 0 || lda % 4 != 0 || ldb % 4 != 0 || ldc % 4 != 0) {
     rgcn_set_error("gemm_tn_tf32x3: M, N and leading dimensions must be multiples of 4");
@@ -1461,7 +1461,7 @@ int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t l
   const int64_t tiles = tiles_of(M, N, BN);
   const int64_t kb_total = (K + BK - 1) / BK, sms = sm_count();
   int64_t splits = 1, kb_per_split = kb_total, best = -1;
-  for (int64_t s = 1; s <= kb_total && (s == 1 || s * tiles <= 8 * sms); ++s) {
+  for (int64_t s = 1; s <= kb_total && (s == 1 || s * tiles <= 8 * sms) && (max_splits <= 0 || s <= max_splits); ++s) {
     const int64_t kps = (kb_total + s - 1) / s, s_eff = (kb_total + kps - 1) / kps;   // no empty split
     const int64_t cost = (s_eff * tiles + sms - 1) / sms * (kps + TN_KB_FIXED);
     if (best < 0 || cost < best) {

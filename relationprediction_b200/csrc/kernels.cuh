@@ -194,8 +194,10 @@ int launch_gemm_ensemble_topk_tf32x3(const float* qa_hi, const float* qa_lo, con
 int launch_ensemble_topk_merge(const EnsCand* cand, int64_t n, int per_row, int k, int32_t* ids, double* u,
                                double* scores, cudaStream_t st);
 
+// max_splits > 0 caps the split-K count; max_splits = 1 makes C bitwise repeatable (one CTA adds each tile's parts
+// in order), at the cost of fewer CTAs when the output has few tiles
 int launch_gemm_tn_tf32x3(const float* A, int64_t lda, const float* B, int64_t ldb, float* C, int64_t ldc,
-                          int M, int N, int K, int accumulate, cudaStream_t st);
+                          int M, int N, int K, int accumulate, cudaStream_t st, int max_splits = 0);
 
 // 1-N training (onen.cu and the EPI = 5 scoring GEMM).  Loss parts the GEMM writes for M queries and N entities:
 int64_t gemm_onen_loss_parts(int64_t M, int N);
@@ -323,3 +325,37 @@ int launch_rotate_rank_prepare(const float* codes, const float* rel, int d, cons
 int launch_rotate_rank(const float* Q, const float* codes, int V, int d, int64_t n, const float* gold_D,
                        const int32_t* gold_col, const uint32_t* known, int32_t* raw_cnt, int32_t* known_cnt,
                        cudaStream_t st);
+
+// conve.cu -- the ConvE query network (DESIGN.md section 1): d = h w, image 2h x w, C filters 3x3, F = C (2h-2)(w-2)
+// feature columns stored with leading dimension Fp (F rounded up to 4).  Masks are uint8 keep-masks or null.
+// Feature rows Feat [n, Fp] of the queries X[t] (anchor in column acol, relation row rel[X[t][1]])
+int launch_conve_conv_fwd(const float* codes, const float* rel, int d, int h, int C, const int32_t* X, int acol,
+                          int64_t n, const float* filt, const float* cbias, const uint8_t* in_mask, float inv_in,
+                          const uint8_t* feat_mask, float inv_feat, int Fp, float* Feat, cudaStream_t st);
+// Q = relu((Q + b) hid_mask / keep) in place, Q [n, d]
+int launch_conve_fc_act(float* Q, int64_t n, int d, const float* b, const uint8_t* hid_mask, float inv_hid,
+                        cudaStream_t st);
+// dZ [m, d] and dZt [d, ldt] (columns m..ldt-1 zero) = dQ [Q > 0] hid_mask / keep
+int launch_conve_dz(const float* Q, const float* dQ, int64_t m, int d, const uint8_t* hid_mask, float inv_hid,
+                    float* dZ, float* dZt, int64_t ldt, cudaStream_t st);
+// db (+)= the row sums of dZt [d, m] (leading dimension ldt), each in a fixed order
+int launch_conve_rowsum(const float* dZt, int d, int64_t m, int64_t ldt, float* db, int accumulate, cudaStream_t st);
+// convolution backward: conve_conv_parts(m) filter / bias gradient parts [parts, 10 C] into part, the image gradient
+// red.add into dcodes[anchor = X[t][0]] and drel[X[t][1]]
+int64_t conve_conv_parts(int64_t m);
+int64_t conve_smem_bytes(int d, int h, int w, int C);
+int launch_conve_conv_bwd(const float* codes, const float* rel, int d, int h, int C, const int32_t* X, int64_t m,
+                          const float* filt, const uint8_t* in_mask, float inv_in, const float* Feat, const float* dF,
+                          float inv_feat, int Fp, float* part, float* dcodes, float* drel, cudaStream_t st);
+// dfilt [C, 9] / dbias [C] (+)= the sum of the parts in part order
+int launch_conve_filter_reduce(const float* part, int parts, int C, float* dfilt, float* dbias, int accumulate,
+                               cudaStream_t st);
+// pre-split of W [F, d] zero-padded to Fp rows: transposed = 1 -> [d, Fp], 0 -> [Fp, d]
+int launch_conve_split_w(const float* W, int F, int d, int Fp, int transposed, float* hi, float* lo, cudaStream_t st);
+// dW [F, d] = dWt [d, Fp]^T (first F columns)
+int launch_conve_transpose(const float* dWt, int F, int d, int Fp, float* dW, cudaStream_t st);
+// gold_sig[t] = sigmoid(<Q[t], codes[gold]>), gold = X[t][0] (side 0) or X[t][2] (side 1)
+int launch_conve_gold(const float* Q, const float* codes, int d, const int32_t* X, int64_t n, int side,
+                      float* gold_sig, int32_t* gold_col, cudaStream_t st);
+// dst = g_scale[0] src, any count
+int launch_conve_scale(const float* src, const float* g_scale, int64_t count, float* dst, cudaStream_t st);

@@ -123,9 +123,13 @@ class BilinearDiag(Model):
                 queries = ops.one_to_n_queries(np.asarray(self.X.value, dtype=np.int32).reshape(-1, 3))
                 self._one_to_n_feed = (self.X.value, queries, self.one_to_n_labels.rows(queries))
             _, queries, labels = self._one_to_n_feed
-            self._one_to_n_loss = ops.one_to_n_loss(subject_codes.contiguous(), relation_codes.contiguous(), queries,
-                                                    labels, self.label_smoothing, self.ONE_TO_N, self.relation_count)
+            self._one_to_n_loss = self._one_to_n_op(subject_codes.contiguous(), relation_codes.contiguous(), queries,
+                                                    labels)
         return self._one_to_n_loss
+
+    def _one_to_n_op(self, codes, rel, queries, labels):
+        """(loss, reg) of the 1-N queries with their label rows (ConvE puts its query network here)"""
+        return ops.one_to_n_loss(codes, rel, queries, labels, self.label_smoothing, self.ONE_TO_N, self.relation_count)
 
     def _self_adversarial(self):
         """(loss, reg, energies) of self-adversarial negative sampling over the fed X in the sampler's layout (n

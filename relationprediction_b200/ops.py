@@ -1345,3 +1345,221 @@ def one_to_n_loss(codes, rel, queries, labels, smoothing, decoder, relation_coun
     # inside Function.forward the grad mode is off and needs_input_grad ignores torch.no_grad(): decide here
     grads = torch.is_grad_enabled() and (codes.requires_grad or rel.requires_grad)
     return _OneToNFn.apply(codes, rel, labels, q, float(smoothing), ONE_TO_N_DECODERS[decoder], R, chunk, grads)
+
+
+# ---- ConvE (rgcn_conve_*, include/rgcn_b200.h): the query network in front of the 1-N, rank and top-k paths ----
+class ConvEWeights(tuple):
+    """(rel_inv [R, d], filters [C, 3, 3], conv_bias [C], W_fc [F, d], b_fc [d]) of a ConvE decoder with image height
+    h (d = h w): the reciprocal relation rows and the network weights, CUDA float32, contiguous."""
+
+    def __new__(cls, rel_inv, filters, conv_bias, W_fc, b_fc, h):
+        self = tuple.__new__(cls, (rel_inv, filters, conv_bias, W_fc, b_fc))
+        self.h = int(h)
+        return self
+
+    @property
+    def C(self):
+        return self[1].shape[0]
+
+    def check(self, d):
+        """Checks the shapes against the code width d; returns F."""
+        h, C = self.h, self[1].shape[0] if self[1].dim() else 0
+        if h < 2 or d % h or d // h < 3 or C < 1 or d % 4:
+            raise ValueError("ConvE needs d %% 4 == 0, d = h w with h >= 2, w >= 3 and C >= 1 filters (d = %d, h = %d, "
+                             "C = %d)" % (d, h, C))
+        F = C * (2 * h - 2) * (d // h - 2)
+        for name, t, shape in (("rel_inv", self[0], (self[0].shape[0], d)), ("filters", self[1], (C, 3, 3)),
+                               ("conv_bias", self[2], (C,)), ("W_fc", self[3], (F, d)), ("b_fc", self[4], (d,))):
+            _check_cuda_f32(name, t, shape)
+        return F
+
+
+def _conve_net(weights, masks=(None, None, None), keeps=(1.0, 1.0, 1.0)):
+    rel_inv, filters, conv_bias, W_fc, b_fc = weights
+    ptrs = [_ptr(t).value for t in (rel_inv, filters, conv_bias, W_fc, b_fc) + tuple(masks)]
+    return _lib.ConvENet(weights.h, filters.shape[0], *ptrs, *[float(k) for k in keeps])
+
+
+def _conve_grads(tensors):
+    return _lib.ConvEGrads(*[_ptr(t).value for t in tensors])
+
+
+class _ConvEOneToNFn(torch.autograd.Function):
+    """Returns (loss, reg) of rgcn_conve_one_to_n; the gradients of all seven tensors come from the forward with
+    g_scale = (1, 0) and are finished by rgcn_conve_one_to_n_finish, as _OneToNFn does."""
+
+    @staticmethod
+    def forward(ctx, codes, rel, rel_inv, filters, conv_bias, W_fc, b_fc, labels, queries, smoothing, h, masks, keeps,
+                R, chunk, grads):
+        V, d = codes.shape
+        dev = codes.device
+        weights = ConvEWeights(rel_inv, filters, conv_bias, W_fc, b_fc, h)
+        net = _conve_net(weights, masks, keeps)
+        loss = torch.empty(2, dtype=torch.float32, device=dev)
+        dcodes = torch.empty_like(codes) if grads else None
+        drel = torch.empty_like(rel) if grads else None
+        dnet = [torch.empty_like(t) for t in weights] if grads else None
+        g_loss_only = torch.tensor([1.0, 0.0], dtype=torch.float32, device=dev) if grads else None
+        _call("rgcn_conve_one_to_n", "rgcn_conve_one_to_n_workspace_bytes",
+              (V, R, d, h, weights.C, len(queries), chunk),
+              (_ptr(codes), _ptr(rel), V, rel.shape[0], R, d, ctypes.byref(net), _np_ptr(queries), len(queries),
+               _ptr(labels), smoothing, _ptr(g_loss_only), _ptr(loss), _ptr(dcodes), _ptr(drel),
+               ctypes.byref(_conve_grads(dnet)) if grads else None, chunk), dev)
+        ctx.args = (queries, R, h, keeps)
+        if grads:
+            ctx.save_for_backward(codes, rel, *weights, dcodes, drel, *dnet)
+        return loss[0], loss[1]
+
+    @staticmethod
+    def backward(ctx, g_loss, g_reg):
+        saved = ctx.saved_tensors
+        codes, rel = saved[0], saved[1]
+        weights = ConvEWeights(*saved[2:7], h=ctx.args[2])
+        dcodes_loss, drel_loss, dnet_loss = saved[7], saved[8], saved[9:14]
+        queries, R, h, keeps = ctx.args
+        V, d = codes.shape
+        dev = codes.device
+        gs = torch.zeros(2, dtype=torch.float32, device=dev)
+        if g_loss is not None:
+            gs[0] = g_loss
+        if g_reg is not None:
+            gs[1] = g_reg
+        dcodes, drel = torch.empty_like(codes), torch.empty_like(rel)
+        dnet = [torch.empty_like(t) for t in weights]
+        net = _conve_net(weights)
+        _call("rgcn_conve_one_to_n_finish", "rgcn_conve_one_to_n_finish_workspace_bytes", (len(queries),),
+              (_ptr(codes), _ptr(rel), V, rel.shape[0], R, d, ctypes.byref(net), _np_ptr(queries), len(queries),
+               _ptr(gs), _ptr(dcodes_loss), _ptr(drel_loss), ctypes.byref(_conve_grads(dnet_loss)), _ptr(dcodes),
+               _ptr(drel), ctypes.byref(_conve_grads(dnet))), dev)
+        return (dcodes, drel) + tuple(dnet) + (None,) * 9
+
+
+def _check_conve_masks(masks, n, d, C):
+    masks = tuple(masks) if masks is not None else (None, None, None)
+    for name, m, width in zip(("input_mask", "feature_mask", "hidden_mask"), masks, (2 * d, C, d)):
+        if m is not None and not (m.is_cuda and m.dtype == torch.uint8 and m.is_contiguous()
+                                  and tuple(m.shape) == (n, width)):
+            raise _lib.RgcnError("%s must be a contiguous CUDA uint8 [%d, %d] keep-mask" % (name, n, width))
+    return masks
+
+
+def conve_one_to_n_loss(codes, rel, weights, queries, labels, smoothing, masks=None, keeps=(1.0, 1.0, 1.0),
+                        relation_count=None):
+    """1-N loss of the ConvE decoder: ops.one_to_n_loss with the query rows of the ConvE network (weights a
+    ConvEWeights), (anchor, r, 1) reading rel[r] and (anchor, r, 0) the reciprocal row rel_inv[r].  masks: None or the
+    (input [n, 2d], feature [n, C], hidden [n, d]) uint8 keep-masks of the queries, each None for no dropout, scaled by
+    1 / keeps.  Returns (loss, reg), reg the L2 term of the anchor row and the relation or reciprocal row.
+    Differentiable in codes, rel and the five tensors of weights."""
+    _check_cuda_f32("codes", codes)
+    _check_cuda_f32("relation table", rel)
+    V, d = codes.shape
+    F = weights.check(d)
+    R = rel.shape[0] if relation_count is None else int(relation_count)
+    if weights[0].shape[0] != R:
+        raise _lib.RgcnError("rel_inv must have one row per relation (%d)" % R)
+    q = _check_queries(queries, V, R)
+    words = (V + 31) // 32
+    if not (labels.is_cuda and labels.dtype == torch.int32 and labels.is_contiguous()
+            and tuple(labels.shape) == (len(q), words)):
+        raise _lib.RgcnError("labels must be a contiguous CUDA int32 [n, ceil(V/32)] tensor (bit rows)")
+    if not 0.0 <= float(smoothing) < 1.0:
+        raise ValueError("conve_one_to_n_loss: label smoothing must be in [0, 1), got %r" % (smoothing,))
+    masks = _check_conve_masks(masks, len(q), d, weights.C)
+    Fp = (F + 3) // 4 * 4
+    chunk = max(1, min(len(q), ONE_TO_N_CHUNK_BYTES // ((V + 6 * d + 3 * Fp) * 4)))
+    tensors = (codes, rel) + tuple(weights)
+    grads = torch.is_grad_enabled() and any(t.requires_grad for t in tensors)
+    return _ConvEOneToNFn.apply(codes, rel, *weights, labels, q, float(smoothing), weights.h, masks,
+                                tuple(float(k) for k in keeps), R, chunk, grads)
+
+
+def conve_query_rows(codes, rel, weights, X, side, relation_count=None):
+    """Test-mode ConvE query rows [n, d] of the triples X (int32 [n, 3] CUDA): side 1 f(codes[s], rel[r]), side 0
+    f(codes[o], rel_inv[r]) (rgcn_conve_query_rows)."""
+    _check_cuda_f32("codes", codes)
+    _check_cuda_f32("relation table", rel)
+    V, d = codes.shape
+    weights.check(d)
+    R = rel.shape[0] if relation_count is None else int(relation_count)
+    if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
+        raise _lib.RgcnError("X must be a contiguous CUDA int32 [n,3] tensor")
+    n = X.shape[0]
+    Q = torch.empty((n, d), dtype=torch.float32, device=codes.device)
+    net = _conve_net(weights)
+    _call("rgcn_conve_query_rows", "rgcn_conve_query_rows_workspace_bytes", (d, weights.h, weights.C, n),
+          (_ptr(codes), _ptr(rel), V, rel.shape[0], R, d, ctypes.byref(net), _ptr(X), n, int(side), _ptr(Q)),
+          codes.device)
+    return Q
+
+
+class ConvERanker(object):
+    """Fused all-entity ranking and top-k of the ConvE decoder (rgcn_conve_rank / rgcn_conve_topk): the interface and
+    split reuse of DistMultRanker, the query rows from the ConvE network.  ConvE has no relation prediction (its
+    energy is not linear in the relation row) and is no member of the fused ensemble (EnsembleRanker takes
+    DistMultRanker objects only)."""
+    TOPK_CHUNK_BYTES = DistMultRanker.TOPK_CHUNK_BYTES
+
+    def __init__(self, codes, rel, weights, relation_count=None):
+        _check_cuda_f32("codes", codes)
+        _check_cuda_f32("relation table", rel)
+        weights.check(codes.shape[1])
+        self.codes, self.rel, self.weights = codes, rel, weights
+        self.relation_count = rel.shape[0] if relation_count is None else int(relation_count)
+        self._net = _conve_net(weights)
+        self._ws, self._ws_n, self._split_ready = None, -1, False
+
+    _check_rows = DistMultRanker._check_rows
+    _chunk_rows = DistMultRanker._chunk_rows
+
+    def top_k(self, X, side, k, exclude_mask=None):
+        """As DistMultRanker.top_k, over the ConvE query rows."""
+        lib = _lib.load()
+        V, d = self.codes.shape
+        h, C, R = self.weights.h, self.weights.C, self.relation_count
+        self._check_rows(X, exclude_mask, "exclude_mask")
+        k, n = int(k), X.shape[0]
+        chunk, nb = self._chunk_rows(n, lambda m: lib.rgcn_conve_topk_workspace_bytes(V, d, h, C, m, k),
+                                     "rgcn_conve_topk_workspace_bytes")
+        dev = self.codes.device
+        if self._ws is None or self._ws.numel() < nb:
+            self._ws, self._ws_n, self._split_ready = _workspace(nb, dev), -1, False
+        ids = torch.empty((n, k), dtype=torch.int32, device=dev)
+        energies = torch.empty((n, k), dtype=torch.float32, device=dev)
+        for c0 in range(0, max(n, 1), chunk):
+            c1 = min(n, c0 + chunk)
+            rc = lib.rgcn_conve_topk(_ptr(self.codes), _ptr(self.rel), V, self.rel.shape[0], R, d,
+                                     ctypes.byref(self._net), _ptr(X[c0:c1]), c1 - c0, int(side), k,
+                                     _ptr(None if exclude_mask is None else exclude_mask[c0:c1]),
+                                     int(self._split_ready), _ptr(ids[c0:c1]), _ptr(energies[c0:c1]), _ptr(self._ws),
+                                     self._ws.numel(), _stream(dev))
+            _lib.check(rc, "rgcn_conve_topk")
+            self._split_ready = True
+        return ids, energies
+
+    def rank(self, X, side, known_mask=None):
+        """As DistMultRanker.rank, over the ConvE query rows."""
+        lib = _lib.load()
+        V, d = self.codes.shape
+        h, C, R = self.weights.h, self.weights.C, self.relation_count
+        self._check_rows(X, known_mask, "known_mask")
+        n = X.shape[0]
+        dev = self.codes.device
+        if self._ws is None or n > self._ws_n:
+            nb = lib.rgcn_conve_rank_workspace_bytes(V, d, h, C, n)
+            if nb < 0:
+                _lib.check(int(nb), "rgcn_conve_rank_workspace_bytes")
+            self._ws, self._ws_n, self._split_ready = _workspace(nb, dev), n, False
+        raw = torch.empty(n, dtype=torch.int32, device=dev)
+        filt = torch.empty(n, dtype=torch.int32, device=dev) if known_mask is not None else None
+        rc = lib.rgcn_conve_rank(_ptr(self.codes), _ptr(self.rel), V, self.rel.shape[0], R, d, ctypes.byref(self._net),
+                                 _ptr(X), n, int(side), _ptr(known_mask), int(self._split_ready), _ptr(raw), _ptr(filt),
+                                 _ptr(self._ws), self._ws.numel(), _stream(dev))
+        _lib.check(rc, "rgcn_conve_rank")
+        self._split_ready = True
+        return raw, filt
+
+    def rank_relations(self, X, known_mask=None):
+        raise NotImplementedError("the ConvE decoder has no relation prediction")
+
+    def top_k_relations(self, X, k, exclude_mask=None):
+        raise NotImplementedError("the ConvE decoder has no relation prediction")

@@ -19,6 +19,7 @@ import numpy as np
 
 from .optim import ClippedAdam
 from .common import auxilliaries, evaluation, io, model_builder, settings_reader
+from .decoders.conve import ConvE
 from .decoders.rotate import Rotate
 
 
@@ -288,6 +289,8 @@ def main(argv=None):
     general, opt = settings['General'], settings['Optimizer']
     if args.relation_metrics and isinstance(model, Rotate):
         raise SystemExit("--relation-metrics: the RotatE decoder has no relation prediction")
+    if args.relation_metrics and isinstance(model, ConvE):
+        raise SystemExit("--relation-metrics: the ConvE decoder has no relation prediction")
 
     ns = auxilliaries.NegativeSampler(int(general['NegativeSampleRate']), len(entities))
     adj_list = [[] for _ in entities]
