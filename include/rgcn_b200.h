@@ -378,6 +378,49 @@ int rgcn_diag_backward(const rgcn_graph_t* g, int32_t d, const float* H, const f
                        float* slice_sumsq2, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * CompGCN layer (Name=compgcn, Vashishth et al., ICLR 2020).  Messages as above (forward s->o with weight id r,
+ * backward o->s with weight id r+R); a message composes the sender's row with its weight id's row of the relation
+ * table Z = [Z_forward; Z_inverse]:
+ *
+ *   phi(h, z) = h (.) z  (composition RGCN_COMPOSITION_MULT)   or   h - z  (RGCN_COMPOSITION_SUB)
+ *   A_f[v] = sum_{m -> v, w_m < R}  norm_m phi(H[src_m], Z[w_m]),   A_b[v] likewise over w_m >= R,
+ *   L[v]   = phi(H[v], z_loop)
+ *   Cat    = [ M (.) [A_f | A_b] / keep  |  L ] / 3                         [V_dst, 3 d_in]
+ *   out    = act( Cat W_cat + b ),   Z_next = Z W_rel
+ *
+ * H : [V_src, d_in] (rows [V_dst, V_src) are halo rows that only send);  Z : [n_relw = 2R, d_in];  z_loop : [d_in];
+ * W_cat : [3 d_in, d_out] (W_I; W_O; W_S);  W_rel : [d_in, d_out];  b, db : [d_out];  out, dOut : [V_dst, d_out];
+ * Z_next, dZ_next : [2R, d_out];  drop_mask M (or NULL) : [V_dst, 2 d_in] uint8, keep the keep probability.  act is
+ * ReLU when relu != 0.  d_in % 4 == 0, d_out % 4 == 0.  The forward writes Cat (kept for the backward), out and Z_next.
+ * Backward:  G = dOut * relu'(out),  db = column sums of G,  dW_cat = Cat^T G,  dCat = G W_cat^T,
+ *            dW_rel = Z^T dZ_next,  dZ = dZ_next W_rel^T + the walk's terms, and per message (u = src, S = norm_m times
+ *            the message slab of dCat at dst_m, with M / keep and 1/3 applied):
+ *              mult: dH[u] += Z[w_m] (.) S,  dZ[w_m] += H[u] (.) S        sub: dH[u] += S,  dZ[w_m] -= S
+ *            and per row v < V_dst, with g_L = dCat[v, 2 d_in : 3 d_in] / 3:
+ *              mult: dH[v] += z_loop (.) g_L,  dz_loop += H[v] (.) g_L    sub: dH[v] += g_L,  dz_loop -= g_L
+ * Every output is overwritten.  The forward walks the destination-major CSR view, the backward the source-major one:
+ * a graph prepared without the CSR views (graph_views == 2) is RGCN_ERR_INVALID.
+ * Arguments are checked before any device work: an unknown composition, null pointers, d_in or d_out not a positive
+ * multiple of 4 or keep <= 0 are RGCN_ERR_INVALID, a short workspace RGCN_ERR_WORKSPACE; a host-only graph is
+ * RGCN_ERR_NODEVICE.
+ * ---------------------------------------------------------------------------------------------- */
+#define RGCN_COMPOSITION_MULT 0
+#define RGCN_COMPOSITION_SUB 1
+
+int64_t rgcn_compgcn_workspace_bytes(const rgcn_graph_t* g, int32_t d_in, int32_t d_out, int backward);
+
+int rgcn_compgcn_forward(const rgcn_graph_t* g, int32_t d_in, int32_t d_out, int composition, const float* H,
+                         const float* Z, const float* z_loop, const float* W_cat, const float* W_rel, const float* b,
+                         const uint8_t* drop_mask, float keep, int relu, float* Cat, float* out, float* Z_next,
+                         void* workspace, int64_t workspace_bytes, void* stream);
+
+int rgcn_compgcn_backward(const rgcn_graph_t* g, int32_t d_in, int32_t d_out, int composition, const float* H,
+                          const float* Z, const float* z_loop, const float* W_cat, const float* W_rel,
+                          const uint8_t* drop_mask, float keep, int relu, const float* Cat, const float* out,
+                          const float* dOut, const float* dZ_next, float* dH, float* dZ, float* dz_loop, float* dW_cat,
+                          float* dW_rel, float* db, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
  * Highway skip connection between R-GCN layers (SkipConnections=Highway, model_builder.py:304-305;
  * extras/highway_layer.py:14-38).  c1 = the wrapped layer's output, c2 = the layer's input:
  *

@@ -23,6 +23,7 @@ EXPORTED_SYMBOLS = [
     "rgcn_basis_onehot_workspace_bytes", "rgcn_basis_onehot_forward", "rgcn_basis_onehot_backward",
     "rgcn_basis_diagcoef_workspace_bytes", "rgcn_basis_diagcoef_forward", "rgcn_basis_diagcoef_backward",
     "rgcn_diag_workspace_bytes", "rgcn_diag_forward", "rgcn_diag_backward",
+    "rgcn_compgcn_workspace_bytes", "rgcn_compgcn_forward", "rgcn_compgcn_backward",
     "rgcn_highway_workspace_bytes", "rgcn_highway_forward", "rgcn_highway_backward",
     "rgcn_variational_workspace_bytes", "rgcn_variational_forward", "rgcn_variational_backward",
     "distmult_forward", "distmult_backward", "distmult_rank_workspace_bytes", "distmult_rank",
@@ -179,6 +180,14 @@ def _declare(lib):
     lib.rgcn_diag_backward.restype = c_int
     lib.rgcn_diag_backward.argtypes = [vp, c_int32, vp, vp, vp, vp, vp, c_float, c_int, vp, vp, vp, vp, vp, vp, vp,
                                        vp, vp, c_int64, vp]
+    lib.rgcn_compgcn_workspace_bytes.restype = c_int64
+    lib.rgcn_compgcn_workspace_bytes.argtypes = [vp, c_int32, c_int32, c_int]
+    lib.rgcn_compgcn_forward.restype = c_int
+    lib.rgcn_compgcn_forward.argtypes = [vp, c_int32, c_int32, c_int, vp, vp, vp, vp, vp, vp, vp, c_float, c_int, vp,
+                                         vp, vp, vp, c_int64, vp]
+    lib.rgcn_compgcn_backward.restype = c_int
+    lib.rgcn_compgcn_backward.argtypes = [vp, c_int32, c_int32, c_int, vp, vp, vp, vp, vp, vp, c_float, c_int, vp,
+                                          vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, c_int64, vp]
     lib.rgcn_highway_workspace_bytes.restype = c_int64
     lib.rgcn_highway_workspace_bytes.argtypes = [c_int64, c_int32, c_int]
     lib.rgcn_highway_forward.restype = c_int

@@ -1,6 +1,7 @@
 """Name= -> component chain factory (reference: common/model_builder.py:26-184, :273-319).
 
-Only the branches on the accelerated path are built: encoders `gcn_diag` (DiagGcn layers), `gcn_basis` (BasisGcn, or ConcatGcn
+Only the branches on the accelerated path are built: encoders `gcn_diag` (DiagGcn layers), `compgcn` (CompGcn layers,
+which the reference does not have; they learn the relation codes), `gcn_basis` (BasisGcn, or ConcatGcn
 when Concatenation=Yes, BasisGcnTimesDiag when DiagonalCoefficients=Yes; with UseInputTransform=No layer 0 is a one-hot
 BasisGcn; SkipConnections=Highway wraps every
 feature-input layer in a HighwayLayer), `embedding`, and the variational encoders `variational_embedding` and
@@ -15,6 +16,7 @@ from ..encoders.affine_transform import AffineTransform
 from ..encoders.message_gcns.gcn_basis import BasisGcn
 from ..encoders.message_gcns.gcn_basis_concat import ConcatGcn
 from ..encoders.message_gcns.gcn_basis_times_diag import BasisGcnTimesDiag
+from ..encoders.message_gcns.compgcn import CompGcn, parse_composition
 from ..encoders.message_gcns.gcn_diag import DiagGcn
 from ..encoders.relation_embedding import RelationEmbedding
 from ..extras.graph_representations import Representation
@@ -55,6 +57,33 @@ def build_encoder(encoder_settings, triples):
             encoding = AffineTransform(projection_shape, encoder_settings, next_component=encoding,
                                        onehot_input=False, use_nonlinearity=False, use_bias=True)
         return RelationEmbedding(relation_shape, encoder_settings, next_component=encoding)
+
+    if name == "compgcn":
+        # A bias-free linear one-hot embedding of width InternalEncoderDimension, then NumberOfLayers CompGcn layers
+        # (the last one linear, of width CodeDimension).  The relation codes are the top layer's Z^L[0:R]: no
+        # RelationEmbedding and no output projection, since the relation codes would not pass through one.  The basis
+        # and ablation flags are not read.
+        parse_composition(encoder_settings)
+        if _flag(encoder_settings, 'UseOutputTransform') == "Yes":
+            raise ValueError("Encoder Name=compgcn takes no UseOutputTransform=Yes: the relation codes would not "
+                             "pass through the output projection")
+        skip = _flag(encoder_settings, 'SkipConnections', 'None')
+        if skip != 'None':
+            raise ValueError("Encoder Name=compgcn takes no SkipConnections (got %r): the relation codes would not "
+                             "pass through them" % skip)
+        graph = Representation(triples, encoder_settings)
+        d_int = int(encoder_settings['InternalEncoderDimension'])
+        d_code = int(encoder_settings['CodeDimension'])
+        layers = int(encoder_settings['NumberOfLayers'])
+        if layers < 1:
+            raise ValueError("Encoder Name=compgcn needs NumberOfLayers >= 1, got %d" % layers)
+        encoding = AffineTransform([int(encoder_settings['EntityCount']), d_int], encoder_settings,
+                                   next_component=graph, onehot_input=True, use_bias=False, use_nonlinearity=False)
+        for layer in range(layers):
+            top = layer == layers - 1
+            encoding = CompGcn([d_int, d_code if top else d_int], encoder_settings, next_component=encoding,
+                               use_nonlinearity=not top, owns_relations=layer == 0, top=top)
+        return encoding
 
     if name == "gcn_basis":
         graph = Representation(triples, encoder_settings)

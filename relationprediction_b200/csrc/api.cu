@@ -1058,6 +1058,125 @@ extern "C" int rgcn_diag_backward(const rgcn_graph_t* g, int32_t d, const float*
 }
 
 // ------------------------------------------------------------------------------------------------
+// CompGCN layer (Name=compgcn, compgcn.cu): the walk writes the GEMM operand Cat, one GEMM with the bias + ReLU
+// epilogue makes `out`, a second one the next relation table
+// ------------------------------------------------------------------------------------------------
+extern "C" int64_t rgcn_compgcn_workspace_bytes(const rgcn_graph_t* g, int32_t d_in, int32_t d_out, int backward) {
+  if (!g || d_in <= 0 || d_out <= 0) {
+    rgcn_set_error("rgcn_compgcn_workspace_bytes: bad arguments");
+    return RGCN_ERR_INVALID;
+  }
+  int64_t bytes = align_up((int64_t)2 * 3 * d_in * d_out * 4);  // hi/lo split of W_cat (the largest split operand)
+  if (backward) {
+    bytes += align_up((int64_t)g->V_dst * d_out * 4);      // G
+    bytes += align_up((int64_t)g->V_dst * 3 * d_in * 4);   // dCat
+  }
+  return bytes + 256;
+}
+
+// shape, pointer and workspace checks come first (they need no device), then the graph
+static int compgcn_checks(const rgcn_graph_t* g, int32_t d_in, int32_t d_out, int composition, bool pointers_ok,
+                          float keep, int backward, int64_t workspace_bytes, const char* who) {
+  int rc = shape_checks(g, d_in, 1, who);
+  if (!rc && (d_out <= 0 || d_out % 4 != 0)) {
+    rgcn_set_error(std::string(who) + ": need d_out > 0, d_out % 4 == 0");
+    rc = RGCN_ERR_INVALID;
+  }
+  if (!rc && composition != RGCN_COMPOSITION_MULT && composition != RGCN_COMPOSITION_SUB) {
+    rgcn_set_error(std::string(who) + ": composition must be RGCN_COMPOSITION_MULT or RGCN_COMPOSITION_SUB");
+    rc = RGCN_ERR_INVALID;
+  }
+  if (!rc) rc = pointer_checks(pointers_ok, keep, who);
+  if (!rc) rc = workspace_checks(workspace_bytes, rgcn_compgcn_workspace_bytes(g, d_in, d_out, backward), who);
+  if (!rc) rc = graph_checks(g, d_in, 1, who, true, true, false);
+  return rc;
+}
+
+extern "C" int rgcn_compgcn_forward(const rgcn_graph_t* g, int32_t d_in, int32_t d_out, int composition,
+                                    const float* H, const float* Z, const float* z_loop, const float* W_cat,
+                                    const float* W_rel, const float* b, const uint8_t* drop_mask, float keep, int relu,
+                                    float* Cat, float* out, float* Z_next, void* workspace, int64_t workspace_bytes,
+                                    void* stream) {
+  const char* who = "rgcn_compgcn_forward";
+  int rc = compgcn_checks(g, d_in, d_out, composition,
+                          H && Z && z_loop && W_cat && W_rel && b && Cat && out && Z_next && workspace, keep, 0,
+                          workspace_bytes, who);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
+  if (rc) return rc;
+  Carver ws(workspace, workspace_bytes);
+  float* split_ws = ws.take<float>((int64_t)2 * 3 * d_in * d_out);
+  const int64_t ldc = 3 * (int64_t)d_in;
+  MARK("start");
+  // Cat = [mask / keep (.) [A_f | A_b] | phi(H, z_loop)] / 3; the split rows are reduced into zeroed rows
+  rc = launch_zero_rows(Cat, ldc, g->by_dst.d_split_rows, (int)g->by_dst.n_split, st);
+  if (!rc)
+    rc = launch_compgcn_fwd(composition, g->by_dst.d_items, (int)g->by_dst.n_items, g->by_dst.d_nbr, g->by_dst.d_relw,
+                            g->by_dst.d_norm, H, Z, z_loop, d_in, g->n_relw, drop_mask, 1.0f / keep, Cat, st);
+  if (rc) return rc;
+  MARK("compgcn_walk_fwd");
+  // out = act(Cat W_cat + b)
+  rc = launch_gemm_split_b(W_cat, d_out, d_out, (int)ldc, 1, split_ws, split_ws + (size_t)d_out * ldc, st);
+  if (!rc)
+    rc = launch_gemm_bias_act_tf32x3(Cat, ldc, split_ws, split_ws + (size_t)d_out * ldc, ldc, b, relu, out, d_out,
+                                     g->V_dst, d_out, (int)ldc, st);
+  if (rc) return rc;
+  MARK("compgcn_gemm_out");
+  // Z_next = Z W_rel
+  rc = gemm_any(st, split_ws, false, false, g->n_relw, d_out, d_in, Z, d_in, W_rel, d_out, 0.f, Z_next, d_out);
+  MARK("compgcn_gemm_rel");
+  return rc;
+}
+
+extern "C" int rgcn_compgcn_backward(const rgcn_graph_t* g, int32_t d_in, int32_t d_out, int composition,
+                                     const float* H, const float* Z, const float* z_loop, const float* W_cat,
+                                     const float* W_rel, const uint8_t* drop_mask, float keep, int relu,
+                                     const float* Cat, const float* out, const float* dOut, const float* dZ_next,
+                                     float* dH, float* dZ, float* dz_loop, float* dW_cat, float* dW_rel, float* db,
+                                     void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_compgcn_backward";
+  int rc = compgcn_checks(g, d_in, d_out, composition,
+                          H && Z && z_loop && W_cat && W_rel && Cat && dOut && dZ_next && dH && dZ && dz_loop &&
+                              dW_cat && dW_rel && db && workspace && (!relu || out),
+                          keep, 1, workspace_bytes, who);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = rgcn_check_cuda(cudaSetDevice(g->device), "cudaSetDevice");
+  if (rc) return rc;
+  Carver ws(workspace, workspace_bytes);
+  float* split_ws = ws.take<float>((int64_t)2 * 3 * d_in * d_out);
+  float* G = ws.take<float>((int64_t)g->V_dst * d_out);
+  float* dCat = ws.take<float>((int64_t)g->V_dst * 3 * d_in);
+  const int64_t ldc = 3 * (int64_t)d_in;
+  MARK("start");
+  // G = dOut * relu'(out) (the dropout is inside Cat);  db = column sums of G
+  float* dS = G;
+  rc = grad_prologue(dOut, out, nullptr, 1.f, relu, (int64_t)g->V_dst * d_out, G, dS, st);
+  if (!rc) rc = launch_diagcoef_colsum(G, g->V_dst, d_out, db, st);
+  if (rc) return rc;
+  MARK("grad_prologue_db");
+  // dW_cat = Cat^T G,  dCat = G W_cat^T
+  rc = gemm_any(st, split_ws, true, false, ldc, d_out, g->V_dst, Cat, ldc, G, d_out, 0.f, dW_cat, d_out);
+  if (!rc) rc = gemm_any(st, split_ws, false, true, g->V_dst, ldc, d_out, G, d_out, W_cat, d_out, 0.f, dCat, ldc);
+  if (rc) return rc;
+  MARK("compgcn_gemms_cat");
+  // dW_rel = Z^T dZ_next;  dZ = dZ_next W_rel^T, then the walk adds its terms
+  rc = gemm_any(st, split_ws, true, false, d_in, d_out, g->n_relw, Z, d_in, dZ_next, d_out, 0.f, dW_rel, d_out);
+  if (!rc) rc = gemm_any(st, split_ws, false, true, g->n_relw, d_in, d_out, dZ_next, d_out, W_rel, d_out, 0.f, dZ, d_in);
+  if (rc) return rc;
+  MARK("compgcn_gemms_rel");
+  rc = rgcn_check_cuda(cudaMemsetAsync(dz_loop, 0, (size_t)d_in * 4, st), "memset(dz_loop)");
+  if (!rc) rc = launch_zero_rows(dH, d_in, g->by_src.d_split_rows, (int)g->by_src.n_split, st);
+  if (!rc)
+    rc = launch_compgcn_bwd(composition, g->by_src.d_items, (int)g->by_src.n_items, g->by_src.d_nbr, g->by_src.d_relw,
+                            g->by_src.d_norm, dCat, H, Z, z_loop, d_in, g->n_relw, g->V_dst, drop_mask, 1.0f / keep,
+                            dH, dZ, dz_loop, st);
+  MARK("compgcn_walk_bwd");
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Highway skip connection (extras/highway_layer.py): one gate GEMM with the blend epilogue forward; an elementwise
 // prologue and two GEMMs backward
 // ------------------------------------------------------------------------------------------------

@@ -25,9 +25,9 @@
 // The NT and ensemble kernels are persistent (min(tiles, SMs) CTAs walk the tiles; the producer runs on into the next
 // tile while the consumers finish the last one); the TN kernel keeps one tile (x split-K) per CTA.
 //
-// The epilogues of the NT kernel are functors (StoreEpi, RankEpi, HighwayEpi, VarEpi, TopKEpi, BceEpi): a struct with
-// the epilogue's data and one operator()(tile, big, small) over the accumulator fragment.  Epilogue<EPI> maps the
-// integer of k_gemm_tf32x3<EPI> to its functor (EPI_STORE = 0 .. EPI_BCE = 5).  A new epilogue is one such struct, one
+// The epilogues of the NT kernel are functors (StoreEpi, BiasActEpi, RankEpi, HighwayEpi, VarEpi, TopKEpi, BceEpi): a
+// struct with the epilogue's data and one operator()(tile, big, small) over the accumulator fragment.  Epilogue<EPI>
+// maps the integer of k_gemm_tf32x3<EPI> to its functor (EPI_STORE = 0 .. EPI_BIAS_ACT = 6).  A new epilogue is one such struct, one
 // Epilogue<n> line and one launcher that ends in launch_persistent.  The two-member kernel k_gemm_ensemble<EPI> takes its
 // functor (EnsRankEpi, EnsTopKEpi) directly, over both members' accumulators.
 #include <cuda_runtime.h>
@@ -302,6 +302,34 @@ struct StoreEpi {
   }
 };
 
+// EPI = 6: BIAS + ACTIVATION epilogue (the CompGCN layer, compgcn.cu): C[M, N] = act(tile + bias[col]), act = ReLU
+// when `relu` is set, the identity otherwise.
+struct BiasActEpi {
+  float* C;                    // [M, ldc]
+  int64_t ldc;
+  const float* bias;           // [N]
+  int relu;
+
+  __device__ __forceinline__ void operator()(const TileCtx& t, const float (&big)[N_FRAG],
+                                             const float (&small)[N_FRAG]) const {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = t.r0 + 8 * h;
+      if (row >= t.M) continue;
+      float* crow = C + (size_t)row * ldc;
+      for_each_pair(t, h, [&](int r, int col) {
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(bias + col));
+        float2 o = make_float2(big[r] + small[r] + bb.x, big[r + 1] + small[r + 1] + bb.y);
+        if (relu) {
+          o.x = fmaxf(o.x, 0.f);
+          o.y = fmaxf(o.y, 0.f);
+        }
+        *reinterpret_cast<float2*>(crow + col) = o;
+      });
+    }
+  }
+};
+
 // EPI = 1: RANKING epilogue (all-entity scoring of the DistMult decoder, decoders/bilinear_diag.py:51-61, fused with
 // the rank counts of common/evaluation.py:148-159): the C tile is never written.  Row m of A is a query (e1*r or r*e2),
 // row n of Bt an entity code; each energy goes through the reference's float32 sigmoid and is compared with the gold
@@ -533,10 +561,11 @@ struct BceEpi {
 
 // k_gemm_tf32x3<EPI> runs the epilogue Epilogue<EPI>::type.  There is no primary definition: an integer without a
 // line here does not compile.
-enum : int { EPI_STORE = 0, EPI_RANK = 1, EPI_HIGHWAY = 2, EPI_VAR = 3, EPI_TOPK = 4, EPI_BCE = 5 };
+enum : int { EPI_STORE = 0, EPI_RANK = 1, EPI_HIGHWAY = 2, EPI_VAR = 3, EPI_TOPK = 4, EPI_BCE = 5, EPI_BIAS_ACT = 6 };
 template <int EPI>
 struct Epilogue;
 template <> struct Epilogue<EPI_STORE> { using type = StoreEpi; };
+template <> struct Epilogue<EPI_BIAS_ACT> { using type = BiasActEpi; };
 template <> struct Epilogue<EPI_RANK> { using type = RankEpi; };
 template <> struct Epilogue<EPI_HIGHWAY> { using type = HighwayEpi; };
 template <> struct Epilogue<EPI_VAR> { using type = VarEpi; };
@@ -1291,6 +1320,19 @@ int launch_gemm_tf32x3(const float* A, int64_t lda, const float* Bt_hi, const fl
   }
   return launch_nt<EPI_STORE>("gemm_tf32x3", "k_gemm_tf32x3", TILE_LIMIT, st, A, lda, Bt_hi, Bt_lo, ldb, M, N, K,
                               StoreEpi{C, ldc, accumulate});
+}
+
+// GEMM with the bias + activation epilogue (EPI = 6): C[M, N] = act(A[M, K] B + bias), B pre-split as Bt [N, K].
+int launch_gemm_bias_act_tf32x3(const float* A, int64_t lda, const float* Bt_hi, const float* Bt_lo, int64_t ldb,
+                                const float* bias, int relu, float* C, int64_t ldc, int M, int N, int K,
+                                cudaStream_t st) {
+  if (M == 0 || N == 0) return RGCN_OK;
+  if (K <= 0 || K % 4 != 0 || N % 4 != 0 || lda % 4 != 0 || ldb % 4 != 0 || ldc % 4 != 0) {
+    rgcn_set_error("gemm_bias_act_tf32x3: K > 0; K, N and leading dimensions must be multiples of 4");
+    return RGCN_ERR_INVALID;
+  }
+  return launch_nt<EPI_BIAS_ACT>("gemm_bias_act_tf32x3", "k_gemm_tf32x3<bias_act>", TILE_LIMIT, st, A, lda, Bt_hi,
+                                 Bt_lo, ldb, M, N, K, BiasActEpi{C, ldc, bias, relu});
 }
 
 // Scoring GEMM with the ranking epilogue: queries Q [M,K] against the pre-split entity codes Bt [N,K]; the counts

@@ -117,6 +117,22 @@ int launch_diaggcn_bwd(const WorkItem* items, int n_items, const int32_t* nbr, c
                        const float* G, const float* H, const float* Df, const float* Db, int d, int n_relw, float* dH,
                        float* dDf, float* dDb, float* sumsq2, cudaStream_t st);
 
+// compgcn.cu -- CompGCN layer (Name=compgcn); Z [2R][d] (weight id w reads Z[w]), phi = h (.) z (op 0, mult) or
+// h - z (op 1, sub).  Forward, destination-major view: Cat [V_dst, 3d] =
+//   [ mask / keep (.) A_f | mask / keep (.) A_b | phi(H[row], z_loop) ] / 3,   A_dir[row] = sum_m norm_m phi(H[src_m], Z[w_m])
+// (mask [V_dst, 2d] or null; split rows of Cat zeroed by the caller).
+int launch_compgcn_fwd(int op, const WorkItem* items, int n_items, const int32_t* nbr, const int32_t* relw,
+                       const float* norm, const float* H, const float* Z, const float* zloop, int d, int n_relw,
+                       const uint8_t* mask, float inv_keep, float* Cat, cudaStream_t st);
+// Backward, source-major view (rows = sources u), dCat = dL/dCat:  per (u, w) run S = sum_m norm_m dCat'_slab(w)[dst_m]
+// (dCat' = dCat with the mask / keep and the 1/3 of the forward), dH[u] = sum of the runs' phi_h^T S plus, for
+// u < V_dst, the loop term; dZ[w] and dz_loop accumulate the phi_z^T S terms (zeroed by the caller; split rows of dH
+// zeroed by the caller).
+int launch_compgcn_bwd(int op, const WorkItem* items, int n_items, const int32_t* nbr, const int32_t* relw,
+                       const float* norm, const float* dCat, const float* H, const float* Z, const float* zloop, int d,
+                       int n_relw, int V_dst, const uint8_t* mask, float inv_keep, float* dH, float* dZ,
+                       float* dzloop, cudaStream_t st);
+
 // Basis coefficient gradient (destination major):
 //   dC[w][b] += sum_{m into row, relw_m = w} norm_m * < H[src_m,:], dAgg[row][dir][:, b] >
 int launch_basis_dc(const AggLaunch& a, const float* dAgg, int B, int n_relw, float* dC,
@@ -148,6 +164,10 @@ int launch_gemm_split_b(const float* B, int64_t ldb, int N, int K, int transpose
                         cudaStream_t st);
 int launch_gemm_tf32x3(const float* A, int64_t lda, const float* Bt_hi, const float* Bt_lo, int64_t ldb,
                        float* C, int64_t ldc, int M, int N, int K, int accumulate, cudaStream_t st);
+// C = act(A Bt^T + bias), act = ReLU if relu, the identity otherwise; bias [N]
+int launch_gemm_bias_act_tf32x3(const float* A, int64_t lda, const float* Bt_hi, const float* Bt_lo, int64_t ldb,
+                                const float* bias, int relu, float* C, int64_t ldc, int M, int N, int K,
+                                cudaStream_t st);
 
 int launch_gemm_rank_tf32x3(const float* Q, int64_t ldq, const float* Bt_hi, const float* Bt_lo, int64_t ldb, int M,
                             int N, int K, const float* gold_sig, const int32_t* gold_col, const uint32_t* known,

@@ -456,6 +456,67 @@ def diag_layer(H, D_forward, D_backward, W_self, b, graph, drop_mask=None, keep=
     return _DiagLayerFn.apply(H, D_forward, D_backward, W_self, b, graph, drop_mask, keep, relu)
 
 
+COMPOSITIONS = ("mult", "sub")   # the composition codes of the library: RGCN_COMPOSITION_MULT = 0, _SUB = 1
+
+
+class _CompGcnLayerFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, H, Z, z_loop, W_cat, W_rel, b, graph, op, drop_mask, keep, relu):
+        if not (isinstance(H, torch.Tensor) and H.dim() == 2 and isinstance(W_cat, torch.Tensor) and W_cat.dim() == 2):
+            raise _lib.RgcnError("H must be a [V_src, d_in] tensor and W_cat a [3 d_in, d_out] tensor")
+        d_in, d_out = H.shape[1], W_cat.shape[1]
+        _check_cuda_f32("H", H, (graph.V_src, d_in))
+        _check_cuda_f32("Z", Z, (graph.n_relw, d_in))
+        _check_cuda_f32("z_loop", z_loop, (d_in,))
+        _check_cuda_f32("W_cat", W_cat, (3 * d_in, d_out))
+        _check_cuda_f32("W_rel", W_rel, (d_in, d_out))
+        _check_cuda_f32("b", b, (d_out,))
+        mask = _mask_arg(drop_mask, graph.V_dst, 2 * d_in)
+        dev = H.device
+        Cat = torch.empty(graph.V_dst, 3 * d_in, dtype=torch.float32, device=dev)
+        out = torch.empty(graph.V_dst, d_out, dtype=torch.float32, device=dev)
+        Z_next = torch.empty(graph.n_relw, d_out, dtype=torch.float32, device=dev)
+        _call("rgcn_compgcn_forward", "rgcn_compgcn_workspace_bytes", (graph.handle, d_in, d_out, 0),
+              (graph.handle, d_in, d_out, op, _ptr(H), _ptr(Z), _ptr(z_loop), _ptr(W_cat), _ptr(W_rel), _ptr(b),
+               _ptr(mask), float(keep), int(bool(relu)), _ptr(Cat), _ptr(out), _ptr(Z_next)), dev)
+        ctx.graph, ctx.op, ctx.keep, ctx.relu, ctx.mask = graph, op, float(keep), bool(relu), mask
+        ctx.save_for_backward(H, Z, z_loop, W_cat, W_rel, Cat, out)
+        return out, Z_next
+
+    @staticmethod
+    def backward(ctx, dOut, dZ_next):
+        H, Z, z_loop, W_cat, W_rel, Cat, out = ctx.saved_tensors
+        graph = ctx.graph
+        d_in, d_out = H.shape[1], W_cat.shape[1]
+        dOut, dZ_next = dOut.contiguous(), dZ_next.contiguous()
+        _check_cuda_f32("dOut", dOut, (graph.V_dst, d_out))
+        _check_cuda_f32("dZ_next", dZ_next, (graph.n_relw, d_out))
+        dev = H.device
+        dH, dZ, dz_loop = torch.empty_like(H), torch.empty_like(Z), torch.empty_like(z_loop)
+        dW_cat, dW_rel = torch.empty_like(W_cat), torch.empty_like(W_rel)
+        db = torch.empty(d_out, dtype=torch.float32, device=dev)
+        _call("rgcn_compgcn_backward", "rgcn_compgcn_workspace_bytes", (graph.handle, d_in, d_out, 1),
+              (graph.handle, d_in, d_out, ctx.op, _ptr(H), _ptr(Z), _ptr(z_loop), _ptr(W_cat), _ptr(W_rel),
+               _ptr(ctx.mask), ctx.keep, int(ctx.relu), _ptr(Cat), _ptr(out), _ptr(dOut), _ptr(dZ_next), _ptr(dH),
+               _ptr(dZ), _ptr(dz_loop), _ptr(dW_cat), _ptr(dW_rel), _ptr(db)), dev)
+        return dH, dZ, dz_loop, dW_cat, dW_rel, db, None, None, None, None, None
+
+
+def compgcn_layer(H, Z, z_loop, W_cat, W_rel, b, graph, composition="mult", drop_mask=None, keep=1.0, relu=True):
+    """CompGCN layer (Vashishth et al., ICLR 2020) as one library call each way.  A message s -> o of weight id w
+    (forward relation r: w = r, its inverse: w = R + r) is norm * phi(H[s], Z[w]) with phi = h * z ("mult") or
+    h - z ("sub"); with A_f / A_b the two directions' sums, L = phi(H[:V_dst], z_loop) and M the [V_dst, 2 d_in]
+    keep-mask,
+        out    = act([M * [A_f | A_b] / keep | L] / 3 @ W_cat + b),     W_cat = [W_I; W_O; W_S] : [3 d_in, d_out]
+        Z_next = Z @ W_rel.
+    Z : [2R, d_in], z_loop : [d_in], W_rel : [d_in, d_out].  Returns (out, Z_next), differentiable in H, Z, z_loop
+    and every weight."""
+    if composition not in COMPOSITIONS:
+        raise ValueError("composition must be one of %s, got %r" % (", ".join(COMPOSITIONS), composition))
+    return _CompGcnLayerFn.apply(H, Z, z_loop, W_cat, W_rel, b, graph, COMPOSITIONS.index(composition), drop_mask,
+                                 keep, relu)
+
+
 class _HighwayFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, c1, c2, W, b):
