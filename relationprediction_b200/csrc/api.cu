@@ -340,6 +340,11 @@ extern "C" int rgcn_gemm_tf32x3(const float* A, int64_t lda, const float* B, int
     rgcn_set_error("rgcn_gemm_tf32x3: bad arguments");
     return RGCN_ERR_INVALID;
   }
+  // the GEMM launcher's own checks, made before the split so that a refused call launches nothing
+  if (K % 4 != 0 || N % 4 != 0 || lda % 4 != 0 || ldc % 4 != 0) {
+    rgcn_set_error("rgcn_gemm_tf32x3: K, N, lda and ldc must be multiples of 4");
+    return RGCN_ERR_INVALID;
+  }
   if (workspace_bytes < (int64_t)2 * N * K * 4) {
     rgcn_set_error("rgcn_gemm_tf32x3: workspace too small (need 2*N*K floats)");
     return RGCN_ERR_WORKSPACE;
