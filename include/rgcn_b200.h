@@ -835,6 +835,73 @@ int rgcn_rotate_rank(const float* codes, const float* rel, int32_t V, int32_t Vr
                      int64_t n, int side, const uint32_t* known_mask, int32_t* raw_rank, int32_t* filtered_rank,
                      void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * TransE decoder (Bordes et al., NIPS 2013) with the L1 distance.  d % 4 == 0 is required (else RGCN_ERR_INVALID).
+ * Entity and relation rows are plain real vectors of d columns; all d columns of a relation row are used.  With
+ * h = codes[X[n,0]], r = rel[X[n,1]], t = codes[X[n,2]] and gamma the margin (finite, else RGCN_ERR_INVALID):
+ *
+ *   u_k = (h_k + r_k) - t_k  (each rounding pinned),   energy[n] = gamma - sum_k |u_k|
+ *   loss_out[0] = mean_n( (1-y)x + log1p(exp(-|x|)) + max(-x,0) )          (only if Y != NULL)
+ *   loss_out[1] = mean(h^2) + mean(r^2) + mean(t^2) over the gathered rows, each mean over N*d (un-scaled)
+ * Shapes, pointers and upstream gradients are those of rgcn_rotate_forward / rgcn_rotate_backward.  The backward
+ * ACCUMULATES (+=) into dcodes [V,d] and drel [Vrel,d], with s = sign(u) (0 where u = 0):
+ *   dE/dh = dE/dr = -s,  dE/dt = +s
+ * plus 2*g_reg*x/(N*d) on all three rows, and, when rel_slice_sumsq != NULL, adds to that device float the sum over
+ * triples of |dL/dr|^2 (the relation table's IndexedSlices term).
+ *
+ * rgcn_transe_self_adversarial_forward: rgcn_self_adversarial_forward for TransE (same layout, loss, coef, workspace
+ * rgcn_self_adversarial_workspace_bytes(N, K) and errors) with the L2 term above; its backward is rgcn_transe_backward
+ * with Y = NULL and g_energy = g_loss coef.
+ *
+ * Queries rank the rows of a table by L1 distance to one query row q: D_v = sum_k |q_k - v_k| in float32, summed in
+ * one fixed order for every candidate and the gold, so equal rows tie exactly.
+ *   rgcn_transe_rank / rgcn_transe_topk: the candidates are the V entities.  Side 1 (objects corrupted, gold t)
+ *     q = h + r; side 0 (subjects corrupted, gold h) q = t - r.
+ *   rgcn_transe_relation_rank / rgcn_transe_relation_topk: (h, ?, t) queries, q = t - h; the candidates are rel[0:R]
+ *     (1 <= R <= Vrel, else RGCN_ERR_INVALID), gold r = X[n,1] in [0, R).
+ * *_rank: raw_rank[t] = #{ v : D_v <= D_gold } (the gold always counts itself), filtered_rank[t] = raw_rank[t] -
+ *   #{ v in known(t) : D_v <= D_gold } + 1 (only when filtered_rank != NULL, which needs known_mask: uint32
+ *   [n, ceil(C/32)] device, C = V or R).  distmult_rank's counting rules on the distance: the ranks do not depend on
+ *   gamma.
+ * *_topk: the k candidates of smallest D per row, in ascending order of D, the smaller id first on ties, never one
+ *   whose bit is set in exclude_mask (uint32 [n, ceil(C/32)] device, or NULL); 1 <= k <= 128.  ids int32 [n, k] and
+ *   energies float32 [n, k] = gamma - D (rounded once) device; the tail of a row with fewer than k eligible candidates
+ *   is id -1, energy -inf.  The order is by D, so it is exact where two D round to the same energy.  The predicted
+ *   column of X is not read.  Bitwise repeatable.
+ * workspace : rgcn_transe_rank_workspace_bytes(V, d, n), rgcn_transe_topk_workspace_bytes(V, d, n, k),
+ *   rgcn_transe_relation_rank_workspace_bytes(R, d, n), rgcn_transe_relation_topk_workspace_bytes(R, d, n, k); the
+ *   top-k ones are linear in n (about 4 d + 8 k ceil(C/128) bytes per query).  No split: nothing to reuse.
+ * Errors, before any device work: RGCN_ERR_INVALID (null pointers, sizes, d % 4 != 0, gamma not finite, side, k, R,
+ * filtered ranks without a known mask, and those of rgcn_self_adversarial_forward), RGCN_ERR_WORKSPACE,
+ * RGCN_ERR_NODEVICE.  The *_workspace_bytes functions return RGCN_ERR_INVALID (-1) on bad arguments.
+ * ---------------------------------------------------------------------------------------------- */
+int rgcn_transe_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                        int64_t N, const float* Y, float gamma, float* energies, float* loss_out, void* stream);
+int rgcn_transe_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                         int64_t N, const float* Y, float gamma, const float* energies, float g_loss, float g_reg,
+                         const float* g_scale_dev, const float* g_energy, float* dcodes, float* drel,
+                         float* rel_slice_sumsq, void* stream);
+int rgcn_transe_self_adversarial_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                         const int32_t* X, int64_t N, int32_t K, float alpha, float gamma,
+                                         float* energies, float* coef, float* loss_out, void* workspace,
+                                         int64_t workspace_bytes, void* stream);
+int64_t rgcn_transe_rank_workspace_bytes(int32_t V, int32_t d, int64_t n);
+int rgcn_transe_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                     int64_t n, int side, const uint32_t* known_mask, int32_t* raw_rank, int32_t* filtered_rank,
+                     void* workspace, int64_t workspace_bytes, void* stream);
+int64_t rgcn_transe_topk_workspace_bytes(int32_t V, int32_t d, int64_t n, int32_t k);
+int rgcn_transe_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                     int64_t n, int side, int32_t k, const uint32_t* exclude_mask, float gamma, int32_t* ids,
+                     float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+int64_t rgcn_transe_relation_rank_workspace_bytes(int32_t R, int32_t d, int64_t n);
+int rgcn_transe_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                              const int32_t* X, int64_t n, const uint32_t* known_mask, int32_t* raw_rank,
+                              int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream);
+int64_t rgcn_transe_relation_topk_workspace_bytes(int32_t R, int32_t d, int64_t n, int32_t k);
+int rgcn_transe_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                              const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask, float gamma,
+                              int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- ConvE decoder (DESIGN.md section 1): query rows q = f(anchor row, relation row), energy <q, codes[v]> ----
  * A query (anchor a, relation r, side) reads codes[a] and rel[r] (side 1, object query (a, r, ?)) or rel_inv[r]
  * (side 0, subject query (?, r, a), the reciprocal relation).  f: the two rows reshaped to h x w (d = h w) and stacked into a

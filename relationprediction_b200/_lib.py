@@ -42,6 +42,10 @@ EXPORTED_SYMBOLS = [
     "rgcn_self_adversarial_workspace_bytes", "rgcn_self_adversarial_forward",
     "rgcn_rotate_forward", "rgcn_rotate_backward", "rgcn_rotate_self_adversarial_forward",
     "rgcn_rotate_rank_workspace_bytes", "rgcn_rotate_rank",
+    "rgcn_transe_forward", "rgcn_transe_backward", "rgcn_transe_self_adversarial_forward",
+    "rgcn_transe_rank_workspace_bytes", "rgcn_transe_rank", "rgcn_transe_topk_workspace_bytes", "rgcn_transe_topk",
+    "rgcn_transe_relation_rank_workspace_bytes", "rgcn_transe_relation_rank",
+    "rgcn_transe_relation_topk_workspace_bytes", "rgcn_transe_relation_topk",
     "rgcn_conve_one_to_n_workspace_bytes", "rgcn_conve_one_to_n", "rgcn_conve_one_to_n_finish_workspace_bytes",
     "rgcn_conve_one_to_n_finish", "rgcn_conve_query_rows_workspace_bytes", "rgcn_conve_query_rows",
     "rgcn_conve_rank_workspace_bytes", "rgcn_conve_rank", "rgcn_conve_topk_workspace_bytes", "rgcn_conve_topk",
@@ -301,6 +305,30 @@ def _declare(lib):
     lib.rgcn_rotate_rank.restype = c_int
     lib.rgcn_rotate_rank.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, vp, vp, vp, vp, c_int64,
                                      vp]
+    # TransE: the RotatE argument lists; top-k as distmult_topk without reuse_split, plus gamma
+    for fn in ("forward", "backward", "self_adversarial_forward"):
+        getattr(lib, "rgcn_transe_" + fn).restype = c_int
+        getattr(lib, "rgcn_transe_" + fn).argtypes = getattr(lib, "rgcn_rotate_" + fn).argtypes
+    lib.rgcn_transe_rank_workspace_bytes.restype = c_int64
+    lib.rgcn_transe_rank_workspace_bytes.argtypes = [c_int32, c_int32, c_int64]
+    lib.rgcn_transe_rank.restype = c_int
+    lib.rgcn_transe_rank.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, vp, vp, vp, vp, c_int64,
+                                     vp]
+    lib.rgcn_transe_topk_workspace_bytes.restype = c_int64
+    lib.rgcn_transe_topk_workspace_bytes.argtypes = [c_int32, c_int32, c_int64, c_int32]
+    lib.rgcn_transe_topk.restype = c_int
+    lib.rgcn_transe_topk.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, c_int32, vp, c_float, vp,
+                                     vp, vp, c_int64, vp]
+    lib.rgcn_transe_relation_rank_workspace_bytes.restype = c_int64
+    lib.rgcn_transe_relation_rank_workspace_bytes.argtypes = [c_int32, c_int32, c_int64]
+    lib.rgcn_transe_relation_rank.restype = c_int
+    lib.rgcn_transe_relation_rank.argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, vp, c_int64, vp, vp, vp, vp,
+                                              c_int64, vp]
+    lib.rgcn_transe_relation_topk_workspace_bytes.restype = c_int64
+    lib.rgcn_transe_relation_topk_workspace_bytes.argtypes = [c_int32, c_int32, c_int64, c_int32]
+    lib.rgcn_transe_relation_topk.restype = c_int
+    lib.rgcn_transe_relation_topk.argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, vp, c_int64, c_int32, vp,
+                                              c_float, vp, vp, vp, c_int64, vp]
     net, grads = POINTER(ConvENet), POINTER(ConvEGrads)
     lib.rgcn_conve_one_to_n_workspace_bytes.restype = c_int64
     lib.rgcn_conve_one_to_n_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_int64, c_int64]

@@ -5,13 +5,15 @@ which the reference does not have; they learn the relation codes), `gcn_basis` (
 when Concatenation=Yes, BasisGcnTimesDiag when DiagonalCoefficients=Yes; with UseInputTransform=No layer 0 is a one-hot
 BasisGcn; SkipConnections=Highway wraps every
 feature-input layer in a HighwayLayer), `embedding`, and the variational encoders `variational_embedding` and
-`variational_gcn_basis` (a VariationalEncoding over two linear AffineTransform heads); decoders `bilinear-diag`, `complex` and
-`rotate` (RotatE, which the reference does not have) and `conve` (ConvE, 1-N training only).  Unknown names return None exactly
+`variational_gcn_basis` (a VariationalEncoding over two linear AffineTransform heads); decoders `bilinear-diag`, `complex`,
+`rotate` (RotatE, which the reference does not have), `transe` (TransE, L1 distance; nor this) and `conve` (ConvE, 1-N
+training only).  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag, parse_training_objective
 from ..decoders.complex import Complex
 from ..decoders.conve import ConvE
 from ..decoders.rotate import Rotate
+from ..decoders.transe import TransE
 from ..encoders.affine_transform import AffineTransform
 from ..encoders.message_gcns.gcn_basis import BasisGcn
 from ..encoders.message_gcns.gcn_basis_concat import ConcatGcn
@@ -203,8 +205,8 @@ def build_decoder(encoder, decoder_settings):
         return ConvE(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
     if decoder_settings['Name'] not in ("bilinear-diag", "complex"):
         objective = parse_training_objective(decoder_settings)[0]
-        # RotatE trains under SelfAdversarial (the objective of its paper) but has no 1-N scoring GEMM
-        if objective != 'NegativeSampling' and not (decoder_settings['Name'] == "rotate"
+        # RotatE and TransE train under SelfAdversarial (the objective of the RotatE paper) but have no 1-N scoring GEMM
+        if objective != 'NegativeSampling' and not (decoder_settings['Name'] in ("rotate", "transe")
                                                     and objective == 'SelfAdversarial'):
             raise ValueError("TrainingObjective=%s needs the bilinear-diag or complex decoder, not %r"
                              % (objective, decoder_settings['Name']))
@@ -214,4 +216,6 @@ def build_decoder(encoder, decoder_settings):
         return Complex(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
     if decoder_settings['Name'] == "rotate":
         return Rotate(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
+    if decoder_settings['Name'] == "transe":
+        return TransE(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
     return None

@@ -2920,3 +2920,199 @@ extern "C" int rgcn_rotate_rank(const float* codes, const float* rel, int32_t V,
   if (!rc) rc = launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
   return rc;
 }
+
+// ------------------------------------------------------------------------------------------------
+// TransE (transe.cu): scorer, backward, self-adversarial forward, and ranking and top-k by L1 distance over all
+// entities or over the first R relations.  Every argument is checked before any device work, with RotatE's rules.
+// ------------------------------------------------------------------------------------------------
+extern "C" int rgcn_transe_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                   const int32_t* X, int64_t N, const float* Y, float gamma, float* energies,
+                                   float* loss_out, void* stream) {
+  const int rc = rotate_checks("rgcn_transe_forward", codes && rel && loss_out && (N <= 0 || (X && energies)), V, Vrel,
+                               d, N, gamma);
+  if (rc) return rc;
+  return launch_transe_forward(codes, rel, d, X, N, Y, gamma, energies, loss_out, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_transe_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                    const int32_t* X, int64_t N, const float* Y, float gamma, const float* energies,
+                                    float g_loss, float g_reg, const float* g_scale_dev, const float* g_energy,
+                                    float* dcodes, float* drel, float* rel_slice_sumsq, void* stream) {
+  const int rc = rotate_checks("rgcn_transe_backward",
+                               codes && rel && dcodes && drel && (N <= 0 || X) && (!Y || energies), V, Vrel, d, N,
+                               gamma);
+  if (rc) return rc;
+  return launch_transe_backward(codes, rel, d, X, N, Y, energies, g_loss, g_reg, g_scale_dev, g_energy, dcodes, drel,
+                                rel_slice_sumsq, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_transe_self_adversarial_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                                                    int32_t d, const int32_t* X, int64_t N, int32_t K, float alpha,
+                                                    float gamma, float* energies, float* coef, float* loss_out,
+                                                    void* workspace, int64_t workspace_bytes, void* stream) {
+  const std::string who = "rgcn_transe_self_adversarial_forward";
+  if (!std::isfinite(gamma)) {
+    rgcn_set_error(who + ": the margin gamma must be finite");
+    return RGCN_ERR_INVALID;
+  }
+  const int rc = self_adversarial_checks(
+      who, codes && rel && loss_out && workspace && (N <= 0 || (X && energies && coef)), V, Vrel, d, N, K, alpha,
+      workspace_bytes);
+  if (rc) return rc;
+  Carver ws(workspace, workspace_bytes);
+  float* parts = ws.take<float>(2 * (N / ((int64_t)K + 1)));
+  return launch_self_adversarial_forward(SELFADV_TRANSE, codes, rel, d, X, N, K, alpha, gamma, energies, coef,
+                                         loss_out, parts, (cudaStream_t)stream);
+}
+
+// Rank workspace: [Q n*d | gold_D n | gold_col n | raw_cnt n | known_cnt n] (rgcn_rotate_rank's); top-k workspace:
+// [Q n*d | cand n*ceil(C/128)*k (-D, id) pairs], C the candidate count (V or R).  No split: nothing to reuse.
+static bool transe_sizes_ok(int32_t C, int32_t d, int64_t n, int64_t per_row) {
+  return C > 0 && d > 0 && d % 4 == 0 && n >= 0 && (n == 0 || per_row <= ((int64_t)1 << 60) / n);
+}
+
+static int64_t transe_rank_bytes(const char* who, int32_t C, int32_t d, int64_t n) {
+  if (!transe_sizes_ok(C, d, n, (int64_t)d * 4 + 16)) {
+    rgcn_set_error(std::string(who) + ": bad arguments (need a candidate count > 0, d > 0, d % 4 == 0, n >= 0)");
+    return RGCN_ERR_INVALID;
+  }
+  return align_up(n * d * 4) + 4 * align_up(n * 4) + 256;
+}
+
+static int64_t transe_topk_bytes(const char* who, int32_t C, int32_t d, int64_t n, int32_t k) {
+  if (k < 1 || k > 128 || !transe_sizes_ok(C, d, n, (int64_t)d * 4 + (int64_t)transe_topk_tiles(C) * k * 8)) {
+    rgcn_set_error(std::string(who) + ": bad arguments (need a candidate count > 0, d > 0, d % 4 == 0, n >= 0, "
+                   "1 <= k <= 128)");
+    return RGCN_ERR_INVALID;
+  }
+  return align_up(n * d * 4) + align_up(n * transe_topk_tiles(C) * k * 8) + 256;
+}
+
+extern "C" int64_t rgcn_transe_rank_workspace_bytes(int32_t V, int32_t d, int64_t n) {
+  return transe_rank_bytes("rgcn_transe_rank_workspace_bytes", V, d, n);
+}
+
+extern "C" int64_t rgcn_transe_topk_workspace_bytes(int32_t V, int32_t d, int64_t n, int32_t k) {
+  return transe_topk_bytes("rgcn_transe_topk_workspace_bytes", V, d, n, k);
+}
+
+extern "C" int64_t rgcn_transe_relation_rank_workspace_bytes(int32_t R, int32_t d, int64_t n) {
+  return transe_rank_bytes("rgcn_transe_relation_rank_workspace_bytes", R, d, n);
+}
+
+extern "C" int64_t rgcn_transe_relation_topk_workspace_bytes(int32_t R, int32_t d, int64_t n, int32_t k) {
+  return transe_topk_bytes("rgcn_transe_relation_topk_workspace_bytes", R, d, n, k);
+}
+
+// The checks every TransE query entry point shares.  mode: 0 / 1 the entity side, TRANSE_RELATIONS relation queries
+// against rel[0:C] (C = R, 1 <= R <= Vrel); out = raw_rank or ids (and energies, `out2`).
+static int transe_query_checks(const std::string& who, const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                               int32_t C, int32_t d, const int32_t* X, int64_t n, int mode, const void* out,
+                               const void* out2, const void* workspace) {
+  if (!codes || !rel || !workspace || (n > 0 && (!X || !out || !out2))) {
+    rgcn_set_error(who + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 || n < 0 || n > 0x7fffffffLL || (mode != 0 && mode != 1 &&
+                                                                                     mode != TRANSE_RELATIONS)) {
+    rgcn_set_error(who + ": bad arguments (need V > 0, Vrel > 0, d % 4 == 0, 0 <= n < 2^31, side in {0,1})");
+    return RGCN_ERR_INVALID;
+  }
+  if (mode == TRANSE_RELATIONS && !relation_count_ok(who.c_str(), C, Vrel)) return RGCN_ERR_INVALID;
+  return RGCN_OK;
+}
+
+static int transe_rank_body(const std::string& who, const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                            int32_t C, int32_t d, const int32_t* X, int64_t n, int mode, const uint32_t* known_mask,
+                            int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                            cudaStream_t st) {
+  int rc = transe_query_checks(who, codes, rel, V, Vrel, C, d, X, n, mode, raw_rank, raw_rank, workspace);
+  if (rc) return rc;
+  if (filtered_rank && !known_mask) {
+    rgcn_set_error(who + ": bad arguments (filtered ranks need a known mask)");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < transe_rank_bytes(who.c_str(), C, d, n)) {
+    rgcn_set_error(who + ": workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who.c_str());
+  if (rc || n == 0) return rc;
+  Carver ws(workspace, workspace_bytes);
+  float* Q = ws.take<float>(n * d);
+  float* gold_D = ws.take<float>(n);
+  int32_t* gold_col = ws.take<int32_t>(n);
+  int32_t* raw_cnt = ws.take<int32_t>(n);
+  int32_t* known_cnt = ws.take<int32_t>(n);
+  rc = rgcn_check_cuda(cudaMemsetAsync(raw_cnt, 0, (char*)(known_cnt + n) - (char*)raw_cnt, st), "memset(rank counts)");
+  if (!rc) rc = launch_transe_prepare(codes, rel, d, X, n, mode, Q, gold_D, gold_col, st);
+  if (!rc)
+    rc = launch_transe_rank(Q, mode == TRANSE_RELATIONS ? rel : codes, C, d, n, gold_D, gold_col, known_mask, raw_cnt,
+                            known_cnt, st);
+  if (!rc) rc = launch_distmult_rank_finalize(raw_cnt, known_cnt, n, raw_rank, filtered_rank, st);
+  return rc;
+}
+
+static int transe_topk_body(const std::string& who, const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                            int32_t C, int32_t d, const int32_t* X, int64_t n, int mode, int32_t k,
+                            const uint32_t* exclude_mask, float gamma, int32_t* ids, float* energies, void* workspace,
+                            int64_t workspace_bytes, cudaStream_t st) {
+  int rc = transe_query_checks(who, codes, rel, V, Vrel, C, d, X, n, mode, ids, energies, workspace);
+  if (rc) return rc;
+  if (k < 1 || k > 128) {
+    rgcn_set_error(who + ": k = " + std::to_string(k) + " is out of range (1 <= k <= 128)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!std::isfinite(gamma)) {
+    rgcn_set_error(who + ": the margin gamma must be finite");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < transe_topk_bytes(who.c_str(), C, d, n, k)) {
+    rgcn_set_error(who + ": workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  rc = onen_device_checks(who.c_str());
+  if (rc || n == 0) return rc;
+  Carver ws(workspace, workspace_bytes);
+  float* Q = ws.take<float>(n * d);
+  uint2* cand = ws.take<uint2>(n * transe_topk_tiles(C) * k);
+  rc = launch_transe_prepare(codes, rel, d, X, n, mode, Q, nullptr, nullptr, st);
+  if (!rc)
+    rc = launch_transe_topk(Q, mode == TRANSE_RELATIONS ? rel : codes, C, d, n, exclude_mask, k, gamma, cand, ids,
+                            energies, st);
+  return rc;
+}
+
+extern "C" int rgcn_transe_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                const int32_t* X, int64_t n, int side, const uint32_t* known_mask,
+                                int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                                void* stream) {
+  if (side != 0 && side != 1) side = -1;   // refused by the shared checks
+  return transe_rank_body("rgcn_transe_rank", codes, rel, V, Vrel, V, d, X, n, side, known_mask, raw_rank,
+                          filtered_rank, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_transe_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                const int32_t* X, int64_t n, int side, int32_t k, const uint32_t* exclude_mask,
+                                float gamma, int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes,
+                                void* stream) {
+  if (side != 0 && side != 1) side = -1;
+  return transe_topk_body("rgcn_transe_topk", codes, rel, V, Vrel, V, d, X, n, side, k, exclude_mask, gamma, ids,
+                          energies, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_transe_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                         int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
+                                         int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
+                                         int64_t workspace_bytes, void* stream) {
+  return transe_rank_body("rgcn_transe_relation_rank", codes, rel, V, Vrel, R, d, X, n, TRANSE_RELATIONS, known_mask,
+                          raw_rank, filtered_rank, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_transe_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                         int32_t d, const int32_t* X, int64_t n, int32_t k,
+                                         const uint32_t* exclude_mask, float gamma, int32_t* ids, float* energies,
+                                         void* workspace, int64_t workspace_bytes, void* stream) {
+  return transe_topk_body("rgcn_transe_relation_topk", codes, rel, V, Vrel, R, d, X, n, TRANSE_RELATIONS, k,
+                          exclude_mask, gamma, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
+}

@@ -322,10 +322,10 @@ int launch_complex_relation_prepare(const float* codes, const float* rel, int d,
                                     float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
 
 // self_adversarial.cu -- self-adversarial objective over N = n (K + 1) triples in the sampler's layout (decoder: one of
-// the SELFADV_* kinds; gamma is read by RotatE only): energies [N], the energy-gradient coefficients coef [N],
+// the SELFADV_* kinds; gamma is read by RotatE and TransE only): energies [N], the energy-gradient coefficients coef [N],
 // loss_out[0] the loss, loss_out[1] the decoder's L2 term of its NegativeSampling forward; parts: 2n floats of scratch
 // for the per-group loss and norm parts
-enum { SELFADV_DISTMULT = 0, SELFADV_COMPLEX = 1, SELFADV_ROTATE = 2 };
+enum { SELFADV_DISTMULT = 0, SELFADV_COMPLEX = 1, SELFADV_ROTATE = 2, SELFADV_TRANSE = 3 };
 int launch_self_adversarial_forward(int decoder, const float* codes, const float* rel, int d, const int32_t* X,
                                     int64_t N, int K, float alpha, float gamma, float* energies, float* coef,
                                     float* loss_out, float* parts, cudaStream_t st);
@@ -345,6 +345,31 @@ int launch_rotate_rank_prepare(const float* codes, const float* rel, int d, cons
 int launch_rotate_rank(const float* Q, const float* codes, int V, int d, int64_t n, const float* gold_D,
                        const int32_t* gold_col, const uint32_t* known, int32_t* raw_cnt, int32_t* known_cnt,
                        cudaStream_t st);
+
+// transe.cu -- TransE (DESIGN.md section 1).  Scorer and backward: the contracts of the RotatE launchers; rows are
+// plain real vectors of d % 4 == 0 columns, all d columns of the relation row are used.
+int launch_transe_forward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                          float gamma, float* energies, float* loss_out, cudaStream_t st);
+int launch_transe_backward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                           const float* energies, float g_loss, float g_reg, const float* g_scale_dev,
+                           const float* g_energy, float* dcodes, float* drel, float* rel_slice_sumsq, cudaStream_t st);
+// query rows Q [n, d] of X: mode 1 (objects corrupted) codes[s] + rel[r], gold o; mode 0 (subjects corrupted)
+// codes[o] - rel[r], gold s; mode TRANSE_RELATIONS codes[o] - codes[s], gold r (the candidates are rel).  With gold_D,
+// also gold_D[t] = the gold's distance and gold_col[t] its id (gold_D == nullptr: Q only; the gold is not read).
+enum { TRANSE_RELATIONS = 2 };
+int launch_transe_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int mode,
+                          float* Q, float* gold_D, int32_t* gold_col, cudaStream_t st);
+// ranks against the first V rows of `table`: raw_cnt / known_cnt (zeroed by the caller) += the counts of
+// D_v <= gold_D (the gold always counts), known [n, ceil(V/32)] or nullptr
+int launch_transe_rank(const float* Q, const float* table, int V, int d, int64_t n, const float* gold_D,
+                       const int32_t* gold_col, const uint32_t* known, int32_t* raw_cnt, int32_t* known_cnt,
+                       cudaStream_t st);
+// top-k against the first V rows of `table`: ids [n, k] / energies [n, k] = gamma - D of every row's k smallest D, the
+// smaller id first on ties, never a column whose bit is set in excl [n, ceil(V/32)] (or nullptr); the tail (-1, -inf).
+// cand: n * transe_topk_tiles(V) * k candidates of scratch.
+inline int transe_topk_tiles(int V) { return (V + 127) / 128; }
+int launch_transe_topk(const float* Q, const float* table, int V, int d, int64_t n, const uint32_t* excl, int k,
+                       float gamma, uint2* cand, int32_t* ids, float* energies, cudaStream_t st);
 
 // conve.cu -- the ConvE query network (DESIGN.md section 1): d = h w, image 2h x w, C filters 3x3, F = C (2h-2)(w-2)
 // feature columns stored with leading dimension Fp (F rounded up to 4).  Masks are uint8 keep-masks or null.

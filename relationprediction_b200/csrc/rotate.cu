@@ -4,11 +4,12 @@
 //   u_k = a_k e^{i theta_k} - c_k,   D = sum_{k<h} |u_k|,   E = gamma - D.
 // The scorer and its backward have the ComplEx shape (a warp owns a triple, a lane the column pairs (k, k + h)).  The
 // ranking cannot be a GEMM -- a modulus is not a product -- so k_rotate_rank is a tiled all-pairs distance kernel on
-// the CUDA cores.
+// the CUDA cores: k_dist_tile (dist_tile.cuh) with RotatE's per-pair modulus.
 #include <cuda_runtime.h>
 
 #include <algorithm>
 
+#include "dist_tile.cuh"
 #include "kernels.cuh"
 #include "triple_rows.cuh"
 
@@ -127,19 +128,16 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// ---- all-entity ranking by distance -------------------------------------------------------------------------------
-// D = sum_k |q_k - v_k| in one fixed order: ascending k in chunks of RK_KC column pairs, each chunk summed from 0 by
-// rotate_dist_step and its sum added to the total, every rounding pinned (no contraction choice is left to the
-// compiler).  The gold's distance (k_rotate_rank_prepare) and every candidate's (k_rotate_rank) are formed this way on
-// one thread each, so the gold ties with itself -- and duplicated rows tie -- bit for bit; zero-padded columns add +0.
-// The chunked sum keeps the float32 error of D near 440 (d = 500) several times below that of one running sum, which
-// decides how many near-ties float32 ranks differently from float64.
-constexpr int RK_TILE = 128, RK_KC = 8, RK_LD = RK_TILE + 4;   // +4: spread the transposing writes over the banks
-constexpr int RK_STAGE = 2 * RK_KC * RK_LD;                    // floats of one operand's chunk
-
+// ---- all-entity ranking by distance (the tile kernel and its fixed summation order: dist_tile.cuh) -------------
 __device__ __forceinline__ float rotate_dist_step(float qr, float qi, float vr, float vi, float acc) {
   return __fadd_rn(acc, rotate_modulus(__fsub_rn(qr, vr), __fsub_rn(qi, vi)));
 }
+
+struct RotateStep {
+  __device__ __forceinline__ static float step(float qr, float qi, float vr, float vi, float acc) {
+    return rotate_dist_step(qr, qi, vr, vi, acc);
+  }
+};
 
 // One warp per query t.  side 1 (objects corrupted): q = codes[s] e^{i theta}, gold o; side 0 (subjects corrupted):
 // q = codes[o] e^{-i theta}, gold s -- |a e^{i theta} - c| = |a - c e^{-i theta}|.  Lane 0 then sums the gold's
@@ -185,124 +183,6 @@ __global__ void __launch_bounds__(256)
       gold_col[t] = gold;
     }
     __syncwarp();
-  }
-}
-
-// The tiled all-pairs distance kernel: a CTA owns 128 queries x 128 entities, 256 threads as a 16 x 16 grid, each
-// thread an 8 x 8 register tile (rows ty*4 + 64 i + a, columns tx*4 + 64 j + b, i, j < 2, a, b < 4).  The k range goes
-// in chunks of RK_KC column pairs; each chunk of both operands is staged k-major ([re 0..KC-1 | im 0..KC-1][row]) in
-// shared memory by 4-byte cp.async, double-buffered, with zero fill past n / V / h.  The epilogue counts, per query
-// row, the columns < V with D <= gold_D (or the gold itself), and among them the known ones; the 16 threads of a row
-// sum by shuffles and add once per row and CTA.
-
-__device__ __forceinline__ void cp_async4(float* dst, const float* src, bool valid) {
-  const unsigned saddr = (unsigned)__cvta_generic_to_shared(dst);
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(saddr), "l"(src), "r"(valid ? 4 : 0) : "memory");
-}
-
-// chunk k0 of rows row0.. of a [rows, d] operand into stage (thread tid copies 8 of its 128 x 16 floats)
-__device__ __forceinline__ void rk_load_chunk(float* stage, const float* __restrict__ A, int64_t rows, int64_t row0,
-                                              int d, int h, int k0, int tid) {
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const int e = tid + 256 * i, row = e >> 4, c = e & 15, kk = c & 7;
-    const int64_t gr = row0 + row;
-    const bool valid = gr < rows && k0 + kk < h;
-    const float* src = valid ? A + (size_t)gr * d + (c < RK_KC ? 0 : h) + k0 + kk : A;
-    cp_async4(stage + c * RK_LD + row, src, valid);
-  }
-}
-
-__global__ void __launch_bounds__(256, 1)
-    k_rotate_rank(const float* __restrict__ Q, const float* __restrict__ codes, int V, int d, int64_t n,
-                  const float* __restrict__ gold_D, const int32_t* __restrict__ gold_col,
-                  const uint32_t* __restrict__ known, int words, int32_t* __restrict__ raw_cnt,
-                  int32_t* __restrict__ known_cnt) {
-  __shared__ __align__(16) float sq[2][RK_STAGE];
-  __shared__ __align__(16) float sv[2][RK_STAGE];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int h = d >> 1, chunks = (h + RK_KC - 1) / RK_KC;
-  const int64_t col0 = (int64_t)blockIdx.x * RK_TILE;
-  for (int64_t row0 = (int64_t)blockIdx.y * RK_TILE; row0 < n; row0 += (int64_t)gridDim.y * RK_TILE) {
-    float acc[8][8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) acc[i][j] = 0.f;
-    rk_load_chunk(sq[0], Q, n, row0, d, h, 0, tid);
-    rk_load_chunk(sv[0], codes, V, col0, d, h, 0, tid);
-    asm volatile("cp.async.commit_group;" ::: "memory");
-    for (int c = 0; c < chunks; ++c) {
-      if (c + 1 < chunks) {
-        rk_load_chunk(sq[(c + 1) & 1], Q, n, row0, d, h, (c + 1) * RK_KC, tid);
-        rk_load_chunk(sv[(c + 1) & 1], codes, V, col0, d, h, (c + 1) * RK_KC, tid);
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-      asm volatile("cp.async.wait_group 1;" ::: "memory");
-      __syncthreads();
-      const float* a = sq[c & 1];
-      const float* b = sv[c & 1];
-      float part[8][8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) part[i][j] = 0.f;
-#pragma unroll 1
-      for (int kk = 0; kk < RK_KC; ++kk) {
-        float qr[8], qi[8], vr[8], vi[8];
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const float4 x = *reinterpret_cast<const float4*>(a + kk * RK_LD + ty * 4 + 64 * i);
-          const float4 y = *reinterpret_cast<const float4*>(a + (RK_KC + kk) * RK_LD + ty * 4 + 64 * i);
-          const float4 z = *reinterpret_cast<const float4*>(b + kk * RK_LD + tx * 4 + 64 * i);
-          const float4 w = *reinterpret_cast<const float4*>(b + (RK_KC + kk) * RK_LD + tx * 4 + 64 * i);
-          qr[4 * i] = x.x, qr[4 * i + 1] = x.y, qr[4 * i + 2] = x.z, qr[4 * i + 3] = x.w;
-          qi[4 * i] = y.x, qi[4 * i + 1] = y.y, qi[4 * i + 2] = y.z, qi[4 * i + 3] = y.w;
-          vr[4 * i] = z.x, vr[4 * i + 1] = z.y, vr[4 * i + 2] = z.z, vr[4 * i + 3] = z.w;
-          vi[4 * i] = w.x, vi[4 * i + 1] = w.y, vi[4 * i + 2] = w.z, vi[4 * i + 3] = w.w;
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-#pragma unroll
-          for (int j = 0; j < 8; ++j) part[i][j] = rotate_dist_step(qr[i], qi[i], vr[j], vi[j], part[i][j]);
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[i][j] = __fadd_rn(acc[i][j], part[i][j]);
-      __syncthreads();   // the buffer just read is the one the next iteration refills
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int64_t row = row0 + ty * 4 + 64 * (i >> 2) + (i & 3);
-      int raw = 0, kn = 0;
-      if (row < n) {
-        const float g = __ldg(gold_D + row);
-        const int gc = __ldg(gold_col + row);
-#pragma unroll
-        for (int jb = 0; jb < 2; ++jb) {
-          const int64_t cb = col0 + tx * 4 + 64 * jb;   // 4 columns in one 32-bit word of the mask
-          const uint32_t word = (known && cb < V) ? __ldg(known + (size_t)row * words + (cb >> 5)) : 0u;
-#pragma unroll
-          for (int b4 = 0; b4 < 4; ++b4) {
-            const int64_t col = cb + b4;
-            if (col < V && (acc[i][4 * jb + b4] <= g || col == gc)) {
-              ++raw;
-              kn += (int)((word >> (col & 31)) & 1u);
-            }
-          }
-        }
-      }
-#pragma unroll
-      for (int o = 1; o < 16; o <<= 1) {
-        raw += __shfl_xor_sync(FULL, raw, o);
-        kn += __shfl_xor_sync(FULL, kn, o);
-      }
-      if (tx == 0 && row < n) {
-        if (raw) atomicAdd(raw_cnt + row, raw);
-        if (kn) atomicAdd(known_cnt + row, kn);
-      }
-    }
   }
 }
 
@@ -358,7 +238,7 @@ int launch_rotate_rank(const float* Q, const float* codes, int V, int d, int64_t
                        const int32_t* gold_col, const uint32_t* known, int32_t* raw_cnt, int32_t* known_cnt,
                        cudaStream_t st) {
   if (n == 0) return RGCN_OK;
-  const dim3 grid((V + RK_TILE - 1) / RK_TILE, (unsigned)std::min<int64_t>((n + RK_TILE - 1) / RK_TILE, 65535));
-  k_rotate_rank<<<grid, 256, 0, st>>>(Q, codes, V, d, n, gold_D, gold_col, known, (V + 31) / 32, raw_cnt, known_cnt);
-  return check_launch("k_rotate_rank");
+  k_dist_tile<RotateStep, DistRankEpi><<<dist_tile_grid(V, n), 256, 0, st>>>(Q, codes, V, d, n, gold_D, gold_col, known,
+                                                                            (V + 31) / 32, raw_cnt, known_cnt);
+  return check_launch("k_dist_tile<rotate, rank>");
 }

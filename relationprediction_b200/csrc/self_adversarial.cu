@@ -1,5 +1,5 @@
-// self_adversarial.cu -- self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) for the DistMult, ComplEx
-// and RotatE decoders, sm_90a: the forward of the objective, which also writes each triple's energy gradient.
+// self_adversarial.cu -- self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) for the DistMult, ComplEx,
+// RotatE and TransE decoders, sm_90a: the forward of the objective, which also writes each triple's energy gradient.
 //
 // The fed triples follow the negative sampler's layout (auxilliaries.py:13-33): for N = n (K + 1) rows, rows 0..n-1
 // are the positives and row i + n j (j = 1..K) is the j-th corruption of positive i.  With s_i the positive's energy
@@ -34,7 +34,8 @@ __device__ __forceinline__ float sigmoid(float x) { return 1.f / (1.f + expf(-x)
 // over the corruptions; lane j % 32 stores energy j.  Pass 2 walks the group in strides of 32 -- so any K works -- and
 // every lane reads back only the energies it stored itself, forms p, the coefficient and its loss terms.  The loss and
 // the squared norms of the group's rows go to one part each per group, for a reduction in a fixed order.  `rows` is
-// the decoder's functor (RotateRows carries gamma); it comes last so the other parameters keep their offsets.
+// the decoder's functor (RotateRows and TransERows carry gamma); it comes last so the other parameters keep their
+// offsets.
 template <class Rows>
 __global__ void __launch_bounds__(256)
     k_selfadv_fwd(const float* __restrict__ codes, const float* __restrict__ rel, int d, const int32_t* __restrict__ X,
@@ -107,6 +108,9 @@ int launch_self_adversarial_forward(int decoder, const float* codes, const float
   else if (decoder == SELFADV_COMPLEX)
     k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
                                           ComplexRows<2>{});
+  else if (decoder == SELFADV_TRANSE)
+    k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
+                                          TransERows<4>{gamma});
   else if (d % 8 == 0)
     k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
                                           RotateRows<4>{gamma});

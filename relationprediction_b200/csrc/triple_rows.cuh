@@ -1,7 +1,7 @@
-// triple_rows.cuh -- the row arithmetic of the DistMult, ComplEx and RotatE triple scorers: one warp owns one triple
-// (s, r, o) and each lane forms its share of the energy and of the squared norms of the gathered rows.  Shared by
-// the NegativeSampling scorers (distmult.cu / complex.cu / rotate.cu) and the self-adversarial scorer
-// (self_adversarial.cu), so both objectives score a triple with the same float operations in the same order.
+// triple_rows.cuh -- the row arithmetic of the DistMult, ComplEx, RotatE and TransE triple scorers: one warp owns
+// one triple (s, r, o) and each lane forms its share of the energy and of the squared norms of the gathered rows.
+// Shared by the NegativeSampling scorers (distmult.cu / complex.cu / rotate.cu / transe.cu) and the self-adversarial
+// scorer (self_adversarial.cu), so both objectives score a triple with the same float operations in the same order.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -133,6 +133,35 @@ struct RotateRows {
         e -= rotate_modulus(ur, ui);
         q += ar[j] * ar[j] + ai[j] * ai[j];
         q += cr[j] * cr[j] + ci[j] * ci[j];
+      }
+    }
+  }
+};
+
+// TransE: u_k = (h_k + r_k) - t_k with both roundings pinned, so that the ranker's query row q = h + r (rounded once)
+// gives the same per-column term.  The scorer, its backward and the self-adversarial scorer all form u here.
+__device__ __forceinline__ float transe_residual(float h, float r, float t) { return __fsub_rn(__fadd_rn(h, r), t); }
+
+// TransE (DESIGN.md section 1): energy gamma - sum_k |h_k + r_k - t_k| over all d columns of plain real rows.  A lane
+// owns W consecutive columns (W = 4: d % 4 == 0 is required); lane 0's share carries gamma.  q gets the squared norms
+// of all three rows: a translation is regularised like a DistMult relation.
+template <int W>
+struct TransERows {
+  float gamma;
+
+  __device__ __forceinline__ void partial(const float* __restrict__ codes, const float* __restrict__ rel, int d, int s,
+                                          int r, int o, int lane, float& e, float& q) const {
+    const float* e1 = codes + (size_t)s * d;
+    const float* rr = rel + (size_t)r * d;
+    const float* e2 = codes + (size_t)o * d;
+    if (lane == 0) e += gamma;
+    for (int k = lane * W; k < d; k += 32 * W) {
+      float a[W], b[W], c[W];
+      Vec<W>::load(e1 + k, a), Vec<W>::load(rr + k, b), Vec<W>::load(e2 + k, c);
+#pragma unroll
+      for (int j = 0; j < W; ++j) {
+        e -= fabsf(transe_residual(a[j], b[j], c[j]));
+        q += a[j] * a[j] + b[j] * b[j] + c[j] * c[j];
       }
     }
   }

@@ -709,7 +709,7 @@ def complex_score(codes, rel, X, Y=None):
 def _check_gamma(gamma):
     gamma = float(gamma)
     if not np.isfinite(gamma):
-        raise ValueError("the RotatE margin gamma must be finite, got %r" % (gamma,))
+        raise ValueError("the margin gamma must be finite, got %r" % (gamma,))
     return gamma
 
 
@@ -732,10 +732,33 @@ def rotate_score(codes, rel, X, Y=None, *, gamma):
     return _RotateFn.apply(codes, rel, X, Y, _check_gamma(gamma))
 
 
-# decoder -> (the decoder kind of rgcn_self_adversarial_forward, or None: its own entry point; the scorer's backward)
+class _TransEFn(torch.autograd.Function):
+    """Returns (energies[N], loss, reg) of the TransE scorer, same conventions as _DistMultFn."""
+
+    @staticmethod
+    def forward(ctx, codes, rel, X, Y, gamma):
+        return _triple_forward(ctx, "rgcn_transe_forward", codes, rel, X, Y, (gamma,))
+
+    @staticmethod
+    def backward(ctx, g_energy, g_loss, g_reg):
+        return _triple_backward(ctx, "rgcn_transe_backward", g_energy, g_loss, g_reg) + (None,)
+
+
+def transe_score(codes, rel, X, Y=None, *, gamma):
+    """TransE energies gamma - sum_k |h_k + r_k - t_k| (plain real rows, all d columns of the relation row), the mean
+    sigmoid cross-entropy (0 if Y is None) and the L2 term mean(h^2) + mean(r^2) + mean(t^2) of the gathered rows
+    (include/rgcn_b200.h, rgcn_transe_forward)."""
+    return _TransEFn.apply(codes, rel, X, Y, _check_gamma(gamma))
+
+
+# decoder -> (the decoder kind of rgcn_self_adversarial_forward, or the name of the decoder's own entry point, which
+# takes the margin gamma; the scorer's backward)
 SELF_ADVERSARIAL_DECODERS = {"distmult": (_lib.RGCN_DECODER_DISTMULT, "distmult_backward_slices"),
                              "complex": (_lib.RGCN_DECODER_COMPLEX, "rgcn_complex_backward"),
-                             "rotate": (None, "rgcn_rotate_backward")}
+                             "rotate": ("rgcn_rotate_self_adversarial_forward", "rgcn_rotate_backward"),
+                             "transe": ("rgcn_transe_self_adversarial_forward", "rgcn_transe_backward")}
+# the decoders whose energy carries the margin gamma
+MARGIN_DECODERS = ("rotate", "transe")
 
 
 class _SelfAdversarialFn(torch.autograd.Function):
@@ -754,14 +777,13 @@ class _SelfAdversarialFn(torch.autograd.Function):
         loss2 = torch.empty(2, dtype=torch.float32, device=dev)
         rows = (_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, K, alpha)
         outs = (_ptr(energies), _ptr(coef), _ptr(loss2))
-        if kind is None:
-            _call("rgcn_rotate_self_adversarial_forward", "rgcn_self_adversarial_workspace_bytes", (N, K),
-                  rows + (gamma,) + outs, dev)
+        if isinstance(kind, str):
+            _call(kind, "rgcn_self_adversarial_workspace_bytes", (N, K), rows + (gamma,) + outs, dev)
         else:
             _call("rgcn_self_adversarial_forward", "rgcn_self_adversarial_workspace_bytes", (N, K),
                   (kind,) + rows + outs, dev)
         ctx.bwd = bwd
-        ctx.extra = () if kind is not None else (gamma,)
+        ctx.extra = (gamma,) if isinstance(kind, str) else ()
         ctx.rel_param = rel
         ctx.save_for_backward(codes, rel, X, coef)
         return loss2[0], loss2[1], energies
@@ -797,14 +819,14 @@ def self_adversarial_loss(codes, rel, X, K, alpha, decoder, *, gamma=None):
     the negative sampler's layout: rows 0..n-1 the positives, row i + n j (j = 1..K) the j-th corruption of positive i,
     N = n (K + 1).  Returns (loss, reg, energies): loss = 1/(2n) sum_i [softplus(-s_i) + sum_j p_ij softplus(s_ij)] with
     p_ij = softmax_j(alpha s_ij) held constant, reg = the decoder's L2 term over all N triples, energies [N].
-    decoder is "distmult", "complex" or "rotate"; gamma is the RotatE margin, needed by "rotate" only.
+    decoder is "distmult", "complex", "rotate" or "transe"; gamma is the margin, needed by "rotate" and "transe" only.
     Differentiable in codes and rel."""
     if decoder not in SELF_ADVERSARIAL_DECODERS:
         raise ValueError("self_adversarial_loss: decoder must be one of %s, got %r"
                          % (sorted(SELF_ADVERSARIAL_DECODERS), decoder))
-    if (decoder == "rotate") != (gamma is not None):
-        raise ValueError("self_adversarial_loss: the margin gamma goes with decoder 'rotate' only (got decoder %r, "
-                         "gamma %r)" % (decoder, gamma))
+    if (decoder in MARGIN_DECODERS) != (gamma is not None):
+        raise ValueError("self_adversarial_loss: the margin gamma goes with decoders 'rotate' and 'transe' only (got "
+                         "decoder %r, gamma %r)" % (decoder, gamma))
     if gamma is not None:
         gamma = _check_gamma(gamma)
     K, alpha = int(K), float(alpha)
@@ -1114,6 +1136,108 @@ class RotateRanker(object):
 
     def top_k_relations(self, X, k, exclude_mask=None):
         raise NotImplementedError("the RotatE decoder has no relation prediction")
+
+
+class TransERanker(object):
+    """Ranking and top-k of the TransE decoder by L1 distance (rgcn_transe_rank / _topk / _relation_rank /
+    _relation_topk), with DistMultRanker's interface: every query ranks the rows of a table by D = sum_k |q_k - v_k|,
+    D <= D_gold in place of score >= gold score, so the ranks do not depend on the margin.  top_k / top_k_relations
+    return the energies gamma - D of the k smallest D (gamma = 0: -D).  There is no split to reuse; queries go to the
+    library in chunks whose workspace stays under TOPK_CHUNK_BYTES.  No member of the fused ensemble."""
+    TOPK_CHUNK_BYTES = DistMultRanker.TOPK_CHUNK_BYTES
+
+    def __init__(self, codes, rel, relation_count=None, gamma=0.0):
+        _check_cuda_f32("codes", codes)
+        _check_cuda_f32("relation table", rel)
+        self.codes, self.rel = codes, rel
+        self.relation_count = rel.shape[0] if relation_count is None else int(relation_count)
+        self.gamma = _check_gamma(gamma)
+        self._ws = None
+
+    _check_rows = DistMultRanker._check_rows
+    _chunk_rows = DistMultRanker._chunk_rows
+
+    def _calls(self, X, mask, name, relations, workspace_bytes):
+        """Checks X and the mask ([n, ceil(V/32)], or [n, ceil(R/32)] for relation queries), sizes the workspace for
+        chunks of at most TOPK_CHUNK_BYTES, and yields (c0, c1) per chunk."""
+        if relations:
+            self._check_rows(X, mask, name, self.relation_count, "R")
+        else:
+            self._check_rows(X, mask, name)
+        n = X.shape[0]
+        chunk, nb = self._chunk_rows(n, workspace_bytes, "TransE workspace bytes")
+        if self._ws is None or self._ws.numel() < nb:
+            self._ws = _workspace(nb, self.codes.device)
+        for c0 in range(0, max(n, 1), chunk):
+            yield c0, min(n, c0 + chunk)
+
+    # lead: the arguments before X; side: () for relation queries, else (side,), which goes after n
+    def _rank(self, entry, X, known_mask, lead, side, workspace_bytes):
+        lib = _lib.load()
+        dev = self.codes.device
+        n = X.shape[0]
+        raw = torch.empty(n, dtype=torch.int32, device=dev)
+        filt = torch.empty(n, dtype=torch.int32, device=dev) if known_mask is not None else None
+        for c0, c1 in self._calls(X, known_mask, "known_mask", not side, workspace_bytes):
+            rc = getattr(lib, entry)(*lead, _ptr(X[c0:c1]), c1 - c0, *side,
+                                     _ptr(None if known_mask is None else known_mask[c0:c1]), _ptr(raw[c0:c1]),
+                                     _ptr(None if filt is None else filt[c0:c1]), _ptr(self._ws), self._ws.numel(),
+                                     _stream(dev))
+            _lib.check(rc, entry)
+        return raw, filt
+
+    def _top_k(self, entry, X, k, exclude_mask, lead, side, workspace_bytes):
+        lib = _lib.load()
+        dev = self.codes.device
+        k, n = int(k), X.shape[0]
+        ids = torch.empty((n, k), dtype=torch.int32, device=dev)
+        energies = torch.empty((n, k), dtype=torch.float32, device=dev)
+        for c0, c1 in self._calls(X, exclude_mask, "exclude_mask", not side, workspace_bytes):
+            rc = getattr(lib, entry)(*lead, _ptr(X[c0:c1]), c1 - c0, *side, k,
+                                     _ptr(None if exclude_mask is None else exclude_mask[c0:c1]), self.gamma,
+                                     _ptr(ids[c0:c1]), _ptr(energies[c0:c1]), _ptr(self._ws), self._ws.numel(),
+                                     _stream(dev))
+            _lib.check(rc, entry)
+        return ids, energies
+
+    def _lead(self, relations):
+        V, d = self.codes.shape
+        head = (_ptr(self.codes), _ptr(self.rel), V, self.rel.shape[0])
+        return head + ((self.relation_count, d) if relations else (d,))
+
+    def rank(self, X, side, known_mask=None):
+        """X int32 [n,3] CUDA; side 0 = subjects corrupted (q = t - r), 1 = objects (q = h + r); known_mask uint32
+        [n, ceil(V/32)] CUDA (as int32) or None.  Returns (raw_rank, filtered_rank or None) int32 CUDA tensors."""
+        lib = _lib.load()
+        V, d = self.codes.shape
+        return self._rank("rgcn_transe_rank", X, known_mask, self._lead(False), (int(side),),
+                          lambda m: lib.rgcn_transe_rank_workspace_bytes(V, d, m))
+
+    def top_k(self, X, side, k, exclude_mask=None):
+        """The k entities of smallest distance for every triple of X (side 0 predicts subjects, 1 objects; the
+        predicted column is not read), D ascending and the smaller id first on ties, never one whose bit is set in
+        exclude_mask (uint32 [n, ceil(V/32)] CUDA, as int32, or None).  Returns (ids int32 [n,k], energies
+        gamma - D float32 [n,k]) CUDA tensors; rows with fewer than k eligible entities end in (-1, -inf)."""
+        lib = _lib.load()
+        V, d = self.codes.shape
+        return self._top_k("rgcn_transe_topk", X, k, exclude_mask, self._lead(False), (int(side),),
+                           lambda m: lib.rgcn_transe_topk_workspace_bytes(V, d, m, int(k)))
+
+    def rank_relations(self, X, known_mask=None):
+        """Ranks of the relation X[t, 1] in [0, R) among rel[0:R] for the pair (X[t, 0], X[t, 2]), q = t - h, by the
+        rules of rank; known_mask uint32 [n, ceil(R/32)] CUDA (as int32) or None."""
+        lib = _lib.load()
+        R, d = self.relation_count, self.codes.shape[1]
+        return self._rank("rgcn_transe_relation_rank", X, known_mask, self._lead(True), (),
+                          lambda m: lib.rgcn_transe_relation_rank_workspace_bytes(R, d, m))
+
+    def top_k_relations(self, X, k, exclude_mask=None):
+        """The k relations of rel[0:R] of smallest distance for every pair (X[t, 0], ?, X[t, 2]) (the relation column
+        is not read), with top_k's order, exclusion and padding; exclude_mask uint32 [n, ceil(R/32)] CUDA or None."""
+        lib = _lib.load()
+        R, d = self.relation_count, self.codes.shape[1]
+        return self._top_k("rgcn_transe_relation_topk", X, k, exclude_mask, self._lead(True), (),
+                           lambda m: lib.rgcn_transe_relation_topk_workspace_bytes(R, d, m, int(k)))
 
 
 class EnsembleRanker(object):
