@@ -902,6 +902,73 @@ int rgcn_transe_relation_topk(const float* codes, const float* rel, int32_t V, i
                               const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask, float gamma,
                               int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * QuatE decoder (Zhang, Tay, Yao, Liu; NeurIPS 2019).  d % 4 == 0 is required (else RGCN_ERR_INVALID).  Quaternion k of
+ * a row x is x_k = (x[4k], x[4k+1], x[4k+2], x[4k+3]) = a + b i + c j + d k.  With h = codes[X[n,0]], r = rel[X[n,1]],
+ * t = codes[X[n,2]], (x) the Hamilton product and <.,.> the real 4-dot:
+ *
+ *   rh_k = r_k / max(|r_k|, 1e-12)       (IEEE-rounded sqrt and division)
+ *   energy[n] = sum_k <h_k (x) rh_k, t_k>  =  sum_k <h_k, t_k (x) conj(rh_k)>  =  sum_k <rh_k, conj(h_k) (x) t_k>
+ *   loss_out[0] = mean_n( (1-y)x + log1p(exp(-|x|)) + max(-x,0) )          (only if Y != NULL)
+ *   loss_out[1] = mean(h^2) + mean(r^2) + mean(t^2) over the gathered RAW rows, each mean over N*d (un-scaled)
+ * rgcn_quate_forward / rgcn_quate_backward: the shapes, pointers, upstream gradients and accumulation (+=) of
+ * distmult_forward / distmult_backward_slices.  The gradient of rh_k goes back to r_k as (g - rh_k <rh_k, g>) / |r_k|
+ * when |r_k| > 1e-12, else g / 1e-12: a zero quaternion never gives a NaN.
+ *
+ * rgcn_quate_self_adversarial_forward: rgcn_self_adversarial_forward for QuatE (no decoder kind, no margin; same
+ * layout, loss, coef, workspace rgcn_self_adversarial_workspace_bytes(N, K) and errors) with the L2 term above; its
+ * backward is rgcn_quate_backward with Y = NULL and g_energy = g_loss coef.
+ *
+ * The energy is linear in each row, so every query is one query row Q against a table, on the scoring GEMMs of
+ * DistMult with their counting, top-k and BCE rules:
+ *   rgcn_quate_rank / rgcn_quate_topk: distmult_rank / distmult_topk with side 1 (objects) Q = h (x) rh and side 0
+ *     (subjects) Q = t (x) conj(rh), against the V entities; workspaces distmult_rank_workspace_bytes and
+ *     rgcn_topk_workspace_bytes, reuse_split as there.
+ *   rgcn_quate_relation_rank / rgcn_quate_relation_topk: distmult_relation_rank / distmult_relation_topk with
+ *     Q = conj(h) (x) t against the normalised rows rh[0:R] (1 <= R <= Vrel); rows R..Vrel-1 are never normalised,
+ *     scored, counted or returned.  Workspaces rgcn_quate_relation_rank_workspace_bytes(R, d, n) and
+ *     rgcn_quate_relation_topk_workspace_bytes(R, d, n, k): the relation workspaces plus R*d floats for rh.  With
+ *     reuse_split, the normalised table and its split are those of the previous call on the same workspace.
+ *   rgcn_quate_one_to_n: distmult_one_to_n with these query rows (workspace rgcn_one_to_n_workspace_bytes); the L2
+ *     term is DistMult's, so rgcn_one_to_n_finish is its backward as it is.
+ *   rgcn_quate_query_rows: Q [n, d] (device) of the triples X for one side, the rows the entity ranks score.
+ * Errors, before any device work: RGCN_ERR_INVALID (null pointers, sizes, d % 4 != 0, side, k, R, filtered ranks
+ * without a known mask, and those of the DistMult entry points), RGCN_ERR_WORKSPACE, RGCN_ERR_NODEVICE (the scorer,
+ * backward, self-adversarial, 1-N and query-row entries).  The *_workspace_bytes functions return RGCN_ERR_INVALID (-1)
+ * on bad arguments.
+ * ---------------------------------------------------------------------------------------------- */
+int rgcn_quate_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                       int64_t N, const float* Y, float* energies, float* loss_out, void* stream);
+int rgcn_quate_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                        int64_t N, const float* Y, const float* energies, float g_loss, float g_reg,
+                        const float* g_scale_dev, const float* g_energy, float* dcodes, float* drel,
+                        float* rel_slice_sumsq, void* stream);
+int rgcn_quate_self_adversarial_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                        const int32_t* X, int64_t N, int32_t K, float alpha, float* energies,
+                                        float* coef, float* loss_out, void* workspace, int64_t workspace_bytes,
+                                        void* stream);
+int rgcn_quate_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                    int64_t n, int side, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
+                    int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream);
+int rgcn_quate_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                    int64_t n, int side, int32_t k, const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
+                    float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+int64_t rgcn_quate_relation_rank_workspace_bytes(int32_t R, int32_t d, int64_t n);
+int rgcn_quate_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                             const int32_t* X, int64_t n, const uint32_t* known_mask, int reuse_split,
+                             int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                             void* stream);
+int64_t rgcn_quate_relation_topk_workspace_bytes(int32_t R, int32_t d, int64_t n, int32_t k);
+int rgcn_quate_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                             const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask, int reuse_split,
+                             int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+int rgcn_quate_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                        const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
+                        const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk, void* workspace,
+                        int64_t workspace_bytes, void* stream);
+int rgcn_quate_query_rows(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                          int64_t n, int side, float* Q, void* stream);
+
 /* ---- ConvE decoder (DESIGN.md section 1): query rows q = f(anchor row, relation row), energy <q, codes[v]> ----
  * A query (anchor a, relation r, side) reads codes[a] and rel[r] (side 1, object query (a, r, ?)) or rel_inv[r]
  * (side 0, subject query (?, r, a), the reciprocal relation).  f: the two rows reshaped to h x w (d = h w) and stacked into a

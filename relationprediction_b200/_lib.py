@@ -46,6 +46,10 @@ EXPORTED_SYMBOLS = [
     "rgcn_transe_rank_workspace_bytes", "rgcn_transe_rank", "rgcn_transe_topk_workspace_bytes", "rgcn_transe_topk",
     "rgcn_transe_relation_rank_workspace_bytes", "rgcn_transe_relation_rank",
     "rgcn_transe_relation_topk_workspace_bytes", "rgcn_transe_relation_topk",
+    "rgcn_quate_forward", "rgcn_quate_backward", "rgcn_quate_self_adversarial_forward", "rgcn_quate_rank",
+    "rgcn_quate_topk", "rgcn_quate_relation_rank_workspace_bytes", "rgcn_quate_relation_rank",
+    "rgcn_quate_relation_topk_workspace_bytes", "rgcn_quate_relation_topk", "rgcn_quate_one_to_n",
+    "rgcn_quate_query_rows",
     "rgcn_conve_one_to_n_workspace_bytes", "rgcn_conve_one_to_n", "rgcn_conve_one_to_n_finish_workspace_bytes",
     "rgcn_conve_one_to_n_finish", "rgcn_conve_query_rows_workspace_bytes", "rgcn_conve_query_rows",
     "rgcn_conve_rank_workspace_bytes", "rgcn_conve_rank", "rgcn_conve_topk_workspace_bytes", "rgcn_conve_topk",
@@ -329,6 +333,23 @@ def _declare(lib):
     lib.rgcn_transe_relation_topk.restype = c_int
     lib.rgcn_transe_relation_topk.argtypes = [vp, vp, c_int32, c_int32, c_int32, c_int32, vp, c_int64, c_int32, vp,
                                               c_float, vp, vp, vp, c_int64, vp]
+    # QuatE: the DistMult argument lists; self-adversarial as rgcn_self_adversarial_forward without the decoder kind
+    lib.rgcn_quate_forward.restype = c_int
+    lib.rgcn_quate_forward.argtypes = lib.distmult_forward.argtypes
+    lib.rgcn_quate_backward.restype = c_int
+    lib.rgcn_quate_backward.argtypes = lib.distmult_backward_slices.argtypes
+    lib.rgcn_quate_self_adversarial_forward.restype = c_int
+    lib.rgcn_quate_self_adversarial_forward.argtypes = lib.rgcn_self_adversarial_forward.argtypes[1:]
+    for name, like in (("rgcn_quate_rank", "distmult_rank"), ("rgcn_quate_topk", "distmult_topk"),
+                       ("rgcn_quate_relation_rank", "distmult_relation_rank"),
+                       ("rgcn_quate_relation_topk", "distmult_relation_topk"),
+                       ("rgcn_quate_one_to_n", "distmult_one_to_n"),
+                       ("rgcn_quate_relation_rank_workspace_bytes", "rgcn_relation_rank_workspace_bytes"),
+                       ("rgcn_quate_relation_topk_workspace_bytes", "rgcn_relation_topk_workspace_bytes")):
+        getattr(lib, name).restype = getattr(lib, like).restype
+        getattr(lib, name).argtypes = getattr(lib, like).argtypes
+    lib.rgcn_quate_query_rows.restype = c_int
+    lib.rgcn_quate_query_rows.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, vp, vp]
     net, grads = POINTER(ConvENet), POINTER(ConvEGrads)
     lib.rgcn_conve_one_to_n_workspace_bytes.restype = c_int64
     lib.rgcn_conve_one_to_n_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_int64, c_int64]

@@ -3116,3 +3116,205 @@ extern "C" int rgcn_transe_relation_topk(const float* codes, const float* rel, i
   return transe_topk_body("rgcn_transe_relation_topk", codes, rel, V, Vrel, R, d, X, n, TRANSE_RELATIONS, k,
                           exclude_mask, gamma, ids, energies, workspace, workspace_bytes, (cudaStream_t)stream);
 }
+
+// ------------------------------------------------------------------------------------------------
+// QuatE (quate.cu): scorer, backward, self-adversarial forward, and the DistMult scoring GEMMs behind QuatE's query
+// rows: entity and relation ranks and top-k, 1-N training and the query rows of the score matrices.  Every argument is
+// checked before any device work.
+// ------------------------------------------------------------------------------------------------
+static int quate_checks(const std::string& who, bool pointers_ok, int32_t V, int32_t Vrel, int32_t d, int64_t N) {
+  if (!pointers_ok) {
+    rgcn_set_error(who + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 || N < 0) {
+    rgcn_set_error(who + ": bad sizes (need V > 0, Vrel > 0, d > 0, d % 4 == 0, N >= 0)");
+    return RGCN_ERR_INVALID;
+  }
+  return onen_device_checks(who.c_str());
+}
+
+extern "C" int rgcn_quate_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                  const int32_t* X, int64_t N, const float* Y, float* energies, float* loss_out,
+                                  void* stream) {
+  const int rc = quate_checks("rgcn_quate_forward", codes && rel && loss_out && (N <= 0 || (X && energies)), V, Vrel,
+                              d, N);
+  if (rc) return rc;
+  return launch_quate_forward(codes, rel, d, X, N, Y, energies, loss_out, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_quate_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                   const int32_t* X, int64_t N, const float* Y, const float* energies, float g_loss,
+                                   float g_reg, const float* g_scale_dev, const float* g_energy, float* dcodes,
+                                   float* drel, float* rel_slice_sumsq, void* stream) {
+  const int rc = quate_checks("rgcn_quate_backward",
+                              codes && rel && dcodes && drel && (N <= 0 || X) && (!Y || energies), V, Vrel, d, N);
+  if (rc) return rc;
+  return launch_quate_backward(codes, rel, d, X, N, Y, energies, g_loss, g_reg, g_scale_dev, g_energy, dcodes, drel,
+                               rel_slice_sumsq, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_quate_self_adversarial_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                                                   int32_t d, const int32_t* X, int64_t N, int32_t K, float alpha,
+                                                   float* energies, float* coef, float* loss_out, void* workspace,
+                                                   int64_t workspace_bytes, void* stream) {
+  const std::string who = "rgcn_quate_self_adversarial_forward";
+  const int rc = self_adversarial_checks(
+      who, codes && rel && loss_out && workspace && (N <= 0 || (X && energies && coef)), V, Vrel, d, N, K, alpha,
+      workspace_bytes);
+  if (rc) return rc;
+  Carver ws(workspace, workspace_bytes);
+  float* parts = ws.take<float>(2 * (N / ((int64_t)K + 1)));
+  return launch_self_adversarial_forward(SELFADV_QUATE, codes, rel, d, X, N, K, alpha, 0.f, energies, coef, loss_out,
+                                         parts, (cudaStream_t)stream);
+}
+
+// Entity queries: rank_with_queries / topk_with_queries with QuatE's query rows, in the DistMult workspaces
+// (distmult_rank_workspace_bytes, rgcn_topk_workspace_bytes), whose split of the codes is reused alike.
+extern "C" int rgcn_quate_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                               const int32_t* X, int64_t n, int side, const uint32_t* known_mask, int reuse_split,
+                               int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                               void* stream) {
+  return rank_with_queries("rgcn_quate_rank", launch_quate_rank_prepare, codes, V, distmult_rank_workspace_bytes, codes,
+                           rel, V, Vrel, d, X, n, side, known_mask, reuse_split, raw_rank, filtered_rank, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_quate_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                               const int32_t* X, int64_t n, int side, int32_t k, const uint32_t* exclude_mask,
+                               int reuse_split, int32_t* ids, float* energies, void* workspace,
+                               int64_t workspace_bytes, void* stream) {
+  return topk_with_queries("rgcn_quate_topk", launch_quate_rank_prepare, codes, V, rgcn_topk_workspace_bytes, codes,
+                           rel, V, Vrel, d, X, n, side, k, exclude_mask, reuse_split, ids, energies, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
+}
+
+// Relation queries: workspace [rh R*d | the workspace of rank_with_queries / topk_with_queries over rh].  Without
+// reuse_split, rel[0:R] is normalised into rh and rh is split; with it, both are those of the previous call on the
+// same workspace.
+extern "C" int64_t rgcn_quate_relation_rank_workspace_bytes(int32_t R, int32_t d, int64_t n) {
+  const int64_t rest = rgcn_relation_rank_workspace_bytes(R, d, n);
+  return rest < 0 ? rest : align_up((int64_t)R * d * 4) + rest;
+}
+
+extern "C" int64_t rgcn_quate_relation_topk_workspace_bytes(int32_t R, int32_t d, int64_t n, int32_t k) {
+  const int64_t rest = rgcn_relation_topk_workspace_bytes(R, d, n, k);
+  return rest < 0 ? rest : align_up((int64_t)R * d * 4) + rest;
+}
+
+// The checks of the two relation entry points that must come before the normalisation; rank_with_queries /
+// topk_with_queries then check the rest (all of them before their own device work).
+static int quate_relation_checks(const char* who, const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                                 int32_t R, int32_t d, const int32_t* X, int64_t n, const void* out, const void* out2,
+                                 const void* workspace, int64_t need, int64_t workspace_bytes) {
+  if (!codes || !rel || !workspace || (n > 0 && (!X || !out || !out2))) {
+    rgcn_set_error(std::string(who) + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (V <= 0 || Vrel <= 0 || d <= 0 || d % 4 != 0 || n < 0 || n > 0x7fffffffLL) {
+    rgcn_set_error(std::string(who) + ": bad arguments (need V > 0, Vrel > 0, d % 4 == 0, 0 <= n < 2^31)");
+    return RGCN_ERR_INVALID;
+  }
+  if (!relation_count_ok(who, R, Vrel)) return RGCN_ERR_INVALID;
+  if (need < 0) return (int)need;
+  if (workspace_bytes < need) {
+    rgcn_set_error(std::string(who) + ": workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  return RGCN_OK;
+}
+
+static int quate_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int,
+                                  float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st) {
+  return launch_quate_relation_prepare(codes, rel, d, X, n, Q, gold_sig, gold_col, st);
+}
+
+extern "C" int rgcn_quate_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                        int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
+                                        int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
+                                        int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_quate_relation_rank";
+  int rc = quate_relation_checks(who, codes, rel, V, Vrel, R, d, X, n, raw_rank, raw_rank, workspace,
+                                 rgcn_quate_relation_rank_workspace_bytes(R, d, n), workspace_bytes);
+  if (rc) return rc;
+  if (filtered_rank && !known_mask) {
+    rgcn_set_error(std::string(who) + ": bad arguments (filtered ranks need a known mask)");
+    return RGCN_ERR_INVALID;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver ws(workspace, workspace_bytes);
+  float* rh = ws.take<float>((int64_t)R * d);
+  if (!reuse_split) rc = launch_quate_normalize(rel, R, d, rh, st);
+  if (rc) return rc;
+  return rank_with_queries(who, quate_relation_prepare, rh, R, rgcn_relation_rank_workspace_bytes, codes, rel, V, Vrel,
+                           d, X, n, 0, known_mask, reuse_split, raw_rank, filtered_rank, ws.base + ws.off,
+                           workspace_bytes - ws.off, st);
+}
+
+extern "C" int rgcn_quate_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                        int32_t d, const int32_t* X, int64_t n, int32_t k,
+                                        const uint32_t* exclude_mask, int reuse_split, int32_t* ids, float* energies,
+                                        void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_quate_relation_topk";
+  if (k < 1 || k > 128) {
+    rgcn_set_error(std::string(who) + ": k = " + std::to_string(k) + " is out of range (1 <= k <= 128)");
+    return RGCN_ERR_INVALID;
+  }
+  int rc = quate_relation_checks(who, codes, rel, V, Vrel, R, d, X, n, ids, energies, workspace,
+                                 rgcn_quate_relation_topk_workspace_bytes(R, d, n, k), workspace_bytes);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  Carver ws(workspace, workspace_bytes);
+  float* rh = ws.take<float>((int64_t)R * d);
+  if (!reuse_split) rc = launch_quate_normalize(rel, R, d, rh, st);
+  if (rc) return rc;
+  return topk_with_queries(who, quate_relation_prepare, rh, R, rgcn_relation_topk_workspace_bytes, codes, rel, V, Vrel,
+                           d, X, n, 0, k, exclude_mask, reuse_split, ids, energies, ws.base + ws.off,
+                           workspace_bytes - ws.off, st);
+}
+
+// 1-N training: the one_to_n() body with QuatE's query rows and query backward, one launch per side run in a chunk.
+// The workspace is rgcn_one_to_n_workspace_bytes, and the backward of a call made with g_scale = (1, 0) is
+// rgcn_one_to_n_finish: the L2 term is DistMult's.
+extern "C" int rgcn_quate_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                                   const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
+                                   const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk,
+                                   void* workspace, int64_t workspace_bytes, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const OnenStep prepare = [=](const OnenChunk& k, float* Q) {
+    int rc = RGCN_OK;
+    for (const OnenRun& run : *k.runs) {
+      const int64_t b = std::max(run.begin, k.c0), e = std::min(run.end, k.c1);
+      if (!rc && b < e)
+        rc = launch_quate_rank_prepare(codes, rel, d, k.X + 3 * b, e - b, run.side, Q + (b - k.c0) * d, nullptr,
+                                       nullptr, st);
+    }
+    return rc;
+  };
+  const OnenStep query_bwd = [=](const OnenChunk& k, float* dQ) {
+    int rc = RGCN_OK;
+    for (const OnenRun& run : *k.runs) {
+      const int64_t b = std::max(run.begin, k.c0), e = std::min(run.end, k.c1);
+      if (!rc && b < e)
+        rc = launch_quate_query_bwd(codes, rel, d, k.X + 3 * b, e - b, run.side, dQ + (b - k.c0) * d, g_scale,
+                                    k.c_reg, dcodes, drel, st);
+    }
+    return rc;
+  };
+  return one_to_n("rgcn_quate_one_to_n", prepare, query_bwd, false, codes, rel, V, Vrel, R, d, queries, n, labels,
+                  smoothing, g_scale, loss, dcodes, drel, chunk, workspace, workspace_bytes, st);
+}
+
+// The query rows Q [n, d] of the triples X for one side (the rows the entity ranks score), for the [n, V] score
+// matrices.
+extern "C" int rgcn_quate_query_rows(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                     const int32_t* X, int64_t n, int side, float* Q, void* stream) {
+  const std::string who = "rgcn_quate_query_rows";
+  if (side != 0 && side != 1) {
+    rgcn_set_error(who + ": bad arguments (side in {0,1})");
+    return RGCN_ERR_INVALID;
+  }
+  const int rc = quate_checks(who, codes && rel && (n <= 0 || (X && Q)), V, Vrel, d, n);
+  if (rc) return rc;
+  return launch_quate_rank_prepare(codes, rel, d, X, n, side, Q, nullptr, nullptr, (cudaStream_t)stream);
+}

@@ -325,7 +325,7 @@ int launch_complex_relation_prepare(const float* codes, const float* rel, int d,
 // the SELFADV_* kinds; gamma is read by RotatE and TransE only): energies [N], the energy-gradient coefficients coef [N],
 // loss_out[0] the loss, loss_out[1] the decoder's L2 term of its NegativeSampling forward; parts: 2n floats of scratch
 // for the per-group loss and norm parts
-enum { SELFADV_DISTMULT = 0, SELFADV_COMPLEX = 1, SELFADV_ROTATE = 2, SELFADV_TRANSE = 3 };
+enum { SELFADV_DISTMULT = 0, SELFADV_COMPLEX = 1, SELFADV_ROTATE = 2, SELFADV_TRANSE = 3, SELFADV_QUATE = 4 };
 int launch_self_adversarial_forward(int decoder, const float* codes, const float* rel, int d, const int32_t* X,
                                     int64_t N, int K, float alpha, float gamma, float* energies, float* coef,
                                     float* loss_out, float* parts, cudaStream_t st);
@@ -370,6 +370,27 @@ int launch_transe_rank(const float* Q, const float* table, int V, int d, int64_t
 inline int transe_topk_tiles(int V) { return (V + 127) / 128; }
 int launch_transe_topk(const float* Q, const float* table, int V, int d, int64_t n, const uint32_t* excl, int k,
                        float gamma, uint2* cand, int32_t* ids, float* energies, cudaStream_t st);
+
+// quate.cu -- QuatE (DESIGN.md section 1).  Scorer and backward: the contracts of the DistMult launchers; quaternion k
+// of a row is the float4 at column 4k (d % 4 == 0), the relation quaternions are normalised before use.
+int launch_quate_forward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                         float* energies, float* loss_out, cudaStream_t st);
+int launch_quate_backward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                          const float* energies, float g_loss, float g_reg, const float* g_scale_dev,
+                          const float* g_energy, float* dcodes, float* drel, float* rel_slice_sumsq, cudaStream_t st);
+// entity query rows in launch_distmult_rank_prepare's contract: side 1 Q = h (x) rh, side 0 Q = t (x) conj(rh)
+int launch_quate_rank_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
+                              float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
+// rh [R, d] = the normalised quaternions of rel[0:R]: the candidates of the relation queries
+int launch_quate_normalize(const float* rel, int R, int d, float* rh, cudaStream_t st);
+// pair query rows in launch_distmult_relation_prepare's contract: Q = conj(h) (x) t, the gold scored against the
+// normalised rel[r]
+int launch_quate_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, float* Q,
+                                  float* gold_sig, int32_t* gold_col, cudaStream_t st);
+// 1-N query backward in launch_onen_query_bwd's contract (dQ is never null)
+int launch_quate_query_bwd(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
+                           const float* dQ, const float* g_scale, float c_reg, float* dcodes, float* drel,
+                           cudaStream_t st);
 
 // conve.cu -- the ConvE query network (DESIGN.md section 1): d = h w, image 2h x w, C filters 3x3, F = C (2h-2)(w-2)
 // feature columns stored with leading dimension Fp (F rounded up to 4).  Masks are uint8 keep-masks or null.

@@ -1,5 +1,6 @@
 // self_adversarial.cu -- self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) for the DistMult, ComplEx,
-// RotatE and TransE decoders, sm_90a: the forward of the objective, which also writes each triple's energy gradient.
+// RotatE, TransE and QuatE decoders, sm_90a: the forward of the objective, which also writes each triple's energy
+// gradient.
 //
 // The fed triples follow the negative sampler's layout (auxilliaries.py:13-33): for N = n (K + 1) rows, rows 0..n-1
 // are the positives and row i + n j (j = 1..K) is the j-th corruption of positive i.  With s_i the positive's energy
@@ -108,6 +109,9 @@ int launch_self_adversarial_forward(int decoder, const float* codes, const float
   else if (decoder == SELFADV_COMPLEX)
     k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
                                           ComplexRows<2>{});
+  else if (decoder == SELFADV_QUATE)
+    k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
+                                          QuatERows{});
   else if (decoder == SELFADV_TRANSE)
     k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
                                           TransERows<4>{gamma});

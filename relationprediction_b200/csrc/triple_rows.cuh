@@ -1,7 +1,8 @@
-// triple_rows.cuh -- the row arithmetic of the DistMult, ComplEx, RotatE and TransE triple scorers: one warp owns
-// one triple (s, r, o) and each lane forms its share of the energy and of the squared norms of the gathered rows.
-// Shared by the NegativeSampling scorers (distmult.cu / complex.cu / rotate.cu / transe.cu) and the self-adversarial
-// scorer (self_adversarial.cu), so both objectives score a triple with the same float operations in the same order.
+// triple_rows.cuh -- the row arithmetic of the DistMult, ComplEx, RotatE, TransE and QuatE triple scorers: one warp
+// owns one triple (s, r, o) and each lane forms its share of the energy and of the squared norms of the gathered rows.
+// Shared by the NegativeSampling scorers (distmult.cu / complex.cu / rotate.cu / transe.cu / quate.cu) and the
+// self-adversarial scorer (self_adversarial.cu), so both objectives score a triple with the same float operations in
+// the same order.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -163,6 +164,63 @@ struct TransERows {
         e -= fabsf(transe_residual(a[j], b[j], c[j]));
         q += a[j] * a[j] + b[j] * b[j] + c[j] * c[j];
       }
+    }
+  }
+};
+
+// QuatE (DESIGN.md section 1): quaternion k of a row is the aligned float4 at column 4k, (x, y, z, w) = a + b i + c j +
+// d k.  Every QuatE kernel -- scorer, backward, self-adversarial scorer, query rows, query backward -- forms the
+// Hamilton product and the normalised relation quaternion with these helpers, so they all use the same float
+// operations.
+constexpr float QUATE_EPS = 1e-12f;
+
+__device__ __forceinline__ float4 quat_conj(float4 q) { return make_float4(q.x, -q.y, -q.z, -q.w); }
+
+__device__ __forceinline__ float quat_dot(float4 p, float4 q, float acc) {
+  return fmaf(p.w, q.w, fmaf(p.z, q.z, fmaf(p.y, q.y, fmaf(p.x, q.x, acc))));
+}
+
+// the Hamilton product p q
+__device__ __forceinline__ float4 quat_mul(float4 p, float4 q) {
+  return make_float4(fmaf(p.x, q.x, -fmaf(p.y, q.y, fmaf(p.z, q.z, p.w * q.w))),
+                     fmaf(p.x, q.y, fmaf(p.y, q.x, fmaf(p.z, q.w, -(p.w * q.z)))),
+                     fmaf(p.x, q.z, fmaf(-p.y, q.w, fmaf(p.z, q.x, p.w * q.y))),
+                     fmaf(p.x, q.w, fmaf(p.y, q.z, fmaf(-p.z, q.y, p.w * q.x))));
+}
+
+// r / max(|r|, eps) with |r| in m.  IEEE-rounded square root and division: a quaternion whose norm is a power of two
+// normalises exactly.
+__device__ __forceinline__ float4 quat_normalize(float4 r, float& m) {
+  m = __fsqrt_rn(quat_dot(r, r, 0.f));
+  const float s = fmaxf(m, QUATE_EPS);
+  return make_float4(__fdiv_rn(r.x, s), __fdiv_rn(r.y, s), __fdiv_rn(r.z, s), __fdiv_rn(r.w, s));
+}
+
+// the gradient g with respect to rh = quat_normalize(r, m), taken back to r: (g - rh <rh, g>) / m when m > eps, else
+// g / eps (the clamped norm is then a constant), so a zero quaternion never gives a NaN
+__device__ __forceinline__ float4 quat_normalize_bwd(float4 rh, float m, float4 g) {
+  if (!(m > QUATE_EPS)) return make_float4(g.x / QUATE_EPS, g.y / QUATE_EPS, g.z / QUATE_EPS, g.w / QUATE_EPS);
+  const float c = quat_dot(rh, g, 0.f);
+  return make_float4(fmaf(-rh.x, c, g.x) / m, fmaf(-rh.y, c, g.y) / m, fmaf(-rh.z, c, g.z) / m,
+                     fmaf(-rh.w, c, g.w) / m);
+}
+
+// QuatE: e = sum_k <h_k (x) rh_k, t_k> with rh_k the normalised relation quaternion; a lane owns whole quaternions (one
+// float4 per row, d % 4 == 0).  q gets the squared norms of the three raw rows, DistMult's L2 term.
+struct QuatERows {
+  __device__ __forceinline__ static void partial(const float* __restrict__ codes, const float* __restrict__ rel, int d,
+                                                 int s, int r, int o, int lane, float& e, float& q) {
+    const float4* e1 = reinterpret_cast<const float4*>(codes + (size_t)s * d);
+    const float4* rr = reinterpret_cast<const float4*>(rel + (size_t)r * d);
+    const float4* e2 = reinterpret_cast<const float4*>(codes + (size_t)o * d);
+    const int d4 = d >> 2;
+    for (int i = lane; i < d4; i += 32) {
+      const float4 a = __ldg(e1 + i), b = __ldg(rr + i), c = __ldg(e2 + i);
+      float m;
+      e = quat_dot(quat_mul(a, quat_normalize(b, m)), c, e);
+      q += a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
+      q += b.x * b.x + b.y * b.y + b.z * b.z + b.w * b.w;
+      q += c.x * c.x + c.y * c.y + c.z * c.z + c.w * c.w;
     }
   }
 };

@@ -751,12 +751,32 @@ def transe_score(codes, rel, X, Y=None, *, gamma):
     return _TransEFn.apply(codes, rel, X, Y, _check_gamma(gamma))
 
 
+class _QuatEFn(torch.autograd.Function):
+    """Returns (energies[N], loss, reg) of the QuatE scorer, same conventions as _DistMultFn."""
+
+    @staticmethod
+    def forward(ctx, codes, rel, X, Y):
+        return _triple_forward(ctx, "rgcn_quate_forward", codes, rel, X, Y)
+
+    @staticmethod
+    def backward(ctx, g_energy, g_loss, g_reg):
+        return _triple_backward(ctx, "rgcn_quate_backward", g_energy, g_loss, g_reg)
+
+
+def quate_score(codes, rel, X, Y=None):
+    """QuatE energies sum_k <h_k (x) r_k / max(|r_k|, 1e-12), t_k> (quaternion k of a row: columns 4k..4k+3, (x) the
+    Hamilton product), the mean sigmoid cross-entropy (0 if Y is None) and DistMult's L2 term mean(h^2) + mean(r^2) +
+    mean(t^2) of the gathered raw rows (include/rgcn_b200.h, rgcn_quate_forward)."""
+    return _QuatEFn.apply(codes, rel, X, Y)
+
+
 # decoder -> (the decoder kind of rgcn_self_adversarial_forward, or the name of the decoder's own entry point, which
-# takes the margin gamma; the scorer's backward)
+# takes the margin gamma if the decoder is one of MARGIN_DECODERS; the scorer's backward)
 SELF_ADVERSARIAL_DECODERS = {"distmult": (_lib.RGCN_DECODER_DISTMULT, "distmult_backward_slices"),
                              "complex": (_lib.RGCN_DECODER_COMPLEX, "rgcn_complex_backward"),
                              "rotate": ("rgcn_rotate_self_adversarial_forward", "rgcn_rotate_backward"),
-                             "transe": ("rgcn_transe_self_adversarial_forward", "rgcn_transe_backward")}
+                             "transe": ("rgcn_transe_self_adversarial_forward", "rgcn_transe_backward"),
+                             "quate": ("rgcn_quate_self_adversarial_forward", "rgcn_quate_backward")}
 # the decoders whose energy carries the margin gamma
 MARGIN_DECODERS = ("rotate", "transe")
 
@@ -777,13 +797,14 @@ class _SelfAdversarialFn(torch.autograd.Function):
         loss2 = torch.empty(2, dtype=torch.float32, device=dev)
         rows = (_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), N, K, alpha)
         outs = (_ptr(energies), _ptr(coef), _ptr(loss2))
+        margin = (gamma,) if gamma is not None else ()
         if isinstance(kind, str):
-            _call(kind, "rgcn_self_adversarial_workspace_bytes", (N, K), rows + (gamma,) + outs, dev)
+            _call(kind, "rgcn_self_adversarial_workspace_bytes", (N, K), rows + margin + outs, dev)
         else:
             _call("rgcn_self_adversarial_forward", "rgcn_self_adversarial_workspace_bytes", (N, K),
                   (kind,) + rows + outs, dev)
         ctx.bwd = bwd
-        ctx.extra = (gamma,) if isinstance(kind, str) else ()
+        ctx.extra = margin
         ctx.rel_param = rel
         ctx.save_for_backward(codes, rel, X, coef)
         return loss2[0], loss2[1], energies
@@ -819,7 +840,8 @@ def self_adversarial_loss(codes, rel, X, K, alpha, decoder, *, gamma=None):
     the negative sampler's layout: rows 0..n-1 the positives, row i + n j (j = 1..K) the j-th corruption of positive i,
     N = n (K + 1).  Returns (loss, reg, energies): loss = 1/(2n) sum_i [softplus(-s_i) + sum_j p_ij softplus(s_ij)] with
     p_ij = softmax_j(alpha s_ij) held constant, reg = the decoder's L2 term over all N triples, energies [N].
-    decoder is "distmult", "complex", "rotate" or "transe"; gamma is the margin, needed by "rotate" and "transe" only.
+    decoder is "distmult", "complex", "rotate", "transe" or "quate"; gamma is the margin, needed by "rotate" and
+    "transe" only.
     Differentiable in codes and rel."""
     if decoder not in SELF_ADVERSARIAL_DECODERS:
         raise ValueError("self_adversarial_loss: decoder must be one of %s, got %r"
@@ -943,6 +965,8 @@ class DistMultRanker(object):
     workspaces start with the split)."""
     _RANK, _WORKSPACE, _TOPK = "distmult_rank", "distmult_rank_workspace_bytes", "distmult_topk"
     _REL_RANK, _REL_TOPK = "distmult_relation_rank", "distmult_relation_topk"
+    _REL_RANK_WORKSPACE = "rgcn_relation_rank_workspace_bytes"
+    _REL_TOPK_WORKSPACE = "rgcn_relation_topk_workspace_bytes"
     DECODER = _lib.RGCN_DECODER_DISTMULT   # the decoder kind of the ensemble entry point (rgcn_ensemble_rank)
     # device bytes one top_k / top_k_relations / rank_relations call may use beyond the split of its table; more
     # queries than fit go in several calls
@@ -1054,7 +1078,7 @@ class DistMultRanker(object):
         filt = torch.empty(n, dtype=torch.int32, device=dev) if known_mask is not None else None
         fn = getattr(lib, self._REL_RANK)
         for c0, c1 in self._relation_calls(X, known_mask, "known_mask",
-                                           lambda m: lib.rgcn_relation_rank_workspace_bytes(R, d, m)):
+                                           lambda m: getattr(lib, self._REL_RANK_WORKSPACE)(R, d, m)):
             rc = fn(_ptr(self.codes), _ptr(self.rel), self.codes.shape[0], self.rel.shape[0], R, d, _ptr(X[c0:c1]),
                     c1 - c0, _ptr(None if known_mask is None else known_mask[c0:c1]), int(self._rel_split_ready),
                     _ptr(raw[c0:c1]), _ptr(None if filt is None else filt[c0:c1]), _ptr(self._rel_ws),
@@ -1075,7 +1099,7 @@ class DistMultRanker(object):
         energies = torch.empty((n, k), dtype=torch.float32, device=dev)
         fn = getattr(lib, self._REL_TOPK)
         for c0, c1 in self._relation_calls(X, exclude_mask, "exclude_mask",
-                                           lambda m: lib.rgcn_relation_topk_workspace_bytes(R, d, m, k)):
+                                           lambda m: getattr(lib, self._REL_TOPK_WORKSPACE)(R, d, m, k)):
             rc = fn(_ptr(self.codes), _ptr(self.rel), self.codes.shape[0], self.rel.shape[0], R, d, _ptr(X[c0:c1]),
                     c1 - c0, k, _ptr(None if exclude_mask is None else exclude_mask[c0:c1]),
                     int(self._rel_split_ready), _ptr(ids[c0:c1]), _ptr(energies[c0:c1]), _ptr(self._rel_ws),
@@ -1090,6 +1114,45 @@ class ComplexRanker(DistMultRanker):
     _RANK, _WORKSPACE, _TOPK = "rgcn_complex_rank", "rgcn_complex_rank_workspace_bytes", "rgcn_complex_topk"
     _REL_RANK, _REL_TOPK = "rgcn_complex_relation_rank", "rgcn_complex_relation_topk"
     DECODER = _lib.RGCN_DECODER_COMPLEX
+
+
+class QuatERanker(object):
+    """Fused all-entity and all-relation ranking and top-k of the QuatE decoder (rgcn_quate_rank / _topk /
+    _relation_rank / _relation_topk): DistMultRanker's interface, workspaces and split reuse, with QuatE's query rows
+    (side 1 h (x) rh, side 0 t (x) conj(rh), relation pairs conj(h) (x) t against the normalised rel[0:R]).  Not a
+    DistMultRanker: it is no member of the fused ensemble, whose kernels score DistMult and ComplEx rows only."""
+    _RANK, _WORKSPACE, _TOPK = "rgcn_quate_rank", "distmult_rank_workspace_bytes", "rgcn_quate_topk"
+    _REL_RANK, _REL_TOPK = "rgcn_quate_relation_rank", "rgcn_quate_relation_topk"
+    _REL_RANK_WORKSPACE = "rgcn_quate_relation_rank_workspace_bytes"
+    _REL_TOPK_WORKSPACE = "rgcn_quate_relation_topk_workspace_bytes"
+    TOPK_CHUNK_BYTES = DistMultRanker.TOPK_CHUNK_BYTES
+
+    __init__ = DistMultRanker.__init__
+    _check_rows = DistMultRanker._check_rows
+    _chunk_rows = DistMultRanker._chunk_rows
+    _relation_calls = DistMultRanker._relation_calls
+    rank = DistMultRanker.rank
+    top_k = DistMultRanker.top_k
+    rank_relations = DistMultRanker.rank_relations
+    top_k_relations = DistMultRanker.top_k_relations
+
+
+def quate_query_rows(codes, rel, X, side):
+    """QuatE query rows Q [n, d] of the triples X (int32 [n, 3] CUDA): side 1 h (x) rh (scored against the objects),
+    side 0 t (x) conj(rh) (against the subjects); <Q[t], codes[v]> is the energy of the triple with v in the predicted
+    column (rgcn_quate_query_rows)."""
+    _check_cuda_f32("codes", codes)
+    _check_cuda_f32("relation table", rel)
+    if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
+        raise _lib.RgcnError("X must be a contiguous CUDA int32 [n,3] tensor")
+    V, d = codes.shape
+    n = X.shape[0]
+    Q = torch.empty((n, d), dtype=torch.float32, device=codes.device)
+    lib = _lib.load()
+    rc = lib.rgcn_quate_query_rows(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), n, int(side), _ptr(Q),
+                                   _stream(codes.device))
+    _lib.check(rc, "rgcn_quate_query_rows")
+    return Q
 
 
 class RotateRanker(object):
@@ -1400,7 +1463,8 @@ class EnsembleRanker(object):
 
 
 # ---- 1-N training (distmult_one_to_n / rgcn_complex_one_to_n, include/rgcn_b200.h) ----
-ONE_TO_N_DECODERS = {"distmult": "distmult_one_to_n", "complex": "rgcn_complex_one_to_n"}
+ONE_TO_N_DECODERS = {"distmult": "distmult_one_to_n", "complex": "rgcn_complex_one_to_n",
+                     "quate": "rgcn_quate_one_to_n"}
 # device bytes of the per-query buffers (energy gradients Gt [V, chunk], query rows and their gradients) of one
 # internal pass; more queries than fit run in several passes of one call
 ONE_TO_N_CHUNK_BYTES = 1 << 30
@@ -1469,9 +1533,9 @@ class OneToNLabels(object):
 
 
 class _OneToNFn(torch.autograd.Function):
-    """Returns (loss, reg) of distmult_one_to_n / rgcn_complex_one_to_n.  When codes or rel need a gradient, the forward
-    also writes the gradient of the loss alone (g_scale = (1, 0)); the gradient is linear in the two upstream scalars,
-    so the backward is rgcn_one_to_n_finish: one scaling pass and the L2 term, no GEMM."""
+    """Returns (loss, reg) of distmult_one_to_n / rgcn_complex_one_to_n / rgcn_quate_one_to_n.  When codes or rel
+    need a gradient, the forward also writes the gradient of the loss alone (g_scale = (1, 0)); the gradient is linear
+    in the two upstream scalars, so the backward is rgcn_one_to_n_finish: one scaling pass and the L2 term, no GEMM."""
 
     @staticmethod
     def forward(ctx, codes, rel, labels, queries, smoothing, entry, R, chunk, grads):
@@ -1511,8 +1575,8 @@ def one_to_n_loss(codes, rel, queries, labels, smoothing, decoder, relation_coun
     """1-N loss of host queries (anchor, relation, side) int32 [n, 3] against every entity, with the label bits of
     OneToNLabels.rows and label smoothing eps in [0, 1): returns (loss, reg), loss = the mean over the n V scores of the
     sigmoid cross-entropy against y' = (1 - eps) y + eps / V, reg = (|codes[anchor]|^2 + |rel[r]|^2) / (n d) summed
-    over the queries (the decoders' un-scaled L2 term).  decoder is "distmult" or "complex"; the relation ids must be
-    below relation_count (default: all rows of rel).  Differentiable in codes and rel."""
+    over the queries (the decoders' un-scaled L2 term).  decoder is "distmult", "complex" or "quate"; the relation ids
+    must be below relation_count (default: all rows of rel).  Differentiable in codes and rel."""
     if decoder not in ONE_TO_N_DECODERS:
         raise ValueError("one_to_n_loss: decoder must be one of %s, got %r" % (sorted(ONE_TO_N_DECODERS), decoder))
     _check_cuda_f32("codes", codes)
