@@ -969,6 +969,81 @@ int rgcn_quate_one_to_n(const float* codes, const float* rel, int32_t V, int32_t
 int rgcn_quate_query_rows(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
                           int64_t n, int side, float* Q, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * HolE decoder (Nickel, Rosasco, Poggio; AAAI 2016).  d % 4 == 0 is required (else RGCN_ERR_INVALID).  With h, r, t
+ * the RAW rows of a triple, the energy is the circular correlation read by the relation:
+ *
+ *   E = sum_k r_k [h * t]_k,   [h * t]_k = sum_i h_i t_{(i + k) mod d}   ( = <r, irfft(conj(rfft(h)) rfft(t))> )
+ *
+ * Every entry point below except rgcn_hole_transform takes TRANSFORMED tables x~ = x U and returns gradients with
+ * respect to them.  U [d, d] is the orthonormal real DFT basis with interleaved columns: column 0 = 1/sqrt(d) (DC),
+ * column 1 = (-1)^k / sqrt(d) (Nyquist), columns 2f, 2f+1 = sqrt(2/d) (cos, -sin)(2 pi f k / d), f = 1 .. d/2 - 1.
+ * With x~_f = x~[2f] + i x~[2f+1]:
+ *
+ *   E = sqrt(d) (h~0 r~0 t~0 + h~1 r~1 t~1) + sqrt(d/2) sum_f Re(conj(h~_f r~_f) t~_f).
+ *
+ * U is orthogonal, so a caller that transforms its tables, runs these entry points and takes the gradients back with
+ * g U^T gets the raw rows' energies, L2 term and gradients, and the same relation slice norms.
+ *
+ * rgcn_hole_transform: out [rows, d] = x U (inverse = 0) or x U^T (inverse = 1), one 3xTF32 GEMM.  basis is a device
+ *   buffer of d*d floats: unless basis_ready, U is first built into it (in double precision, rounded once); with
+ *   basis_ready it is the U of an earlier call.  out must not alias x.  Workspace rgcn_hole_transform_workspace_bytes(d).
+ * rgcn_hole_forward / rgcn_hole_backward: the shapes, pointers, upstream gradients and accumulation (+=) of
+ *   distmult_forward / distmult_backward_slices; loss_out[1] = mean(h~^2) + mean(r~^2) + mean(t~^2) over the gathered
+ *   rows, DistMult's L2 term.
+ * rgcn_hole_self_adversarial_forward: rgcn_self_adversarial_forward for HolE (no decoder kind, no margin; same layout,
+ *   loss, coef, workspace rgcn_self_adversarial_workspace_bytes(N, K) and errors); its backward is rgcn_hole_backward
+ *   with Y = NULL and g_energy = g_loss coef.
+ *
+ * The energy is linear in each row, so every query is one query row Q against a table, on the scoring GEMMs of
+ * DistMult with their counting, top-k and BCE rules (w = sqrt(d) on DC and Nyquist, sqrt(d/2) on every pair):
+ *   rgcn_hole_rank / rgcn_hole_topk: distmult_rank / distmult_topk with side 1 (objects) Q = w (h~ r~) and side 0
+ *     (subjects) Q = w conj(r~) t~, against the V entities; workspaces distmult_rank_workspace_bytes and
+ *     rgcn_topk_workspace_bytes, reuse_split as there.
+ *   rgcn_hole_relation_rank / rgcn_hole_relation_topk: distmult_relation_rank / distmult_relation_topk with
+ *     Q = w conj(h~) t~ against r~[0:R] (1 <= R <= Vrel); rows R..Vrel-1 are never scored, counted or returned.
+ *     Workspaces rgcn_relation_rank_workspace_bytes and rgcn_relation_topk_workspace_bytes.
+ *   rgcn_hole_one_to_n: distmult_one_to_n with these query rows (workspace rgcn_one_to_n_workspace_bytes); the L2 term
+ *     is DistMult's, so rgcn_one_to_n_finish is its backward as it is.
+ *   rgcn_hole_query_rows: Q [n, d] (device) of the triples X for one side, the rows the entity ranks score.
+ * Errors, before any device work: RGCN_ERR_INVALID (null pointers, sizes, d % 4 != 0, side, k, R, inverse, filtered
+ * ranks without a known mask, and those of the DistMult entry points), RGCN_ERR_WORKSPACE, RGCN_ERR_NODEVICE (the
+ * transform, scorer, backward, self-adversarial, 1-N and query-row entries).  rgcn_hole_transform_workspace_bytes
+ * returns RGCN_ERR_INVALID (-1) on bad arguments.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t rgcn_hole_transform_workspace_bytes(int32_t d);
+int rgcn_hole_transform(const float* x, int64_t rows, int32_t d, int inverse, float* basis, int basis_ready, float* out,
+                        void* workspace, int64_t workspace_bytes, void* stream);
+int rgcn_hole_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                      int64_t N, const float* Y, float* energies, float* loss_out, void* stream);
+int rgcn_hole_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                       int64_t N, const float* Y, const float* energies, float g_loss, float g_reg,
+                       const float* g_scale_dev, const float* g_energy, float* dcodes, float* drel,
+                       float* rel_slice_sumsq, void* stream);
+int rgcn_hole_self_adversarial_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                       const int32_t* X, int64_t N, int32_t K, float alpha, float* energies,
+                                       float* coef, float* loss_out, void* workspace, int64_t workspace_bytes,
+                                       void* stream);
+int rgcn_hole_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                   int64_t n, int side, const uint32_t* known_mask, int reuse_split, int32_t* raw_rank,
+                   int32_t* filtered_rank, void* workspace, int64_t workspace_bytes, void* stream);
+int rgcn_hole_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                   int64_t n, int side, int32_t k, const uint32_t* exclude_mask, int reuse_split, int32_t* ids,
+                   float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+int rgcn_hole_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                            const int32_t* X, int64_t n, const uint32_t* known_mask, int reuse_split,
+                            int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                            void* stream);
+int rgcn_hole_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                            const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask, int reuse_split,
+                            int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes, void* stream);
+int rgcn_hole_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                       const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
+                       const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk, void* workspace,
+                       int64_t workspace_bytes, void* stream);
+int rgcn_hole_query_rows(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d, const int32_t* X,
+                         int64_t n, int side, float* Q, void* stream);
+
 /* ---- ConvE decoder (DESIGN.md section 1): query rows q = f(anchor row, relation row), energy <q, codes[v]> ----
  * A query (anchor a, relation r, side) reads codes[a] and rel[r] (side 1, object query (a, r, ?)) or rel_inv[r]
  * (side 0, subject query (?, r, a), the reciprocal relation).  f: the two rows reshaped to h x w (d = h w) and stacked into a

@@ -50,6 +50,9 @@ EXPORTED_SYMBOLS = [
     "rgcn_quate_topk", "rgcn_quate_relation_rank_workspace_bytes", "rgcn_quate_relation_rank",
     "rgcn_quate_relation_topk_workspace_bytes", "rgcn_quate_relation_topk", "rgcn_quate_one_to_n",
     "rgcn_quate_query_rows",
+    "rgcn_hole_transform_workspace_bytes", "rgcn_hole_transform", "rgcn_hole_forward", "rgcn_hole_backward",
+    "rgcn_hole_self_adversarial_forward", "rgcn_hole_rank", "rgcn_hole_topk", "rgcn_hole_relation_rank",
+    "rgcn_hole_relation_topk", "rgcn_hole_one_to_n", "rgcn_hole_query_rows",
     "rgcn_conve_one_to_n_workspace_bytes", "rgcn_conve_one_to_n", "rgcn_conve_one_to_n_finish_workspace_bytes",
     "rgcn_conve_one_to_n_finish", "rgcn_conve_query_rows_workspace_bytes", "rgcn_conve_query_rows",
     "rgcn_conve_rank_workspace_bytes", "rgcn_conve_rank", "rgcn_conve_topk_workspace_bytes", "rgcn_conve_topk",
@@ -350,6 +353,18 @@ def _declare(lib):
         getattr(lib, name).argtypes = getattr(lib, like).argtypes
     lib.rgcn_quate_query_rows.restype = c_int
     lib.rgcn_quate_query_rows.argtypes = [vp, vp, c_int32, c_int32, c_int32, vp, c_int64, c_int, vp, vp]
+    # HolE: the QuatE argument lists (on transformed tables), plus the basis transform
+    for name in ("forward", "backward", "self_adversarial_forward", "rank", "topk", "one_to_n", "query_rows"):
+        getattr(lib, "rgcn_hole_" + name).restype = getattr(lib, "rgcn_quate_" + name).restype
+        getattr(lib, "rgcn_hole_" + name).argtypes = getattr(lib, "rgcn_quate_" + name).argtypes
+    for name, like in (("rgcn_hole_relation_rank", "distmult_relation_rank"),
+                       ("rgcn_hole_relation_topk", "distmult_relation_topk")):
+        getattr(lib, name).restype = getattr(lib, like).restype
+        getattr(lib, name).argtypes = getattr(lib, like).argtypes
+    lib.rgcn_hole_transform_workspace_bytes.restype = c_int64
+    lib.rgcn_hole_transform_workspace_bytes.argtypes = [c_int32]
+    lib.rgcn_hole_transform.restype = c_int
+    lib.rgcn_hole_transform.argtypes = [vp, c_int64, c_int32, c_int, vp, c_int, vp, vp, c_int64, vp]
     net, grads = POINTER(ConvENet), POINTER(ConvEGrads)
     lib.rgcn_conve_one_to_n_workspace_bytes.restype = c_int64
     lib.rgcn_conve_one_to_n_workspace_bytes.argtypes = [c_int32, c_int32, c_int32, c_int32, c_int32, c_int64, c_int64]

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "librgcn_b200.so")
-SOURCES = ["graph.cu", "graph_device.cu", "rgcn_kernels.cu", "gemm_tf32x3.cu", "distmult.cu", "complex.cu", "basis_onehot.cu", "basis_diagcoef.cu", "gcn_diag.cu", "compgcn.cu", "highway.cu", "variational.cu", "topk.cu", "onen.cu", "self_adversarial.cu", "rotate.cu", "transe.cu", "quate.cu", "conve.cu", "sampler.cu", "optimizer.cu", "block_staged.cu", "slice_norm.cu", "api.cu"]
+SOURCES = ["graph.cu", "graph_device.cu", "rgcn_kernels.cu", "gemm_tf32x3.cu", "distmult.cu", "complex.cu", "basis_onehot.cu", "basis_diagcoef.cu", "gcn_diag.cu", "compgcn.cu", "highway.cu", "variational.cu", "topk.cu", "onen.cu", "self_adversarial.cu", "rotate.cu", "transe.cu", "quate.cu", "hole.cu", "conve.cu", "sampler.cu", "optimizer.cu", "block_staged.cu", "slice_norm.cu", "api.cu"]
 HEADERS = ["graph.h", "kernels.cuh", "triple_rows.cuh", "dist_tile.cuh", os.path.join("..", "..", "include", "rgcn_b200.h")]
 
 

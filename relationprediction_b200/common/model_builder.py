@@ -7,12 +7,13 @@ BasisGcn; SkipConnections=Highway wraps every
 feature-input layer in a HighwayLayer), `embedding`, and the variational encoders `variational_embedding` and
 `variational_gcn_basis` (a VariationalEncoding over two linear AffineTransform heads); decoders `bilinear-diag`, `complex`,
 `rotate` (RotatE, which the reference does not have), `transe` (TransE, L1 distance; nor this), `quate` (QuatE,
-quaternion rotations; nor this, with all three training objectives) and `conve` (ConvE, 1-N training only).  Unknown
-names return None exactly
+quaternion rotations; nor this, with all three training objectives), `hole` (HolE, circular correlation; nor this, with
+all three training objectives) and `conve` (ConvE, 1-N training only).  Unknown names return None exactly
 like the reference (:270, :320); ablation flags that select out-of-scope variants raise."""
 from ..decoders.bilinear_diag import BilinearDiag, parse_training_objective
 from ..decoders.complex import Complex
 from ..decoders.conve import ConvE
+from ..decoders.hole import HolE
 from ..decoders.quate import QuatE
 from ..decoders.rotate import Rotate
 from ..decoders.transe import TransE
@@ -209,6 +210,9 @@ def build_decoder(encoder, decoder_settings):
         # linear in each row, as DistMult: all three objectives (NegativeSampling, SelfAdversarial, 1-N) on the same
         # scoring GEMMs; BilinearDiag.parse_settings checks the objective keys
         return QuatE(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
+    if decoder_settings['Name'] == "hole":
+        # linear in each row once in its Fourier basis: all three objectives on the same scoring GEMMs, as QuatE
+        return HolE(int(decoder_settings['CodeDimension']), decoder_settings, next_component=encoder)
     if decoder_settings['Name'] not in ("bilinear-diag", "complex"):
         objective = parse_training_objective(decoder_settings)[0]
         # RotatE and TransE train under SelfAdversarial (the objective of the RotatE paper) but have no 1-N scoring GEMM

@@ -3318,3 +3318,173 @@ extern "C" int rgcn_quate_query_rows(const float* codes, const float* rel, int32
   if (rc) return rc;
   return launch_quate_rank_prepare(codes, rel, d, X, n, side, Q, nullptr, nullptr, (cudaStream_t)stream);
 }
+
+// ------------------------------------------------------------------------------------------------
+// HolE (hole.cu): the real Fourier basis and its transforms, and the QuatE-shaped surface over transformed tables:
+// scorer, backward, self-adversarial forward, and the DistMult scoring GEMMs behind HolE's query rows (entity and
+// relation ranks and top-k, 1-N training, the query rows of the score matrices).  Every argument is checked before any
+// device work.
+// ------------------------------------------------------------------------------------------------
+extern "C" int64_t rgcn_hole_transform_workspace_bytes(int32_t d) {
+  if (d <= 0 || d % 4 != 0) {
+    rgcn_set_error("rgcn_hole_transform_workspace_bytes: bad arguments (need d > 0, d % 4 == 0)");
+    return RGCN_ERR_INVALID;
+  }
+  return align_up(2 * (int64_t)d * d * 4);   // the hi / lo split of U (gemm_any)
+}
+
+// out = x U (inverse = 0) or x U^T (inverse = 1), one 3xTF32 GEMM; U is built into `basis` first unless basis_ready.
+extern "C" int rgcn_hole_transform(const float* x, int64_t rows, int32_t d, int inverse, float* basis, int basis_ready,
+                                   float* out, void* workspace, int64_t workspace_bytes, void* stream) {
+  const std::string who = "rgcn_hole_transform";
+  if (!basis || !workspace || (rows > 0 && (!x || !out))) {
+    rgcn_set_error(who + ": null pointer");
+    return RGCN_ERR_INVALID;
+  }
+  if (d <= 0 || d % 4 != 0 || rows < 0 || rows > 0x7fffffffLL || (inverse != 0 && inverse != 1) ||
+      (rows > 0 && x == out)) {
+    rgcn_set_error(who + ": bad arguments (need d > 0, d % 4 == 0, 0 <= rows < 2^31, inverse in {0,1}, out != x)");
+    return RGCN_ERR_INVALID;
+  }
+  if (workspace_bytes < rgcn_hole_transform_workspace_bytes(d)) {
+    rgcn_set_error(who + ": workspace too small");
+    return RGCN_ERR_WORKSPACE;
+  }
+  int rc = onen_device_checks(who.c_str());
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!basis_ready) rc = launch_hole_basis(d, basis, st);
+  if (rc) return rc;
+  return gemm_any(st, (float*)workspace, false, inverse != 0, rows, d, d, x, d, basis, d, 0.f, out, d);
+}
+
+extern "C" int rgcn_hole_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                 const int32_t* X, int64_t N, const float* Y, float* energies, float* loss_out,
+                                 void* stream) {
+  const int rc = quate_checks("rgcn_hole_forward", codes && rel && loss_out && (N <= 0 || (X && energies)), V, Vrel,
+                              d, N);
+  if (rc) return rc;
+  return launch_hole_forward(codes, rel, d, X, N, Y, energies, loss_out, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_hole_backward(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                  const int32_t* X, int64_t N, const float* Y, const float* energies, float g_loss,
+                                  float g_reg, const float* g_scale_dev, const float* g_energy, float* dcodes,
+                                  float* drel, float* rel_slice_sumsq, void* stream) {
+  const int rc = quate_checks("rgcn_hole_backward",
+                              codes && rel && dcodes && drel && (N <= 0 || X) && (!Y || energies), V, Vrel, d, N);
+  if (rc) return rc;
+  return launch_hole_backward(codes, rel, d, X, N, Y, energies, g_loss, g_reg, g_scale_dev, g_energy, dcodes, drel,
+                              rel_slice_sumsq, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_hole_self_adversarial_forward(const float* codes, const float* rel, int32_t V, int32_t Vrel,
+                                                  int32_t d, const int32_t* X, int64_t N, int32_t K, float alpha,
+                                                  float* energies, float* coef, float* loss_out, void* workspace,
+                                                  int64_t workspace_bytes, void* stream) {
+  const std::string who = "rgcn_hole_self_adversarial_forward";
+  const int rc = self_adversarial_checks(
+      who, codes && rel && loss_out && workspace && (N <= 0 || (X && energies && coef)), V, Vrel, d, N, K, alpha,
+      workspace_bytes);
+  if (rc) return rc;
+  Carver ws(workspace, workspace_bytes);
+  float* parts = ws.take<float>(2 * (N / ((int64_t)K + 1)));
+  return launch_self_adversarial_forward(SELFADV_HOLE, codes, rel, d, X, N, K, alpha, 0.f, energies, coef, loss_out,
+                                         parts, (cudaStream_t)stream);
+}
+
+// Entity queries: rank_with_queries / topk_with_queries with HolE's query rows, in the DistMult workspaces
+// (distmult_rank_workspace_bytes, rgcn_topk_workspace_bytes), whose split of the codes is reused alike.
+extern "C" int rgcn_hole_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                              const int32_t* X, int64_t n, int side, const uint32_t* known_mask, int reuse_split,
+                              int32_t* raw_rank, int32_t* filtered_rank, void* workspace, int64_t workspace_bytes,
+                              void* stream) {
+  return rank_with_queries("rgcn_hole_rank", launch_hole_rank_prepare, codes, V, distmult_rank_workspace_bytes, codes,
+                           rel, V, Vrel, d, X, n, side, known_mask, reuse_split, raw_rank, filtered_rank, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_hole_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                              const int32_t* X, int64_t n, int side, int32_t k, const uint32_t* exclude_mask,
+                              int reuse_split, int32_t* ids, float* energies, void* workspace, int64_t workspace_bytes,
+                              void* stream) {
+  return topk_with_queries("rgcn_hole_topk", launch_hole_rank_prepare, codes, V, rgcn_topk_workspace_bytes, codes, rel,
+                           V, Vrel, d, X, n, side, k, exclude_mask, reuse_split, ids, energies, workspace,
+                           workspace_bytes, (cudaStream_t)stream);
+}
+
+// Relation queries: the candidates are the transformed rel[0:R] themselves, so these are distmult_relation_rank /
+// _topk with HolE's pair query rows, in the same workspaces (rgcn_relation_rank_workspace_bytes,
+// rgcn_relation_topk_workspace_bytes).
+static int hole_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int,
+                                 float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st) {
+  return launch_hole_relation_prepare(codes, rel, d, X, n, Q, gold_sig, gold_col, st);
+}
+
+extern "C" int rgcn_hole_relation_rank(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                       int32_t d, const int32_t* X, int64_t n, const uint32_t* known_mask,
+                                       int reuse_split, int32_t* raw_rank, int32_t* filtered_rank, void* workspace,
+                                       int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_hole_relation_rank";
+  if (!relation_count_ok(who, R, Vrel)) return RGCN_ERR_INVALID;
+  return rank_with_queries(who, hole_relation_prepare, rel, R, rgcn_relation_rank_workspace_bytes, codes, rel, V, Vrel,
+                           d, X, n, 0, known_mask, reuse_split, raw_rank, filtered_rank, workspace, workspace_bytes,
+                           (cudaStream_t)stream);
+}
+
+extern "C" int rgcn_hole_relation_topk(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R,
+                                       int32_t d, const int32_t* X, int64_t n, int32_t k, const uint32_t* exclude_mask,
+                                       int reuse_split, int32_t* ids, float* energies, void* workspace,
+                                       int64_t workspace_bytes, void* stream) {
+  const char* who = "rgcn_hole_relation_topk";
+  if (!relation_count_ok(who, R, Vrel)) return RGCN_ERR_INVALID;
+  return topk_with_queries(who, hole_relation_prepare, rel, R, rgcn_relation_topk_workspace_bytes, codes, rel, V, Vrel,
+                           d, X, n, 0, k, exclude_mask, reuse_split, ids, energies, workspace, workspace_bytes,
+                           (cudaStream_t)stream);
+}
+
+// 1-N training: the one_to_n() body with HolE's query rows and query backward, one launch per side run in a chunk.
+// The workspace is rgcn_one_to_n_workspace_bytes, and the backward of a call made with g_scale = (1, 0) is
+// rgcn_one_to_n_finish: the L2 term is DistMult's.
+extern "C" int rgcn_hole_one_to_n(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t R, int32_t d,
+                                  const int32_t* queries, int64_t n, const uint32_t* labels, float smoothing,
+                                  const float* g_scale, float* loss, float* dcodes, float* drel, int64_t chunk,
+                                  void* workspace, int64_t workspace_bytes, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const OnenStep prepare = [=](const OnenChunk& k, float* Q) {
+    int rc = RGCN_OK;
+    for (const OnenRun& run : *k.runs) {
+      const int64_t b = std::max(run.begin, k.c0), e = std::min(run.end, k.c1);
+      if (!rc && b < e)
+        rc = launch_hole_rank_prepare(codes, rel, d, k.X + 3 * b, e - b, run.side, Q + (b - k.c0) * d, nullptr,
+                                      nullptr, st);
+    }
+    return rc;
+  };
+  const OnenStep query_bwd = [=](const OnenChunk& k, float* dQ) {
+    int rc = RGCN_OK;
+    for (const OnenRun& run : *k.runs) {
+      const int64_t b = std::max(run.begin, k.c0), e = std::min(run.end, k.c1);
+      if (!rc && b < e)
+        rc = launch_hole_query_bwd(codes, rel, d, k.X + 3 * b, e - b, run.side, dQ + (b - k.c0) * d, g_scale,
+                                   k.c_reg, dcodes, drel, st);
+    }
+    return rc;
+  };
+  return one_to_n("rgcn_hole_one_to_n", prepare, query_bwd, false, codes, rel, V, Vrel, R, d, queries, n, labels,
+                  smoothing, g_scale, loss, dcodes, drel, chunk, workspace, workspace_bytes, st);
+}
+
+// The query rows Q [n, d] of the triples X for one side (the rows the entity ranks score), for the [n, V] score
+// matrices.
+extern "C" int rgcn_hole_query_rows(const float* codes, const float* rel, int32_t V, int32_t Vrel, int32_t d,
+                                    const int32_t* X, int64_t n, int side, float* Q, void* stream) {
+  const std::string who = "rgcn_hole_query_rows";
+  if (side != 0 && side != 1) {
+    rgcn_set_error(who + ": bad arguments (side in {0,1})");
+    return RGCN_ERR_INVALID;
+  }
+  const int rc = quate_checks(who, codes && rel && (n <= 0 || (X && Q)), V, Vrel, d, n);
+  if (rc) return rc;
+  return launch_hole_rank_prepare(codes, rel, d, X, n, side, Q, nullptr, nullptr, (cudaStream_t)stream);
+}

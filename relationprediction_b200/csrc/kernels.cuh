@@ -325,7 +325,8 @@ int launch_complex_relation_prepare(const float* codes, const float* rel, int d,
 // the SELFADV_* kinds; gamma is read by RotatE and TransE only): energies [N], the energy-gradient coefficients coef [N],
 // loss_out[0] the loss, loss_out[1] the decoder's L2 term of its NegativeSampling forward; parts: 2n floats of scratch
 // for the per-group loss and norm parts
-enum { SELFADV_DISTMULT = 0, SELFADV_COMPLEX = 1, SELFADV_ROTATE = 2, SELFADV_TRANSE = 3, SELFADV_QUATE = 4 };
+enum { SELFADV_DISTMULT = 0, SELFADV_COMPLEX = 1, SELFADV_ROTATE = 2, SELFADV_TRANSE = 3, SELFADV_QUATE = 4,
+       SELFADV_HOLE = 5 };
 int launch_self_adversarial_forward(int decoder, const float* codes, const float* rel, int d, const int32_t* X,
                                     int64_t N, int K, float alpha, float gamma, float* energies, float* coef,
                                     float* loss_out, float* parts, cudaStream_t st);
@@ -391,6 +392,26 @@ int launch_quate_relation_prepare(const float* codes, const float* rel, int d, c
 int launch_quate_query_bwd(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
                            const float* dQ, const float* g_scale, float c_reg, float* dcodes, float* drel,
                            cudaStream_t st);
+
+// hole.cu -- HolE (DESIGN.md section 1) on rows in the real Fourier basis x~ = x U.  U [d, d] (d % 4 == 0) into a
+// device buffer:
+int launch_hole_basis(int d, float* U, cudaStream_t st);
+// Scorer and backward over transformed rows: the contracts of the DistMult launchers.
+int launch_hole_forward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                        float* energies, float* loss_out, cudaStream_t st);
+int launch_hole_backward(const float* codes, const float* rel, int d, const int32_t* X, int64_t N, const float* Y,
+                         const float* energies, float g_loss, float g_reg, const float* g_scale_dev,
+                         const float* g_energy, float* dcodes, float* drel, float* rel_slice_sumsq, cudaStream_t st);
+// entity query rows in launch_distmult_rank_prepare's contract: side 1 Q = w (h r), side 0 Q = w conj(r) t
+int launch_hole_rank_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
+                             float* Q, float* gold_sig, int32_t* gold_col, cudaStream_t st);
+// pair query rows in launch_distmult_relation_prepare's contract: Q = w conj(h) t
+int launch_hole_relation_prepare(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, float* Q,
+                                 float* gold_sig, int32_t* gold_col, cudaStream_t st);
+// 1-N query backward in launch_onen_query_bwd's contract (dQ is never null)
+int launch_hole_query_bwd(const float* codes, const float* rel, int d, const int32_t* X, int64_t n, int side,
+                          const float* dQ, const float* g_scale, float c_reg, float* dcodes, float* drel,
+                          cudaStream_t st);
 
 // conve.cu -- the ConvE query network (DESIGN.md section 1): d = h w, image 2h x w, C filters 3x3, F = C (2h-2)(w-2)
 // feature columns stored with leading dimension Fp (F rounded up to 4).  Masks are uint8 keep-masks or null.

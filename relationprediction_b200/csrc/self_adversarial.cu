@@ -1,5 +1,5 @@
 // self_adversarial.cu -- self-adversarial negative sampling (Sun et al., RotatE, ICLR 2019) for the DistMult, ComplEx,
-// RotatE, TransE and QuatE decoders, sm_90a: the forward of the objective, which also writes each triple's energy
+// RotatE, TransE, QuatE and HolE decoders, sm_90a: the forward of the objective, which also writes each triple's energy
 // gradient.
 //
 // The fed triples follow the negative sampler's layout (auxilliaries.py:13-33): for N = n (K + 1) rows, rows 0..n-1
@@ -112,6 +112,9 @@ int launch_self_adversarial_forward(int decoder, const float* codes, const float
   else if (decoder == SELFADV_QUATE)
     k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
                                           QuatERows{});
+  else if (decoder == SELFADV_HOLE)
+    k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
+                                          HolERows{});
   else if (decoder == SELFADV_TRANSE)
     k_selfadv_fwd<<<blocks, 256, 0, st>>>(codes, rel, d, X, n, K, alpha, inv_2n, energies, coef, loss_part, reg_part,
                                           TransERows<4>{gamma});

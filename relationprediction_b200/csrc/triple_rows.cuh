@@ -1,6 +1,7 @@
-// triple_rows.cuh -- the row arithmetic of the DistMult, ComplEx, RotatE, TransE and QuatE triple scorers: one warp
-// owns one triple (s, r, o) and each lane forms its share of the energy and of the squared norms of the gathered rows.
-// Shared by the NegativeSampling scorers (distmult.cu / complex.cu / rotate.cu / transe.cu / quate.cu) and the
+// triple_rows.cuh -- the row arithmetic of the DistMult, ComplEx, RotatE, TransE, QuatE and HolE triple scorers: one
+// warp owns one triple (s, r, o) and each lane forms its share of the energy and of the squared norms of the gathered
+// rows.  Shared by the NegativeSampling scorers (distmult.cu / complex.cu / rotate.cu / transe.cu / quate.cu / hole.cu)
+// and the
 // self-adversarial scorer (self_adversarial.cu), so both objectives score a triple with the same float operations in
 // the same order.
 #pragma once
@@ -218,6 +219,56 @@ struct QuatERows {
       const float4 a = __ldg(e1 + i), b = __ldg(rr + i), c = __ldg(e2 + i);
       float m;
       e = quat_dot(quat_mul(a, quat_normalize(b, m)), c, e);
+      q += a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
+      q += b.x * b.x + b.y * b.y + b.z * b.z + b.w * b.w;
+      q += c.x * c.x + c.y * c.y + c.z * c.z + c.w * c.w;
+    }
+  }
+};
+
+// HolE (DESIGN.md section 1) on rows already in the real Fourier basis x~ = x U.  Float4 i of a row holds columns
+// 4i..4i+3.  For i > 0 those are two frequencies, (re, im) pairs.  Float4 0 (lane 0's first) holds DC and Nyquist, two
+// real columns, then frequency 1.  With the weights w0 = sqrt(d) (DC, Nyquist) and w1 = sqrt(d / 2) (every pair):
+//   E = sum over the columns of  w * Re(conj(h r) t),  DC and Nyquist taken as real numbers.
+// Every HolE kernel -- scorer, backward, self-adversarial scorer, query rows, query backward -- forms its products with
+// these helpers, so they all use the same float operations.
+__device__ __forceinline__ void hole_weights(int d, float& w0, float& w1) {
+  w0 = __fsqrt_rn((float)d);
+  w1 = __fsqrt_rn(0.5f * (float)d);
+}
+
+// w (a b) for float4 i of two rows; first = (i == 0): x and y are then the real DC and Nyquist columns
+__device__ __forceinline__ float4 hole_mul(float4 a, float4 b, bool first, float w0, float w1) {
+  const float x = first ? w0 * (a.x * b.x) : w1 * fmaf(a.x, b.x, -(a.y * b.y));
+  const float y = first ? w0 * (a.y * b.y) : w1 * fmaf(a.x, b.y, a.y * b.x);
+  return make_float4(x, y, w1 * fmaf(a.z, b.z, -(a.w * b.w)), w1 * fmaf(a.z, b.w, a.w * b.z));
+}
+
+// w conj(a) b for float4 i of two rows (DC and Nyquist are real: conj leaves them alone)
+__device__ __forceinline__ float4 hole_cmul(float4 a, float4 b, bool first, float w0, float w1) {
+  const float x = first ? w0 * (a.x * b.x) : w1 * fmaf(a.x, b.x, a.y * b.y);
+  const float y = first ? w0 * (a.y * b.y) : w1 * fmaf(a.x, b.y, -(a.y * b.x));
+  return make_float4(x, y, w1 * fmaf(a.z, b.z, a.w * b.w), w1 * fmaf(a.z, b.w, -(a.w * b.z)));
+}
+
+__device__ __forceinline__ float hole_dot(float4 p, float4 q, float acc) {
+  return fmaf(p.w, q.w, fmaf(p.z, q.z, fmaf(p.y, q.y, fmaf(p.x, q.x, acc))));
+}
+
+// HolE: e = <w (h r), t> over the transformed rows; a lane owns whole float4s (d % 4 == 0).  q gets the squared norms of
+// the three rows: U is orthogonal, so that is DistMult's L2 term of the raw rows.
+struct HolERows {
+  __device__ __forceinline__ static void partial(const float* __restrict__ codes, const float* __restrict__ rel, int d,
+                                                 int s, int r, int o, int lane, float& e, float& q) {
+    const float4* e1 = reinterpret_cast<const float4*>(codes + (size_t)s * d);
+    const float4* rr = reinterpret_cast<const float4*>(rel + (size_t)r * d);
+    const float4* e2 = reinterpret_cast<const float4*>(codes + (size_t)o * d);
+    const int d4 = d >> 2;
+    float w0, w1;
+    hole_weights(d, w0, w1);
+    for (int i = lane; i < d4; i += 32) {
+      const float4 a = __ldg(e1 + i), b = __ldg(rr + i), c = __ldg(e2 + i);
+      e = hole_dot(hole_mul(a, b, i == 0, w0, w1), c, e);
       q += a.x * a.x + a.y * a.y + a.z * a.z + a.w * a.w;
       q += b.x * b.x + b.y * b.y + b.z * b.z + b.w * b.w;
       q += c.x * c.x + c.y * c.y + c.z * c.z + c.w * c.w;

@@ -85,7 +85,7 @@ class BilinearDiag(Model):
         """One fused kernel: three row gathers -> energies (+ sigmoid-CE loss and L2 term in train
         mode).  The gathered e1/r/e2 rows of compute_codes are never materialised."""
         if self._scored[mode] is None:
-            subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode=mode)
+            subject_codes, relation_codes, object_codes = self._all_codes(mode)
             assert subject_codes is object_codes, "DistMult kernel expects one shared entity code matrix"
             Y = None
             if mode == 'train':
@@ -93,6 +93,10 @@ class BilinearDiag(Model):
             self._scored[mode] = self._score_op()(subject_codes.contiguous(), relation_codes.contiguous(),
                                                   self._x_device(), Y)
         return self._scored[mode]
+
+    def _all_codes(self, mode):
+        """(subject, relation, object) code tables the decoder scores: the encoder's (HolE transforms them)"""
+        return self.next_component.get_all_codes(mode=mode)
 
     def _score_op(self):
         return ops.distmult
@@ -104,7 +108,7 @@ class BilinearDiag(Model):
         """(e1s, rs, e2s) row gathers (bilinear_diag.py:14-24) -- only the all-entity scoring GEMMs
         below need them explicitly."""
         if self.encoder_cache[mode] is None:
-            subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode=mode)
+            subject_codes, relation_codes, object_codes = self._all_codes(mode)
             X = self._x_device().long()
             self.encoder_cache[mode] = (subject_codes[X[:, 0]], relation_codes[X[:, 1]], object_codes[X[:, 2]])
         return self.encoder_cache[mode]
@@ -115,7 +119,7 @@ class BilinearDiag(Model):
         if self._one_to_n_loss is None:
             if self.one_to_n_labels is None:
                 raise RuntimeError("TrainingObjective=1-N needs the training labels: call set_one_to_n_labels first")
-            subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='train')
+            subject_codes, relation_codes, object_codes = self._all_codes('train')
             assert subject_codes is object_codes, "1-N training expects one shared entity code matrix"
             # the queries and label rows of a fed array are kept while the same array is fed again: without a graph
             # batch the driver feeds the whole training split every step
@@ -135,7 +139,7 @@ class BilinearDiag(Model):
         """(loss, reg, energies) of self-adversarial negative sampling over the fed X in the sampler's layout (n
         positives, then NegativeSampleRate blocks of their corruptions); Y is not read (ops.self_adversarial_loss)."""
         if self._self_adversarial_loss is None:
-            subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='train')
+            subject_codes, relation_codes, object_codes = self._all_codes('train')
             assert subject_codes is object_codes, "self-adversarial training expects one shared entity code matrix"
             self._self_adversarial_loss = ops.self_adversarial_loss(
                 subject_codes.contiguous(), relation_codes.contiguous(), self._x_device(), self.negative_sample_rate,
@@ -192,7 +196,7 @@ class BilinearDiag(Model):
         predict_all_subject_scores / predict_all_object_scores (bilinear_diag.py:51-61): the encoder runs once,
         the scoring GEMM counts `score >= gold` in its epilogue.  Returns four int arrays
         (raw_subjects, filtered_subjects, raw_objects, filtered_objects)."""
-        subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='test')
+        subject_codes, relation_codes, object_codes = self._all_codes('test')
         assert subject_codes is object_codes, "DistMult ranking expects one shared entity code matrix"
         codes, rel = subject_codes.contiguous(), relation_codes.contiguous()
         ranker = self._ranker(codes, rel)
@@ -215,7 +219,7 @@ class BilinearDiag(Model):
         scoring GEMM keeps each row's best k in its epilogue.  exclude_lists[t] lists the entities row t may not
         return (or None: none excluded).  Returns (ids int64 [n, k], energies float32 [n, k]); energy descending,
         the smaller id first on ties; rows with fewer than k eligible entities end in (-1, -inf)."""
-        subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='test')
+        subject_codes, relation_codes, object_codes = self._all_codes('test')
         assert subject_codes is object_codes, "fused top-k prediction expects one shared entity code matrix"
         codes, rel = subject_codes.contiguous(), relation_codes.contiguous()
         ranker = self._ranker(codes, rel)
@@ -237,7 +241,7 @@ class BilinearDiag(Model):
     def test_ranker(self):
         """The decoder's fused ranker (ops.DistMultRanker / ops.ComplexRanker) over the test-mode codes of the fed
         inputs: one encoder pass.  The ensemble ranker (ops.EnsembleRanker) combines two of these."""
-        subject_codes, relation_codes, object_codes = self.next_component.get_all_codes(mode='test')
+        subject_codes, relation_codes, object_codes = self._all_codes('test')
         assert subject_codes is object_codes, "fused ranking expects one shared entity code matrix"
         return self._ranker(subject_codes.contiguous(), relation_codes.contiguous())
 

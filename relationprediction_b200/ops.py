@@ -176,6 +176,8 @@ def set_slice_norms(enabled):
 
 
 def _add_slice_sumsq(param, value):
+    # a table made by an orthogonal transform (hole_transform) has the slice norms of the table it was made from
+    param = getattr(param, "_slice_source", param)
     prev = getattr(param, "_slice_sumsq", None)
     param._slice_sumsq = value if prev is None else prev + value
 
@@ -770,13 +772,83 @@ def quate_score(codes, rel, X, Y=None):
     return _QuatEFn.apply(codes, rel, X, Y)
 
 
+# ---- HolE (rgcn_hole_*, include/rgcn_b200.h): the real Fourier basis and the scorer over transformed tables ----
+_HOLE_BASES = {}   # (device, d) -> U [d, d]
+
+
+def hole_basis(d, device):
+    """The HolE basis U [d, d] (float32 CUDA, built once per (device, d) by rgcn_hole_transform): the orthonormal real
+    DFT basis with columns DC, Nyquist, then (cos, -sin) pairs of frequencies 1 .. d/2 - 1."""
+    device = torch.device(device)
+    key = (device, int(d))
+    U = _HOLE_BASES.get(key)
+    if U is None:
+        U = torch.empty((d, d), dtype=torch.float32, device=device)
+        _call("rgcn_hole_transform", "rgcn_hole_transform_workspace_bytes", (d,),
+              (None, 0, d, 0, _ptr(U), 0, None), device)
+        _HOLE_BASES[key] = U
+    return U
+
+
+def _hole_apply(x, inverse):
+    """x U (inverse False) or x U^T (inverse True) of a CUDA float32 [rows, d] tensor, one library GEMM"""
+    _check_cuda_f32("rows to transform", x)
+    rows, d = x.shape
+    U = hole_basis(d, x.device)
+    out = torch.empty_like(x)
+    _call("rgcn_hole_transform", "rgcn_hole_transform_workspace_bytes", (d,),
+          (_ptr(x), rows, d, int(inverse), _ptr(U), 1, _ptr(out)), x.device)
+    return out
+
+
+class _HolETransformFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, inverse):
+        ctx.inverse = inverse
+        return _hole_apply(x, inverse)
+
+    @staticmethod
+    def backward(ctx, g):
+        return _hole_apply(g.contiguous(), not ctx.inverse), None
+
+
+def hole_transform(x, inverse=False):
+    """The rows of x [rows, d] (CUDA float32, d % 4 == 0) in the HolE basis, x U (inverse=True: x U^T, which takes
+    them back).  Differentiable: the backward is g U^T (g U).  The result carries the slice norms the HolE backward
+    passes leave on it over to x, or to the table x is a row range of, for optim.ClippedAdam: U is orthogonal, so
+    they are x's own."""
+    out = _HolETransformFn.apply(x, bool(inverse))
+    out._slice_source = getattr(x, "_slice_source", x if x._base is None else x._base)
+    return out
+
+
+class _HolEFn(torch.autograd.Function):
+    """Returns (energies[N], loss, reg) of the HolE scorer over transformed tables, same conventions as _DistMultFn."""
+
+    @staticmethod
+    def forward(ctx, codes, rel, X, Y):
+        return _triple_forward(ctx, "rgcn_hole_forward", codes, rel, X, Y)
+
+    @staticmethod
+    def backward(ctx, g_energy, g_loss, g_reg):
+        return _triple_backward(ctx, "rgcn_hole_backward", g_energy, g_loss, g_reg)
+
+
+def hole_score(codes, rel, X, Y=None):
+    """HolE energies sum_k r_k [h * t]_k (circular correlation) of tables already in the HolE basis (hole_transform),
+    the mean sigmoid cross-entropy (0 if Y is None) and DistMult's L2 term mean(h^2) + mean(r^2) + mean(t^2) of the
+    gathered rows, which the orthogonal basis leaves unchanged (include/rgcn_b200.h, rgcn_hole_forward)."""
+    return _HolEFn.apply(codes, rel, X, Y)
+
+
 # decoder -> (the decoder kind of rgcn_self_adversarial_forward, or the name of the decoder's own entry point, which
 # takes the margin gamma if the decoder is one of MARGIN_DECODERS; the scorer's backward)
 SELF_ADVERSARIAL_DECODERS = {"distmult": (_lib.RGCN_DECODER_DISTMULT, "distmult_backward_slices"),
                              "complex": (_lib.RGCN_DECODER_COMPLEX, "rgcn_complex_backward"),
                              "rotate": ("rgcn_rotate_self_adversarial_forward", "rgcn_rotate_backward"),
                              "transe": ("rgcn_transe_self_adversarial_forward", "rgcn_transe_backward"),
-                             "quate": ("rgcn_quate_self_adversarial_forward", "rgcn_quate_backward")}
+                             "quate": ("rgcn_quate_self_adversarial_forward", "rgcn_quate_backward"),
+                             "hole": ("rgcn_hole_self_adversarial_forward", "rgcn_hole_backward")}
 # the decoders whose energy carries the margin gamma
 MARGIN_DECODERS = ("rotate", "transe")
 
@@ -840,8 +912,8 @@ def self_adversarial_loss(codes, rel, X, K, alpha, decoder, *, gamma=None):
     the negative sampler's layout: rows 0..n-1 the positives, row i + n j (j = 1..K) the j-th corruption of positive i,
     N = n (K + 1).  Returns (loss, reg, energies): loss = 1/(2n) sum_i [softplus(-s_i) + sum_j p_ij softplus(s_ij)] with
     p_ij = softmax_j(alpha s_ij) held constant, reg = the decoder's L2 term over all N triples, energies [N].
-    decoder is "distmult", "complex", "rotate", "transe" or "quate"; gamma is the margin, needed by "rotate" and
-    "transe" only.
+    decoder is "distmult", "complex", "rotate", "transe", "quate" or "hole" (on tables in the HolE basis); gamma is the
+    margin, needed by "rotate" and "transe" only.
     Differentiable in codes and rel."""
     if decoder not in SELF_ADVERSARIAL_DECODERS:
         raise ValueError("self_adversarial_loss: decoder must be one of %s, got %r"
@@ -1155,6 +1227,46 @@ def quate_query_rows(codes, rel, X, side):
     return Q
 
 
+class HolERanker(object):
+    """Fused all-entity and all-relation ranking and top-k of the HolE decoder (rgcn_hole_rank / _topk /
+    _relation_rank / _relation_topk) over tables in the HolE basis (hole_transform): DistMultRanker's interface,
+    workspaces and split reuse, with HolE's query rows (side 1 w (h r), side 0 w conj(r) t, relation pairs
+    w conj(h) t against rel[0:R]).  Not a DistMultRanker: it is no member of the fused ensemble, whose kernels score
+    DistMult and ComplEx rows only."""
+    _RANK, _WORKSPACE, _TOPK = "rgcn_hole_rank", "distmult_rank_workspace_bytes", "rgcn_hole_topk"
+    _REL_RANK, _REL_TOPK = "rgcn_hole_relation_rank", "rgcn_hole_relation_topk"
+    _REL_RANK_WORKSPACE = DistMultRanker._REL_RANK_WORKSPACE
+    _REL_TOPK_WORKSPACE = DistMultRanker._REL_TOPK_WORKSPACE
+    TOPK_CHUNK_BYTES = DistMultRanker.TOPK_CHUNK_BYTES
+
+    __init__ = DistMultRanker.__init__
+    _check_rows = DistMultRanker._check_rows
+    _chunk_rows = DistMultRanker._chunk_rows
+    _relation_calls = DistMultRanker._relation_calls
+    rank = DistMultRanker.rank
+    top_k = DistMultRanker.top_k
+    rank_relations = DistMultRanker.rank_relations
+    top_k_relations = DistMultRanker.top_k_relations
+
+
+def hole_query_rows(codes, rel, X, side):
+    """HolE query rows Q [n, d] of the triples X (int32 [n, 3] CUDA) over tables in the HolE basis: side 1 w (h r)
+    (scored against the objects), side 0 w conj(r) t (against the subjects); <Q[t], codes[v]> is the energy of the
+    triple with v in the predicted column (rgcn_hole_query_rows)."""
+    _check_cuda_f32("codes", codes)
+    _check_cuda_f32("relation table", rel)
+    if not (X.is_cuda and X.dtype == torch.int32 and X.is_contiguous() and X.dim() == 2 and X.shape[1] == 3):
+        raise _lib.RgcnError("X must be a contiguous CUDA int32 [n,3] tensor")
+    V, d = codes.shape
+    n = X.shape[0]
+    Q = torch.empty((n, d), dtype=torch.float32, device=codes.device)
+    lib = _lib.load()
+    rc = lib.rgcn_hole_query_rows(_ptr(codes), _ptr(rel), V, rel.shape[0], d, _ptr(X), n, int(side), _ptr(Q),
+                                  _stream(codes.device))
+    _lib.check(rc, "rgcn_hole_query_rows")
+    return Q
+
+
 class RotateRanker(object):
     """All-entity ranking of the RotatE decoder by distance (rgcn_rotate_rank): rank(X, side, known_mask) as
     DistMultRanker.rank, with D_v = sum_k |q_k - v_k| <= D_gold in place of score >= gold score, so the ranks do not
@@ -1464,7 +1576,7 @@ class EnsembleRanker(object):
 
 # ---- 1-N training (distmult_one_to_n / rgcn_complex_one_to_n, include/rgcn_b200.h) ----
 ONE_TO_N_DECODERS = {"distmult": "distmult_one_to_n", "complex": "rgcn_complex_one_to_n",
-                     "quate": "rgcn_quate_one_to_n"}
+                     "quate": "rgcn_quate_one_to_n", "hole": "rgcn_hole_one_to_n"}
 # device bytes of the per-query buffers (energy gradients Gt [V, chunk], query rows and their gradients) of one
 # internal pass; more queries than fit run in several passes of one call
 ONE_TO_N_CHUNK_BYTES = 1 << 30
@@ -1533,9 +1645,10 @@ class OneToNLabels(object):
 
 
 class _OneToNFn(torch.autograd.Function):
-    """Returns (loss, reg) of distmult_one_to_n / rgcn_complex_one_to_n / rgcn_quate_one_to_n.  When codes or rel
-    need a gradient, the forward also writes the gradient of the loss alone (g_scale = (1, 0)); the gradient is linear
-    in the two upstream scalars, so the backward is rgcn_one_to_n_finish: one scaling pass and the L2 term, no GEMM."""
+    """Returns (loss, reg) of distmult_one_to_n / rgcn_complex_one_to_n / rgcn_quate_one_to_n / rgcn_hole_one_to_n.
+    When codes or rel need a gradient, the forward also writes the gradient of the loss alone (g_scale = (1, 0)); the
+    gradient is linear in the two upstream scalars, so the backward is rgcn_one_to_n_finish: one scaling pass and the
+    L2 term, no GEMM."""
 
     @staticmethod
     def forward(ctx, codes, rel, labels, queries, smoothing, entry, R, chunk, grads):
@@ -1575,8 +1688,9 @@ def one_to_n_loss(codes, rel, queries, labels, smoothing, decoder, relation_coun
     """1-N loss of host queries (anchor, relation, side) int32 [n, 3] against every entity, with the label bits of
     OneToNLabels.rows and label smoothing eps in [0, 1): returns (loss, reg), loss = the mean over the n V scores of the
     sigmoid cross-entropy against y' = (1 - eps) y + eps / V, reg = (|codes[anchor]|^2 + |rel[r]|^2) / (n d) summed
-    over the queries (the decoders' un-scaled L2 term).  decoder is "distmult", "complex" or "quate"; the relation ids
-    must be below relation_count (default: all rows of rel).  Differentiable in codes and rel."""
+    over the queries (the decoders' un-scaled L2 term).  decoder is "distmult", "complex", "quate" or "hole" (on tables
+    in the HolE basis); the relation ids must be below relation_count (default: all rows of rel).  Differentiable in
+    codes and rel."""
     if decoder not in ONE_TO_N_DECODERS:
         raise ValueError("one_to_n_loss: decoder must be one of %s, got %r" % (sorted(ONE_TO_N_DECODERS), decoder))
     _check_cuda_f32("codes", codes)
